@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — megapixels/s decoded (JPEG XL VarDCT d1.0) on N B200s; CPU baseline beside it.
+"""bench.py — megapixels/s decoded (JPEG XL VarDCT d1.0) on N H100s; CPU baseline beside it.
 
 A "step" is one pass of the decode hot path over one batch of independent frames per GPU
 (weak scaling: every rank decodes its own batch; there is no data-path collective — groups and
@@ -10,12 +10,17 @@ bytes in and planar f32 pixels copied back to pinned host memory every step.
   python bench.py --gpus 1 --steps 5 --warmup 3
   python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
   python bench.py --impl reference      # CPU arm: the oracle (port of jxl-oxide's generic path)
+  python bench.py ... --dump-outputs DIR  # also write the last timed step's decoded frames as DIR/<name>.npy
+
+The bench writes nothing into the source tree: the synthetic encoder and its frames are cached in a temporary directory.
 """
 import argparse
+import hashlib
 import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -34,20 +39,42 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 # ----------------------------------------------------------------------------------------------
 # workloads
-def synth_frame(w, h, seed, distance=1.0, extra=()):
-    """Synthetic encoded frame from tools/synth_enc.cc (built on demand; cached under bench_data/)."""
-    tool = os.path.join(ROOT, "tools", "_build_synth_enc")
-    src = os.path.join(ROOT, "tools", "synth_enc.cc")
+def _synth_cache():
+    """Per-user temporary directory for the encoder binary and its frames, keyed by the encoder's sources so that a
+    changed encoder never serves frames made by an older one (the source tree may be read-only)."""
     host = os.path.join(ROOT, "jxl_oxide_b200", "csrc", "host")
-    if not os.path.exists(tool) or os.path.getmtime(tool) < os.path.getmtime(src):
-        subprocess.check_call(["g++", "-std=c++17", "-O2", "-o", tool, src] +
+    srcs = [os.path.join(ROOT, "tools", "synth_enc.cc")] + sorted(os.path.join(host, f) for f in os.listdir(host))
+    digest = hashlib.sha256()
+    for p in srcs:
+        with open(p, "rb") as f:
+            digest.update(f.read())
+    d = os.path.join(tempfile.gettempdir(), f"jxlb_bench_{os.getuid()}", digest.hexdigest()[:16])
+    os.makedirs(d, exist_ok=True)
+    return d
+
+
+def synth_tool():
+    """Path of the built tools/synth_enc.cc (compiled on first use into the cache directory)."""
+    tool = os.path.join(_synth_cache(), "synth_enc")
+    if not os.path.exists(tool):
+        host = os.path.join(ROOT, "jxl_oxide_b200", "csrc", "host")
+        tmp = f"{tool}.{os.getpid()}"
+        subprocess.check_call(["g++", "-std=c++17", "-O2", "-o", tmp, os.path.join(ROOT, "tools", "synth_enc.cc")] +
                               [os.path.join(host, f) for f in ("entropy.cc", "frame_syntax.cc", "modular_syntax.cc", "headers.cc")])
-    os.makedirs(os.path.join(ROOT, "bench_data"), exist_ok=True)
+        os.replace(tmp, tool)
+    return tool
+
+
+def synth_frame(w, h, seed, distance=1.0, extra=()):
+    """Synthetic encoded frame from tools/synth_enc.cc (seeded, so the same arguments give the same bytes)."""
+    tool = synth_tool()
     tag = "".join(extra).replace("-", "")
-    path = os.path.join(ROOT, "bench_data", f"synth_{w}x{h}_d{distance}_s{seed}{tag}.jxl")
+    path = os.path.join(_synth_cache(), f"synth_{w}x{h}_d{distance}_s{seed}{tag}.jxl")
     if not os.path.exists(path):
+        tmp = f"{path}.{os.getpid()}"
         subprocess.check_call([tool, "--width", str(w), "--height", str(h), "--seed", str(seed), "--distance", str(distance),
-                               "-o", path] + list(extra), stderr=subprocess.DEVNULL)
+                               "-o", tmp] + list(extra), stderr=subprocess.DEVNULL)
+        os.replace(tmp, path)
     with open(path, "rb") as f:
         return f.read()
 
@@ -249,9 +276,9 @@ def gpu_local_cpus(device_index):
 
 
 # HF coefficient schedule of the timed run: fixed, never probed inside the bench. 128 = one THREAD per stream (32 streams per
-# warp): a frame's 510 streams then take 16 warps for ~42 ms instead of 510 one-lane warps for ~14 ms. With ~26 frames
-# in their heavy stage the one-lane form alone asks for more warp slots than the GPU has (26 x 510 > 148 x 64) and starves
-# the pixel kernels; measured whole-job (profiles/r02_progress.md section 6): 185-197 frames/s against 116-167.
+# warp): a frame's 510 streams then take 16 warps, slower per frame than 510 one-lane warps. With 16 frames in their
+# heavy stage the one-lane form alone asks for about every warp slot of the GPU (16 x 510 against 132 x 64 on an H100)
+# and starves the pixel kernels.
 # jxlb_decode (one frame, latency matters) keeps the 16-warp form.
 HF_STREAMS_PER_CTA = 128
 HF_LATENCY_SCHEDULE = 16
@@ -278,8 +305,10 @@ def run_ours(args, rank, world, local_rank):
     hf_lanes = int(env_knob) if env_knob is not None else (HF_STREAMS_PER_CTA if args.hf_lanes == "auto" else int(args.hf_lanes))
     desc, frames, (w, h) = load_workload(args.workload, args.frames_per_step)
     px_per_frame = w * h
-    workers = args.contexts or (64 if "mod" in args.workload else 96)
-    heavy = args.heavy_frames or 26  # + 6 batch streams = the device's 32 hardware queues
+    # Device memory grows with workers (LF arena + memory pool each) and heavy slots (~0.9 GB slab each at 8K): 64 workers
+    # with 16 heavy slots use 59.5 GB of an 80 GB H100, 96 workers do not fit
+    workers = args.contexts or 64
+    heavy = args.heavy_frames or (26 if "mod" in args.workload else 16)
     args.contexts, args.heavy_frames = workers, heavy
     pipe = J.Pipeline(local_rank, workers=workers, heavy_frames=heavy, hf_streams_per_cta=hf_lanes, batch_streams=args.batch_streams)
     # encoded frames resident in HBM ("inputs already resident"): one preloaded slot per distinct frame
@@ -355,6 +384,9 @@ def run_ours(args, rank, world, local_rank):
     ms = timed("value", args.steps)
     clocks = sampler.stop()
     launches = pipe.launch_count() - launches0
+    free_b, total_b = torch.cuda.mem_get_info(local_rank)  # the whole device: the library allocates outside torch
+    if args.dump_outputs and rank == 0:  # every rank decodes the same frames
+        dump_outputs(J, pipe, local_rank, frames, slots, args.dump_outputs)
     run_steps("e2e", 1)
     ms_e2e = timed("e2e", args.steps)
     run_steps("u8", 1)
@@ -405,6 +437,7 @@ def run_ours(args, rank, world, local_rank):
             d._L.jxlb_set_hf_streams_per_cta(d._h, hf_lanes)
 
     total_px = px_per_frame * len(frames) * world
+    pipe.close()  # the gather leg builds its own pipeline: two at once do not fit the device
     gather = None
     if args.gather != "none":
         gather = run_gather(args, torch, dist, J, local_rank, world, rank, frames, total_px, barrier, hf_lanes)
@@ -412,19 +445,13 @@ def run_ours(args, rank, world, local_rank):
     e2e_value = total_px / (ms_e2e / args.steps / 1e3) / 1e6
     e2e_u8_value = total_px / (ms_e2e_u8 / args.steps / 1e3) / 1e6
     u8_bytes = px_per_frame * 3
-    pipe.close()
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()
     if rank != 0:
         return
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    peak = peaks.get("hbm_gbs", 6650.0)
-    peak_source = "MEASURED_PEAKS.json hbm_gbs (burst copy bandwidth)" if peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    peak = 3350.0
+    peak_source = "H100 SXM data sheet HBM3 bandwidth (3.35 TB/s)"
     # The dominant HBM-bound work: the pixel chain coefficients -> RGB planes (SURVEY 8d: 24.3 B/px when fully fused).
     # One "launch" = the chain's kernels for one frame; duration = the sum of their CUDA-event times.
     modular = "mod" in args.workload
@@ -432,20 +459,13 @@ def run_ours(args, rank, world, local_rank):
     # Modular: 4 B/sample of decoded residuals read + 4 B/sample of f32 output written, three channels, when Squeeze, RCT
     # and the sample conversion are fully fused (SURVEY 8d)
     chain_bytes = px_per_frame * (24.0 if modular else 24.3)
-    traffic = None
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))
-        if tj.get("workload") == args.workload:
-            traffic = tj.get("chain_dram_bytes_per_frame")
-    except Exception:
-        pass
     roofline = None
     chain_solo_ms = sum(solo.get(k, 0.0) for k in chain)
     chain_load_ms = sum(prof[k]["ms"] for k in chain if k in prof) / max(1, len(frames))
     if chain_solo_ms > 0:
         ach = chain_bytes / (chain_solo_ms / 1e3) / 1e9
         roofline = {"kernel": "+".join(k for k in chain if k in solo), "bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s",
-                    "frac": ach / peak, "traffic": traffic, "peak_source": peak_source,
+                    "frac": ach / peak, "peak_source": peak_source,
                     "bytes_per_launch": chain_bytes, "avg_launch_ms": chain_solo_ms,
                     "per_kernel_ms": {k: round(solo[k], 4) for k in chain if k in solo},
                     "measured": "CUDA events around the chain's launches, one frame alone on the GPU (mean of 3)",
@@ -454,8 +474,9 @@ def run_ours(args, rank, world, local_rank):
                                            "for SMs held by other frames' kernels"},
                     "bound_note": None if modular else
                                   ("reported against the HBM roof as the contract asks; the chain itself is fp32-issue bound: the bit-exact "
-                                   "(un-fused) filter + colour formula needs ~330 fp32 instructions per pixel = 0.29 ms per 8K frame at "
-                                   "148 SMs x 128 lanes x 1.97 GHz, 2.4x the 0.12 ms of the 24.3 B/px at HBM peak (DESIGN.md section 4)"),
+                                   "(un-fused) filter + colour formula needs ~330 fp32 instructions per pixel = 0.33 ms per 8K frame at "
+                                   "132 SMs x 128 lanes x 1.98 GHz (H100 SXM boost), 1.4x the 0.24 ms of the 24.3 B/px at HBM peak "
+                                   "(DESIGN.md section 4)"),
                     "algorithmic_bytes": ("24 B/px x pixels: 3 x 4 B decoded residuals read, 3 x 4 B f32 samples written (Squeeze, RCT and "
                                           "sample conversion fully fused)") if modular else
                                          "24.3 B/px x pixels: 12 B coefficients + 0.33 B LF/meta read, 12 B RGB written (fully fused chain)"}
@@ -494,7 +515,7 @@ def run_ours(args, rank, world, local_rank):
         "data": "synthetic" if "synth" in args.workload else "real-file mosaic",
         "config": {"workload": desc, "frames_per_step_per_gpu": len(frames), "pipeline_workers_per_gpu": pipe_workers(args),
                    "heavy_frames_per_gpu": args.heavy_frames, "lf_batch_streams": args.batch_streams,
-                   "cache": "inputs+planes per step (>= 33 MP x 24 B) exceed L2 (126 MB); no explicit L2 flush",
+                   "cache": "inputs+planes per step (>= 33 MP x 24 B) exceed L2 (50 MB); no explicit L2 flush",
                    "step_barrier": "before and after the K timed steps; frames flow through the in-library pipeline",
                    "hf_streams_per_cta": hf_lanes, "cpu_affinity": "GPU-local CPUs" if cpus else "unchanged"},
         "e2e": {"value": e2e_value, "unit": "MP/s", "h2d_bytes_per_step": int(sum(len(f) for f in frames)),
@@ -507,10 +528,39 @@ def run_ours(args, rank, world, local_rank):
         "gpu_launches": int(launches), "clocks": clocks, "roofline": roofline, "entropy": entropy,
         "kernel_ms_per_step_summed_over_streams": {k: round(v["ms"], 3) for k, v in prof.items()},
         "kernel_ms_per_frame_solo": {k: round(v, 3) for k, v in solo.items()}, "cpu_baseline": cpu,
+        "device": torch.cuda.get_device_name(local_rank),
+        "device_memory_in_use_gb": round((total_b - free_b) / 1e9, 2), "device_memory_gb": round(total_b / 1e9, 2), "dump_outputs": args.dump_outputs,
     }
     if gather is not None:
         line["gather"] = gather
     print(json.dumps(line))
+
+
+def dump_outputs(J, pipe, device, frames, slots, out_dir, budget=60_000_000):
+    """Writes the planar f32 frames (channels, height, width) of the last timed step as out_dir/frame_<k>.npy, one file
+    per distinct frame k of the step in step order. Each is decoded once more by the same pipeline from the same
+    preloaded slot (the decode is deterministic, so these are the arrays the timed step produced). A frame larger than
+    its share of `budget` is stored as a fixed seeded sample of pixel positions, every channel at each position:
+    frame_<k>.npy is then (channels, n) and frame_<k>_index.npy the n flat positions (y * width + x) as float64."""
+    os.makedirs(out_dir, exist_ok=True)
+    order = list(dict.fromkeys(slots))
+    data = {s: f for f, s in zip(frames, slots)}
+    for k, s in enumerate(order):
+        d = J.Decoder(device)
+        d.decode(data[s])
+        fi = d.frame_info(0)
+        c, h, w = fi.num_channels, fi.height, fi.width
+        d.close()
+        out = np.empty((c, h, w), dtype=np.float32)
+        pipe.submit(slot=s, out=out)
+        pipe.wait()
+        n = (budget // len(order)) // (4 * c + 8)
+        if n >= h * w:
+            np.save(os.path.join(out_dir, f"frame_{k}.npy"), out)
+            continue
+        idx = np.unique(np.random.default_rng(1000 + k).integers(0, h * w, n))
+        np.save(os.path.join(out_dir, f"frame_{k}.npy"), out.reshape(c, h * w)[:, idx])
+        np.save(os.path.join(out_dir, f"frame_{k}_index.npy"), idx.astype(np.float64))
 
 
 def pipe_workers(args):
@@ -674,9 +724,9 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="synth8k", help="synth8k | synth4k | mosaic8k | file:PATH")
-    ap.add_argument("--contexts", type=int, default=0, help="pipeline workers = frames in flight per GPU (0: 96, Modular workloads 64)")
+    ap.add_argument("--contexts", type=int, default=0, help="pipeline workers = frames in flight per GPU (0: 64)")
     ap.add_argument("--heavy-frames", type=int, default=0,
-                    help="heavy slots (HBM slab + CUDA stream) per GPU (0: 20, Modular workloads 26)")
+                    help="heavy slots (HBM slab + CUDA stream) per GPU (0: 16, Modular workloads 26)")
     ap.add_argument("--batch-streams", type=int, default=6, help="CUDA streams of the LF batch service")
     ap.add_argument("--frames-per-step", type=int, default=96, help="independent frames decoded per step per GPU")
     ap.add_argument("--cpu-sample-frames", type=int, default=1)
@@ -687,6 +737,9 @@ def main():
                     help="HF coefficient schedule = streams per CTA: 0 (= 4) / 8 / 16 one warp per stream, 32 / 64 / 128 one "
                          "thread per stream; auto = the fixed default (HF_STREAMS_PER_CTA). JXLB_HF_LANES in the environment "
                          "overrides.")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the decoded frames of the last step as DIR/<name>.npy (float32, "
+                         "at most 64 MB in all: a seeded sample of each frame's pixels when they do not fit)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

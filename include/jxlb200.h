@@ -1,4 +1,4 @@
-/* jxlb200 — C ABI of the B200-native JPEG XL decode hot path (libjxlb200.so).
+/* jxlb200 — C ABI of the H100-native JPEG XL decode hot path (libjxlb200.so).
  *
  * This is the boundary a jxl-oxide maintainer binds from Rust (`extern "C"`, see INTEGRATION.md).
  * No C++/torch types cross it: plain pointers, sizes and int status codes. All entry points are
@@ -126,8 +126,8 @@ int32_t jxlb_set_capture(jxlb_decoder* dec, int32_t on);
 int32_t jxlb_set_fuse_filters(jxlb_decoder* dec, int32_t on);
 /* Scheduling of the HF coefficient streams (one per 256x256 group and pass, jxl-frame/src/data/pass_group.rs:31): how
  * many streams share one CTA and its staged tables. 0 (default, = 16), 8, 16, 32: one warp per stream, all presets'
- * tables staged once per CTA - the shortest time for ONE frame (14 ms per 8K frame); 4: the round-1 kernel; 64 / 128:
- * one thread per stream (32 streams per warp): 42 ms for a frame alone, but 16 warps instead of 510, which is what a
+ * tables staged once per CTA - the shortest time for ONE frame; 4: the round-1 kernel; 64 / 128:
+ * one thread per stream (32 streams per warp): slower for a frame alone, but 16 warps instead of 510, which is what a
  * GPU full of frames wants (jxlb_pipeline_create's default). Results are identical; the process-wide default comes
  * from the environment variable JXLB_HF_LANES. */
 int32_t jxlb_set_hf_streams_per_cta(jxlb_decoder* dec, int32_t streams);
@@ -210,8 +210,8 @@ int32_t jxlb_rct_inverse(jxlb_decoder* dec, int32_t* const planes[3], uint32_t w
  * (crates/jxl-render/src/lib.rs:496-509). `workers` frames are in flight (one host thread each, pinned to the CPUs
  * local to the GPU). A frame's LF stage - two long, narrow entropy kernels - holds no CUDA stream: it rides in the
  * kernels of a batch service that merges the LF streams of all frames that are ready. Past the LF stage a frame holds
- * one of `heavy_frames` slots (a pre-allocated slab of HBM for its full-resolution planes + a CUDA stream), so HBM use
- * is heavy_frames x ~25 B/px whatever `workers` is. Frames are reported in completion order. */
+ * one of `heavy_frames` slots (a pre-allocated slab of HBM for its full-resolution planes + a CUDA stream). HBM use
+ * grows with both counts: heavy_frames slabs of ~25 B/px, and per worker an LF arena and a memory pool. Frames are reported in completion order. */
 typedef struct jxlb_pipeline jxlb_pipeline;
 typedef struct {
   int32_t workers;            /* frames in flight (host threads); 0 = default (64) */

@@ -1,8 +1,8 @@
-"""jxl_oxide_b200 — B200-native JPEG XL decode hot path behind jxl-oxide's JxlImage / render_frame() API.
+"""jxl_oxide_b200 — H100-native JPEG XL decode hot path behind jxl-oxide's JxlImage / render_frame() API.
 
 Python host-side mirror of the reference's public interface for this path
 (crates/jxl-oxide/src/lib.rs: JxlImage::builder().read(..), image.render_frame(k) -> Render,
-Render::image_planar()). All sample-level work runs in hand-written sm_100a CUDA kernels inside
+Render::image_planar()). All sample-level work runs in hand-written sm_90a CUDA kernels inside
 libjxlb200.so (C ABI: include/jxlb200.h); this module only marshals bytes and pointers.
 
 There is no CPU fallback: importing works anywhere (so the C ABI can be inspected), but creating a

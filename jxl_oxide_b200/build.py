@@ -1,4 +1,4 @@
-"""Builds libjxlb200.so (sm_100a) in-tree with nvcc. No JIT cache: the .so travels with the repo snapshot.
+"""Builds libjxlb200.so (sm_90a, H100) in-tree with nvcc. No JIT cache: the .so travels with the repo snapshot.
 
 Every source is compiled to its own object file under _obj/ (in parallel, only when it or a header changed), then
 linked; `python -m jxl_oxide_b200.build --force` rebuilds everything, `-v` adds ptxas resource usage."""
@@ -21,9 +21,9 @@ SOURCES = [
 # -fmad=false: the reference's generic float path never contracts a*b+c (SimdVector::muladd is
 # mul+add unless built with +fma, crates/jxl-grid/src/simd.rs:177-199); kernels call __fmaf_rn
 # exactly where the reference calls mul_add.
-NVCC_FLAGS = [
-    "-std=c++17", "-O3", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-fmad=false",
-    "-Xcompiler", "-fPIC,-O2,-ffp-contract=off,-fno-fast-math,-pthread",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ["-std=c++17", "-O3"] + ARCH + [
+    "-lineinfo", "-fmad=false", "-Xcompiler", "-fPIC,-O2,-ffp-contract=off,-fno-fast-math,-pthread",
 ]
 
 
@@ -67,7 +67,7 @@ def build(force=False, verbose=False):
         return obj
     with concurrent.futures.ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as ex:
         objs = list(ex.map(compile_one, srcs))
-    subprocess.check_call([nvcc, "--shared", "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC,-pthread"] + objs +
+    subprocess.check_call([nvcc, "--shared"] + ARCH + ["-Xcompiler", "-fPIC,-pthread"] + objs +
                           ["-o", OUT, "-lcudart"], cwd=CSRC)
     return OUT
 
@@ -88,7 +88,7 @@ def build_variant(name, defines, sources=("kernels/vardct.cu", "kernels/filters_
             obj = _obj_path(src)
         objs.append(obj)
     out = os.path.join(vdir, f"libjxlb200_{name}.so")
-    subprocess.check_call([nvcc, "--shared", "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC,-pthread"] + objs +
+    subprocess.check_call([nvcc, "--shared"] + ARCH + ["-Xcompiler", "-fPIC,-pthread"] + objs +
                           ["-o", out, "-lcudart"], cwd=CSRC)
     return out
 

@@ -31,8 +31,8 @@ CudaBackend::CudaBackend(int device, bool own_stream) : device_(device), own_str
   CUDA_CHECK(cudaSetDevice(device_));
   {
     // The inverse transforms read 32-byte row segments of varblocks whose neighbours (of another size class) are fetched by
-    // another kernel at another time; with the default L2 fetch granularity every such read drags in the rest of its line
-    // (ncu: idct_small 342 MB read for 108 MB of coefficients). JXLB_L2_FETCH = 32 / 64 / 128 sets the device limit.
+    // another kernel at another time; with the default L2 fetch granularity every such read drags in the rest of its line.
+    // JXLB_L2_FETCH = 32 / 64 / 128 sets the device limit.
     static const int l2_fetch = [] {
       const char* e = std::getenv("JXLB_L2_FETCH");
       return e ? std::atoi(e) : 0;
@@ -263,8 +263,8 @@ void CudaBackend::sync() {
   if (!stream_) return;  // a pipeline decoder between leases: nothing of it is queued anywhere
   // The stream writes a sequence number into a mapped host word and the host thread polls it (short spin, then
   // 50 us naps). Waiting inside the driver instead (cudaEventSynchronize, or the implicit wait of a pageable
-  // cudaMemcpyAsync) was measured to return 14-27 ms late on average once 32-48 decoder threads wait at the same time
-  // (profiles/r02_progress.md): the waits serialise on the driver. Here a waiting thread never enters the driver.
+  // cudaMemcpyAsync) was measured to return many milliseconds late once dozens of decoder threads wait at the same time:
+  // the waits serialise on the driver. Here a waiting thread never enters the driver.
   flush_uploads();
   const uint32_t seq = ++sync_seq_;
   launch_signal_word(const_cast<uint32_t*>(h_flag_), seq, S());
@@ -390,8 +390,8 @@ void CudaBackend::set_codestream(const uint8_t* data, size_t size) {
     return;
   }
   size_t need = ((size + 7) & ~size_t(7)) + 64;  // zero padding for the 64-bit bit reader
-  // through pinned memory: a pageable source makes cudaMemcpyAsync stage and wait inside the driver (measured: the
-  // host-bytes path ran 5x slower than the resident one with 32 decoder threads; the copies serialise on the driver)
+  // through pinned memory: a pageable source makes cudaMemcpyAsync stage and wait inside the driver, and with dozens of
+  // decoder threads those copies serialise on the driver
   if (need > input_cap_) {
     if (h_input_) CUDA_CHECK(cudaFreeHost(h_input_));
     h_input_ = nullptr;
@@ -414,8 +414,7 @@ void CudaBackend::set_codestream(const uint8_t* data, size_t size) {
   }
   if (need > codestream_cap_ || in_lf_arena(d_codestream_)) {
     // Stream-ordered (re)allocation with headroom: cudaFree / cudaMalloc wait for the whole device - with dozens of
-    // decoders whose frames differ by a few bytes that was hundreds of device-wide stalls per run (measured: the
-    // host-bytes path 5x slower than the resident one).
+    // decoders whose frames differ by a few bytes that was hundreds of device-wide stalls per run.
     if (d_codestream_ && !in_lf_arena(d_codestream_)) CUDA_CHECK(cudaFreeAsync(d_codestream_, S()));
     d_codestream_ = nullptr;
     codestream_cap_ = std::max<size_t>(need + need / 2, size_t(1) << 20);

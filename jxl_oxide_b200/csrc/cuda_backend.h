@@ -1,4 +1,4 @@
-// CUDA (sm_100a) implementation of the planner's Backend seam: every sample-level stage runs as
+// CUDA (sm_90a) implementation of the planner's Backend seam: every sample-level stage runs as
 // a kernel on one stream; planes live in HBM for the whole frame. There is no CPU fallback: any
 // CUDA failure raises Error(kErrCuda).
 #pragma once

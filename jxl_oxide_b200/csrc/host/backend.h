@@ -1,5 +1,5 @@
 // The seam between the host-side frame planner (syntax parsing + orchestration, this directory)
-// and whatever executes the sample-level work. The product implements it with sm_100a CUDA
+// and whatever executes the sample-level work. The product implements it with sm_90a CUDA
 // kernels (csrc/cuda_backend.cu); the test oracle implements it with a scalar CPU restatement
 // of the reference (oracle/). It plays the role of the reference's arch-dispatched `impls::`
 // modules (crates/jxl-render/src/vardct/mod.rs:25-46, filter/impls.rs:3-25) plus the entropy

@@ -665,12 +665,13 @@ void launch_decode_hf_lanes(const uint8_t* cs, DevFrame f, DevHfParams p, const 
                             uint64_t* end_bits, int* status, int num_jobs, int first_pass, int streams_per_cta,
                             cudaStream_t stream) {
   if (num_jobs <= 0) return;
-  static bool attr_set = false;
-  if (!attr_set) {
+  // C++ function-local statics are initialised once, thread-safely: no worker thread launches before the limits are set
+  static const bool attr_set = [] {
     cudaFuncSetAttribute(decode_hf_lanes_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     cudaFuncSetAttribute(decode_hf_lanes_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    attr_set = true;
-  }
+    return true;
+  }();
+  (void)attr_set;
   static const uint32_t env_stride = [] {
     const char* e = std::getenv("JXLB_HF_LANE_STRIDE");
     const int v = e ? std::atoi(e) : 0;
@@ -691,12 +692,13 @@ namespace {
 template <int W, bool SHARED_CMAP>
 void launch_hf_warps(const uint8_t* cs, DevFrame f, DevHfParams p, const DevHfJob* jobs, uint64_t* end_bits, int* status,
                      int num_jobs, int first_pass, cudaStream_t stream) {
-  static bool attr_set = false;
-  if (!attr_set) {
+  // C++ function-local statics are initialised once, thread-safely: no worker thread launches before the limits are set
+  static const bool attr_set = [] {
     cudaFuncSetAttribute(decode_hf_fast_kernel<false, W, SHARED_CMAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     cudaFuncSetAttribute(decode_hf_fast_kernel<true, W, SHARED_CMAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    attr_set = true;
-  }
+    return true;
+  }();
+  (void)attr_set;
   const HfSmem L = hf_layout(p, W, SHARED_CMAP);
   const int ctas = (num_jobs + W - 1) / W;
   if (f.subsampled)
@@ -710,12 +712,13 @@ namespace {
 template <int W, bool ANS_SMEM>
 void launch_hf_warp(const uint8_t* cs, DevFrame f, DevHfParams p, const DevHfJob* jobs, uint64_t* end_bits, int* status,
                     int num_jobs, int first_pass, cudaStream_t stream) {
-  static bool attr_set = false;
-  if (!attr_set) {
+  // C++ function-local statics are initialised once, thread-safely: no worker thread launches before the limits are set
+  static const bool attr_set = [] {
     cudaFuncSetAttribute(decode_hf_warp_kernel<false, W, ANS_SMEM>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     cudaFuncSetAttribute(decode_hf_warp_kernel<true, W, ANS_SMEM>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    attr_set = true;
-  }
+    return true;
+  }();
+  (void)attr_set;
   const HfSmem L = hf_layout(p, W, true);
   const int ctas = (num_jobs + W - 1) / W;
   if (f.subsampled)

@@ -58,8 +58,8 @@ JXLB_FS float fs_float(uint32_t a) {
 JXLB_FS float fs_absdiff(float a, float b) { return fabsf(fs_sub(a, b)); }
 
 // The Gaborish and distance phases walk the three channels with the same code (a loop, not three unrolled copies): the
-// kernel is straight-line code that every warp executes once, so its size is instruction-fetch traffic (ncu: 2.3 cycles of
-// "no instruction" stall per issue with the fully unrolled 4096-instruction body). JXLB_STRIP_ROLL=0 unrolls them again.
+// kernel is straight-line code that every warp executes once, so its size is instruction-fetch traffic (the fully unrolled
+// body stalls on instruction fetch). JXLB_STRIP_ROLL=0 unrolls them again.
 #ifndef JXLB_STRIP_ROLL
 #define JXLB_STRIP_ROLL 1
 #endif

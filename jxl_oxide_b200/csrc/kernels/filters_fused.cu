@@ -607,8 +607,8 @@ void launch_filters_fused(const DevView in[3], const DevView out[3], DevFusedFil
     }
     v.use_tma = ok ? 1 : 0;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
+  // C++ function-local statics are initialised once, thread-safely: no worker thread launches before the limits are set
+  static const bool attr_set = [] {
     cudaFuncSetAttribute(fused_filter_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 6 * window_size(0) * window_size(0) * 4);
     cudaFuncSetAttribute(fused_filter_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * window_size(2) * window_size(2) * 4);
     cudaFuncSetAttribute(fused_filter_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, 12 * window_size(6) * window_size(6) * 4);
@@ -618,8 +618,9 @@ void launch_filters_fused(const DevView in[3], const DevView out[3], DevFusedFil
     cudaFuncSetAttribute(strip_filter_kernel<2, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, fstrip::kSmemFloats * 4);
     cudaFuncSetAttribute(strip_filter_kernel<2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, fstrip::kSmemFloats * 4);
     cudaFuncSetAttribute(strip_filter_kernel<2, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, fstrip::kSmemFloats * 4);
-    attr_set = true;
-  }
+    return true;
+  }();
+  (void)attr_set;
   dim3 block(32, 8);
   dim3 grid((v.width + kT - 1) / kT, (v.height + kT - 1) / kT);
   v.border_only = 0, v.bx_last = v.by_last = 0, v.nbx = int(grid.x), v.nby = int(grid.y);
@@ -629,9 +630,9 @@ void launch_filters_fused(const DevView in[3], const DevView out[3], DevFusedFil
   static const bool no_strip = std::getenv("JXLB_NO_STRIP") != nullptr;
   const fstrip::StripRect r = fstrip::strip_rect(v.width, v.height);
   // The strip kernel's window origins are 28 + 56 * tx and, for the pulled-back last column of tiles, width - 64: TMA wants the
-  // box to start on a 16-byte boundary in the innermost dimension (cp.async.bulk.tensor with an origin of 325 floats ended in
-  // "illegal instruction": call EE, profiles/r02_raw/r02ee_memcheck_strip3wip.log), so frames whose width is not a multiple of
-  // four samples stay in the general kernel, whose origins are multiples of four by construction.
+  // box to start on a 16-byte boundary in the innermost dimension (cp.async.bulk.tensor with an origin of 325 floats ends in
+  // "illegal instruction"), so frames whose width is not a multiple of four samples stay in the general kernel, whose origins
+  // are multiples of four by construction.
   const bool origins_aligned = (v.width & 3) == 0;
   if (!no_strip && v.use_tma && origins_aligned && p.gab_enabled && (p.epf_iters == 1 || p.epf_iters == 2) && r.x1 > r.x0 && r.y1 > r.y0) {
     FusedMaps smaps;

@@ -1,4 +1,4 @@
-// Launch wrappers for the sm_100a kernels. Plain C++ signatures over raw device pointers so that
+// Launch wrappers for the sm_90a kernels. Plain C++ signatures over raw device pointers so that
 // both the CUDA backend (cuda_backend.cu) and the stage-level C ABI (capi.cu) can call them.
 #pragma once
 #include <cstdint>

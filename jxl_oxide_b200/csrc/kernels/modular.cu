@@ -310,7 +310,7 @@ void launch_modular_xyb(DevView y, DevView x, DevView b, float mx, float my, flo
 void launch_fill_u32(uint32_t* p, size_t n, uint32_t value, cudaStream_t stream) {
   if (!n) return;
   size_t blocks = (n + 1023) / 1024;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;  // grid cap for the grid-stride loop (16 x the H100's 132 SMs)
   fill_kernel<<<unsigned(blocks), 256, 0, stream>>>(p, n, value);
 }
 

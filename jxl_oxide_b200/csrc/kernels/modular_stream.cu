@@ -638,8 +638,8 @@ __global__ void __launch_bounds__(32) modular_stream_kernel(const uint8_t* __res
 }
 
 // The same streams for several frames in ONE launch (csrc/pipeline.cu, LF batch service): CTA i decodes job
-// `refs[i].job` of the frame whose tables `refs[i]` points to. A frame's LF stage is two ~80 / ~25 ms kernels of a
-// dozen one-lane warps; launched per frame they pin one CUDA stream (= one of the device's 32 hardware queues) for
+// `refs[i].job` of the frame whose tables `refs[i]` points to. A frame's LF stage is two long kernels (tens of milliseconds) of
+// a dozen one-lane warps; launched per frame they pin one CUDA stream (= one of the device's 32 hardware queues) for
 // the whole time, which caps the frames in flight. Batched, a handful of streams carry every frame's LF stage.
 template <bool ALLSM>
 __global__ void __launch_bounds__(32) modular_stream_batch_kernel(const DevModularBatchRef* __restrict__ refs, int total) {
@@ -649,7 +649,7 @@ __global__ void __launch_bounds__(32) modular_stream_batch_kernel(const DevModul
   modular_stream_body<ALLSM>(smem, r.cs, r.jobs, r.channels, r.plans, r.end_bits, r.status, int(r.job), nullptr);
   if (r.counter) {
     // this frame's streams are done when its last one is: samples and result words first, then the count, then the word
-    // the frame's host thread is woken by (the rest of the launch belongs to other frames and may run for another 80 ms)
+    // the frame's host thread is woken by (the rest of the launch belongs to other frames and may run for much longer)
     __threadfence_system();
     __syncwarp();
     if ((threadIdx.x & 31) == 0 && atomicAdd(r.counter, 1u) == r.num_jobs - 1) {
@@ -743,12 +743,13 @@ void launch_modular_decode(const uint8_t* cs, const DevModularJob* jobs, const D
                            const DevChannelPlan* plans, uint64_t* end_bits, int* status, int num_jobs, size_t smem_bytes,
                            bool all_tables_staged, cudaStream_t stream, unsigned long long* trace) {
   if (num_jobs <= 0) return;
-  static bool attr_set = false;
-  if (!attr_set) {
+  // C++ function-local statics are initialised once, thread-safely: no worker thread launches before the limits are set
+  static const bool attr_set = [] {
     cudaFuncSetAttribute(modular_stream_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     cudaFuncSetAttribute(modular_stream_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    attr_set = true;
-  }
+    return true;
+  }();
+  (void)attr_set;
   if (all_tables_staged)
     modular_stream_kernel<true><<<num_jobs, 32, smem_bytes, stream>>>(cs, jobs, channels, plans, end_bits, status, num_jobs, trace);
   else
@@ -758,12 +759,13 @@ void launch_modular_decode(const uint8_t* cs, const DevModularJob* jobs, const D
 void launch_modular_decode_batch(const DevModularBatchRef* refs, int total, size_t smem_bytes, bool all_tables_staged,
                                  cudaStream_t stream) {
   if (total <= 0) return;
-  static bool attr_set = false;
-  if (!attr_set) {
+  // C++ function-local statics are initialised once, thread-safely: no worker thread launches before the limits are set
+  static const bool attr_set = [] {
     cudaFuncSetAttribute(modular_stream_batch_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     cudaFuncSetAttribute(modular_stream_batch_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    attr_set = true;
-  }
+    return true;
+  }();
+  (void)attr_set;
   if (all_tables_staged) modular_stream_batch_kernel<true><<<total, 32, smem_bytes, stream>>>(refs, total);
   else modular_stream_batch_kernel<false><<<total, 32, smem_bytes, stream>>>(refs, total);
 }

@@ -533,7 +533,7 @@ __device__ void transform_special(Grid c, int type, float* scratch /* 64 + 48 fl
 
 // Medium class, by shape (width x height in 8x8 cells): 2x1 1x2 2x2 4x1 1x4 4x2 2x4 4x4. The medium kernel walks the shapes
 // one after the other so that the warps of an SM execute the same transform sizes at the same time (its unrolled
-// 8 / 16 / 32-point transforms do not fit the instruction cache together: ncu showed "no instruction" as the top stall).
+// 8 / 16 / 32-point transforms do not fit the instruction cache together: instruction fetch was the top stall).
 constexpr int kMediumShapes = 8;
 __host__ __device__ inline int medium_shape(int w8, int h8) {
   return w8 == 2 ? (h8 == 1 ? 0 : (h8 == 2 ? 2 : 6)) : (w8 == 1 ? (h8 == 2 ? 1 : 4) : (h8 == 1 ? 3 : (h8 == 2 ? 5 : 7)));
@@ -849,9 +849,8 @@ __device__ __forceinline__ void cfl_factors(const DevFrame& f, const DevDequantP
   kb = __fadd_rn(p.base_correlation_b, __fdiv_rn(float(f.b_from_y[ti]), p.colour_factor));
 }
 
-// Experiment knobs (build.build_variant): defaults are the measured best (profiles/r02_progress.md, call U: requesting
-// the three channels together costs idct_small 39 registers and a third of its warps: 0.327 ms against 0.239 ms; medium
-// trips of 4 / 8 / 16 rows: 0.599 / 0.503 / 0.572 ms).
+// Experiment knobs (build.build_variant): defaults are the measured best (requesting the three channels together costs
+// idct_small registers and a third of its warps; medium trips of 8 rows beat 4 and 16).
 #ifndef JXLB_SMALL_PREFETCH
 #define JXLB_SMALL_PREFETCH 0  // idct_small: request the three channels' rows of a block together
 #endif
@@ -1137,12 +1136,12 @@ __global__ void __launch_bounds__(kMediumWarps * 32) idct_medium_kernel(DevFrame
 // Same tiling as idct_medium_kernel (one warp per 32 x 32 tile of equally shaped blocks, lane = tile column in the load /
 // column / store passes, lane = tile row in the row pass) and the same per-sample operations in the same order, but the
 // shape is a template parameter: block-row / row loops are static, so the per-sample pointer selection, shifts and table
-// look-ups of the generic body (which spent ~3x more instructions on indexing than on arithmetic, ncu) fold into
+// look-ups of the generic body (which spent several times more instructions on indexing than on arithmetic) fold into
 // immediates. The shapes are walked one after the other by all CTAs in step, so one instantiation's code is hot at a time,
 // and the line transforms are the shared idct_line_smem<N>.
 #ifndef JXLB_MEDIUM_ROLL
-#define JXLB_MEDIUM_ROLL 0     // medium_walk: block rows / 8-row batches of a tile as loops instead of unrolled. Measured (call Z):
-#endif                         // 12 968 instead of 28 264 instructions, but 0.462 ms against 0.391 ms - the unrolled form wins
+#define JXLB_MEDIUM_ROLL 0     // medium_walk: block rows / 8-row batches of a tile as loops instead of unrolled: less than
+#endif                         // half the instructions, but measured slower - the unrolled form wins
 constexpr int kMediumOuterUnroll = JXLB_MEDIUM_ROLL ? 1 : 32;
 struct MediumBlk {
   uint32_t bx, by;     // block position in 8x8 cells (dequantising frames are never subsampled: the same for all channels)
@@ -1187,8 +1186,8 @@ __device__ __forceinline__ void medium_walk(const DevFrame& f, const DevDequantP
 #pragma unroll 1
     for (int ci = 0; ci < 3; ++ci) {
       const uint32_t c = ci == 0 ? 1u : (ci == 1 ? 0u : 2u);  // Y first: its dequantised samples feed the chroma channels
-      // (requesting the chroma rows into L2 while Y is transformed was measured slower: 0.467 ms against 0.388 ms per 8K frame and
-      // 130 MB more DRAM reads - the tile's three channels already overlap across the SM's warps; profiles/r02_progress.md, call Y)
+      // (requesting the chroma rows into L2 while Y is transformed was measured slower, with more DRAM reads: the tile's three
+      // channels already overlap across the SM's warps)
       const float* __restrict__ matc = dq.matrices + dq.matrix_offset[(set * 3 + c) * 2 + tr] + x;
       const float qb = dq.quant_bias[c], qbn = dq.quant_bias_numerator;
       float* const plane = reinterpret_cast<float*>(f.coeff[c]);
@@ -1260,7 +1259,7 @@ __device__ __forceinline__ void medium_walk(const DevFrame& f, const DevDequantP
 }
 
 #ifndef JXLB_MEDIUM_MINB
-#define JXLB_MEDIUM_MINB 5  // measured: 4 -> 0.419 ms, 5 -> 0.388 ms, 6 -> 0.447 ms (call W)
+#define JXLB_MEDIUM_MINB 5  // the fastest of 4 / 5 / 6 when measured; not re-measured on the H100
 #endif
 __global__ void __launch_bounds__(kMediumWarps * 32, JXLB_MEDIUM_MINB) idct_medium_deq_kernel(DevFrame f, DevDequantParams dq, TransformLists lists) {
   __shared__ float s_tile[kMediumWarps][32 * 33];
@@ -1623,21 +1622,22 @@ void launch_hf_transform(DevFrame f, void* scratch, const DevDequantParams* dq, 
       q += cells + 1;
     }
   }
-  // measured (calls Y, Z): 0.235 ms against 0.241 ms for idct_small, but 140 MB more DRAM reads per 8K frame: off by default
+  // measured: no faster for idct_small, and more DRAM reads per frame: off by default
   static const bool l2_prefetch = std::getenv("JXLB_L2_PREFETCH") != nullptr;
   L.flags = l2_prefetch ? 1u : 0u;
   cudaMemsetAsync(L.counts, 0, 128, stream);
   dim3 cb(32, 8), cg((f.bw + 31) / 32, (f.bh + 7) / 8);
   classify_varblocks_kernel<<<cg, cb, 0, stream>>>(f, L);
-  static int num_sms = 0;
-  if (!num_sms) {
-    int dev = 0;
+  // initialised once, thread-safely (function-local static): no worker thread launches before the limits are set
+  static const int num_sms = [] {
+    int dev = 0, n = 0;
     cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
     cudaFuncSetAttribute(idct_large_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 140 * 1024);
     cudaFuncSetAttribute(idct_large_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 140 * 1024);
     cudaFuncSetAttribute(idct_large64_deq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kL64SmemFloats * 4);
-  }
+    return n;
+  }();
   if (dq && !f.subsampled) {
     launch_idcts<true>(f, *dq, L, cells, num_sms, stream);
   } else {

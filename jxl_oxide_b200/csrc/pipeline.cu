@@ -7,8 +7,8 @@
 // only a few milliseconds in kernels that fill the GPU. Throughput therefore needs many frames in flight, but a
 // frame past its LF stage holds ~25 bytes per pixel of planes. The pipeline separates the two: `workers` frames may be
 // anywhere, at most `heavy_frames` of them past Backend::begin_heavy_stage(); each heavy slot owns a pre-allocated
-// slab the full-resolution planes are carved from, so a frame costs no allocator call and HBM use is bounded by
-// heavy_frames x slab whatever `workers` is. Frames flow without barriers, so the contexts de-phase by themselves and
+// slab the full-resolution planes are carved from, so a frame costs no allocator call. HBM use grows with both counts:
+// heavy_frames x slab, and per worker its LF arena and the memory pool of its decoder (which keeps what it held). Frames flow without barriers, so the contexts de-phase by themselves and
 // the GPU-filling stages of some frames overlap the latency-bound stages of others.
 #include <condition_variable>
 #include <cstdio>
@@ -65,8 +65,8 @@ struct Slab {  // a heavy slot: HBM for a frame's full-resolution planes + the C
   cudaStream_t stream = nullptr;
 };
 
-// LF batch service: the Modular launches of every frame's LF stage (LfCoeff, HfMetadata: ~80 / ~25 ms kernels of a dozen
-// one-lane warps) ride in shared kernels on a few batch streams. A frame in its LF stage therefore holds no CUDA stream
+// LF batch service: the Modular launches of every frame's LF stage (LfCoeff, HfMetadata: long kernels of a dozen one-lane
+// warps) ride in shared kernels on a few batch streams. A frame in its LF stage therefore holds no CUDA stream
 // and any number of frames can be in flight; the device's 32 hardware queues are left to the batch streams and the heavy
 // slots. One service thread: it launches whatever is pending whenever a batch stream is free (so batches grow by
 // themselves under load), polls the mapped completion words of the batches in flight and wakes the frames' threads.
@@ -252,7 +252,7 @@ class BatchService : public LfBatchService {
           break;
         }
       // Pacing: with every batch stream free at once, the first arrival would take one stream, the next arrival the next
-      // one ... and everything after that waits a whole kernel (80 ms) for the streams to free up - again all together.
+      // one ... and everything after that waits a whole (long) kernel for the streams to free up - again all together.
       // Launches are therefore spaced a stream's share of the typical batch duration apart: the streams stay staggered
       // and a frame waits that share at most (half of it on average) for its ride.
       const auto now = std::chrono::steady_clock::now();
@@ -375,7 +375,7 @@ struct jxlb_pipeline {
   }
   // The output ring is allocated in one go the first time a frame asks for `bytes` (and again if a larger frame comes):
   // cudaHostAlloc of a few hundred MB takes tens of milliseconds during which no other thread gets a CUDA call through,
-  // so it must not trickle into steady state buffer by buffer (measured: 12 ms per frame lost that way).
+  // so it must not trickle into steady state buffer by buffer.
   void* acquire_host(size_t bytes) {
     std::unique_lock<std::mutex> lk(mu);
     if (bytes > host_bytes) {
@@ -516,7 +516,7 @@ struct jxlb_pipeline {
         }
         if (rc == JXLB_OK) {
           // Device -> host copies of different streams share the copy engines chunk by chunk; a dozen 400 MB copies
-          // in flight together were measured at 29 GB/s in total against 55 GB/s for one at a time. The decode work of the
+          // in flight together were measured slower in total than one at a time. The decode work of the
           // other frames goes on meanwhile; only the copies queue up.
           rc = jxlb_sync(dec);
           std::lock_guard<std::mutex> copy_lock(copy_mu);
@@ -572,8 +572,7 @@ int32_t jxlb_pipeline_create(int32_t device, const jxlb_pipeline_config* cfg, jx
   {
     // A pipeline owns its device's decode work: L2 fetches 32-byte sectors instead of whole 128-byte lines. The inverse
     // transforms read 32-byte row segments of varblocks whose line neighbours belong to another size class, i.e. to another
-    // kernel at another time; measured on an 8K frame (ncu dram__bytes_read): idct_small 342 -> 121 MB, idct_medium
-    // 533 -> 259 MB, kernel times unchanged (profiles/r02_progress.md, call W). JXLB_L2_FETCH=0 leaves the limit alone,
+    // kernel at another time, so 32-byte fetches read less DRAM for the same kernel times. JXLB_L2_FETCH=0 leaves the limit alone,
     // 64 / 128 set another value (also honoured by stand-alone decoders, which do not touch the limit by default).
     const char* e = std::getenv("JXLB_L2_FETCH");
     const int g = e ? std::atoi(e) : 32;

@@ -267,7 +267,7 @@ def test_blend_modes_and_swapped_patch_roles(dec):
 def test_mutated_streams_end_in_values(dec):
     """Bit flips / truncations / overwritten runs in valid streams: every decode ends in pixels or a
     JxlError value, and the decoder keeps working (tools/mutate_check.py runs the same under
-    compute-sanitizer memcheck: 0 errors, profiles/r01_progress.md)."""
+    compute-sanitizer memcheck)."""
     import random
     import jxl_oxide_b200
     rng = random.Random(99)

@@ -1,7 +1,6 @@
 """The synthetic Modular lossless stream (tools/synth_enc.cc --modular: YCoCg RCT + default Squeeze + weighted predictor,
 BASELINE config #4) decodes, through the oracle, to exactly the image it was made from: the encoder's forward transforms
 are inverted bit for bit by the restated reference path (and the stream's syntax is what the shared parser expects)."""
-import os
 import subprocess
 
 import numpy as np
@@ -12,8 +11,7 @@ import bench
 
 @pytest.mark.parametrize("w,h,seed", [(600, 400, 3), (1100, 700, 5), (513, 900, 2)])
 def test_lossless_round_trip(oracle, tmp_path, w, h, seed):
-    bench.synth_frame(64 * 5, 64 * 5, 1, extra=("--modular",))  # makes sure the tool is built
-    tool = os.path.join(bench.ROOT, "tools", "_build_synth_enc")
+    tool = bench.synth_tool()
     jxl, raw = str(tmp_path / "m.jxl"), str(tmp_path / "m.raw")
     subprocess.check_call([tool, "--modular", "--width", str(w), "--height", str(h), "--seed", str(seed), "-o", jxl, "--dump-raw", raw],
                           stderr=subprocess.DEVNULL)

@@ -8,10 +8,10 @@ weighted sums and the colour stage are contracted to one fused multiply-add each
   1. the error that costs: the copy is compiled for the host (tests/emu harness: every CTA run thread by thread, phase by
      phase; std::fmaf is the same correctly rounded operation as the device's FFMA) and its output is compared with the
      oracle's, sample by sample, in units in the last place of the oracle's value;
-  2. the instructions it saves: static SASS size of strip_filter_kernel<2, sRGB> with and without contraction (nvcc, sm_100a).
+  2. the instructions it saves: static SASS size of strip_filter_kernel<2, sRGB> with and without contraction (nvcc, sm_90a).
 
 Nothing here touches the product sources; the copies live under tools/_fma_build/ (git-ignored).
-    python tools/fma_study.py            # writes profiles/r02_fma_study.md
+    python tools/fma_study.py            # prints the report and writes it to tools/_fma_build/fma_study.md
 """
 import collections
 import ctypes
@@ -160,13 +160,13 @@ def main():
         lines.append(f"| {name} | {n} | {pct(0)} | {pct(1)} | {pct(2)} | {pct(3)} | {100.0 * mid / n:.2f} % | {pct(9)} | {mx} | {amax:.3g} |")
     lines += ["", "Large ULP counts sit on samples near zero (a difference of 1e-7 is many units in the last place of 1e-6): the last column",
               "is the largest absolute difference, to be read against sample values in [0, 1].", "",
-              f"Static size of `strip_filter_kernel<2, sRGB>` (sm_100a): {sum(ce.values())} instructions as shipped "
+              f"Static size of `strip_filter_kernel<2, sRGB>` (sm_90a): {sum(ce.values())} instructions as shipped "
               f"(FADD {ce['FADD']}, FMUL {ce['FMUL']}, FFMA {ce['FFMA']}: {fp(ce)} fp32 arithmetic), {sum(cf.values())} contracted "
               f"(FADD {cf['FADD']}, FMUL {cf['FMUL']}, FFMA {cf['FFMA']}: {fp(cf)}): {100.0 * (1 - sum(cf.values()) / sum(ce.values())):.0f} % fewer "
-              "instructions in a kernel that is bound by instruction issue (ncu: 73 % of the issue slots). The contracted build is not",
+              "instructions in a kernel that is bound by instruction issue. The contracted build is not",
               "within 1 ULP of the reference everywhere (table above), so it does not meet north_star's parity bar as it stands and is",
               "not offered as a run-time option; the shipped kernels keep bit equality."]
-    out = os.path.join(ROOT, "profiles", "r02_fma_study.md")
+    out = os.path.join(BUILD, "fma_study.md")
     with open(out, "w") as f:
         f.write("\n".join(lines) + "\n")
     print("\n".join(lines))
