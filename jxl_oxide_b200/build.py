@@ -13,7 +13,7 @@ OBJ = os.path.join(HERE, "_obj")
 OUT = os.path.join(HERE, "libjxlb200.so")
 
 SOURCES = [
-    "capi.cu", "cuda_backend.cu", "pipeline.cu",
+    "capi.cu", "cuda_backend.cu", "launch_tables.cc", "pipeline.cu",
     "kernels/modular.cu", "kernels/modular_stream.cu", "kernels/entropy.cu", "kernels/blockinfo.cu", "kernels/vardct.cu", "kernels/filters.cu", "kernels/filters_fused.cu",
     "host/entropy.cc", "host/headers.cc", "host/modular_syntax.cc", "host/frame_syntax.cc", "host/planner.cc", "host/icc.cc",
 ]

@@ -1,17 +1,13 @@
 // See cuda_backend.h.
 #include "cuda_backend.h"
-#include "kernels/modular_plan.cuh"
 
 #include <algorithm>
 #include <chrono>
-#include <climits>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <atomic>
-#include <memory>
 #include <thread>
-#include <tuple>
 
 namespace jxlb {
 
@@ -437,12 +433,7 @@ void CudaBackend::new_frame() {
 
 void CudaBackend::ensure_static_tables() {
   if (!d_natural_orders_) {
-    std::vector<uint32_t> all;
-    for (uint32_t id = 0; id < 13; ++id) {
-      natural_order_offset_[id] = uint32_t(all.size());
-      std::vector<uint32_t> o = natural_order(id);
-      all.insert(all.end(), o.begin(), o.end());
-    }
+    const std::vector<uint32_t> all = natural_order_table(natural_order_offset_);
     CUDA_CHECK(cudaMalloc(&d_natural_orders_, all.size() * 4));
     CUDA_CHECK(cudaMemcpy(d_natural_orders_, all.data(), all.size() * 4, cudaMemcpyHostToDevice));
   }
@@ -565,37 +556,6 @@ void CudaBackend::stage_marker(const char* name, const View* views, int n) {
   }
 }
 
-DevEntropyCode CudaBackend::upload_code(const EntropyCode& c) {
-  DevEntropyCode d;
-  std::memset(&d, 0, sizeof(d));
-  d.cluster_map = static_cast<const uint8_t*>(upload_temp(c.cluster_map.data(), c.cluster_map.size()));
-  std::vector<uint32_t> cfg;
-  for (const HybridUintConfig& h : c.configs) cfg.push_back(h.packed());
-  d.configs = static_cast<const uint32_t*>(upload_temp(cfg.data(), cfg.size() * 4));
-  d.log_alphabet_size = c.log_alphabet_size;
-  d.use_prefix = c.use_prefix ? 1 : 0;
-  d.num_clusters = c.num_clusters;
-  d.cluster_map_size = uint32_t(c.cluster_map.size());
-  d.prefix_table_size = uint32_t(c.prefix_table.size());
-  if (c.use_prefix) {
-    d.prefix = static_cast<const uint32_t*>(upload_temp(c.prefix_table.data(), c.prefix_table.size() * 4));
-    std::vector<uint32_t> meta;
-    for (const PrefixMeta& m : c.prefix_meta) {
-      meta.push_back(m.table_offset);
-      meta.push_back(m.root_bits);
-    }
-    d.prefix_meta = static_cast<const uint32_t*>(upload_temp(meta.data(), meta.size() * 4));
-  } else {
-    d.ans = static_cast<const uint64_t*>(upload_temp(c.ans_table.data(), c.ans_table.size() * 8));
-  }
-  d.lz77_enabled = c.lz77_enabled ? 1 : 0;
-  d.lz77_min_symbol = c.lz77_min_symbol;
-  d.lz77_min_length = c.lz77_min_length;
-  d.lz_len_conf = c.lz_len_conf.packed();
-  d.lz_dist_cluster = c.cluster_map.empty() ? 0 : c.cluster_map.back();
-  return d;
-}
-
 namespace {
 const char* dev_status_message(int s) {
   switch (s) {
@@ -606,257 +566,21 @@ const char* dev_status_message(int s) {
     default: return "unknown device decode error";
   }
 }
-// The part of an MA tree one channel of one stream can reach, with static decisions resolved and
-// node indices renumbered from 0 (the reference prunes the same way when it flattens a tree for a
-// channel, crates/jxl-modular/src/ma.rs:579-645). Small enough to live in shared memory even when
-// the frame's global tree has thousands of nodes.
-struct ChannelTree {
-  std::vector<MaNode> nodes;  // nodes[0] is the root
-  int32_t lut_prop = -1, lut_base = 0;
-  std::vector<uint16_t> lut;  // leaf indices into `nodes`
-  bool stream_dependent = false;
-};
-
-constexpr size_t kMaxChannelTreeNodes = 60000;
-
-bool build_channel_tree(const MaTree& t, uint32_t ci, uint32_t stream, int nprev, ChannelTree* out) {
-  auto resolve = [&](uint32_t idx) {
-    for (;;) {
-      const MaNode& n = t.nodes[idx];
-      if (n.property < 0) return idx;
-      int32_t v;
-      if (n.property == 0) v = int32_t(ci);
-      else if (n.property == 1) {
-        v = int32_t(stream);
-        out->stream_dependent = true;
-      } else if (n.property >= 16 && (n.property - 16) / 4 >= nprev) v = 0;
-      else return idx;
-      idx = v > n.value ? n.a : n.b;
-    }
-  };
-  out->nodes.clear();
-  out->nodes.push_back(t.nodes[resolve(0)]);
-  std::vector<uint32_t> stack = {0};
-  while (!stack.empty()) {
-    const uint32_t cur = stack.back();
-    stack.pop_back();
-    if (out->nodes[cur].property < 0) continue;
-    if (out->nodes.size() + 2 > kMaxChannelTreeNodes) return false;
-    const uint32_t a = resolve(out->nodes[cur].a), b = resolve(out->nodes[cur].b);
-    const uint32_t na = uint32_t(out->nodes.size());
-    out->nodes.push_back(t.nodes[a]);
-    out->nodes.push_back(t.nodes[b]);
-    out->nodes[cur].a = na;
-    out->nodes[cur].b = na + 1;
-    stack.push_back(na);
-    stack.push_back(na + 1);
-  }
-  // single-property subtree -> leaf LUT over [lower, upper + 1] (ma.rs:241-330)
-  int prop = -1;
-  int64_t lower = INT64_MAX, upper = INT64_MIN;
-  for (const MaNode& n : out->nodes) {
-    if (n.property < 0) continue;
-    if (n.property >= 16 || (prop >= 0 && prop != n.property)) return true;  // general walk
-    prop = n.property;
-    lower = std::min<int64_t>(lower, n.value);
-    upper = std::max<int64_t>(upper, n.value);
-  }
-  if (prop < 0) {  // single leaf
-    out->lut_prop = 6;
-    out->lut_base = 0;
-    out->lut.assign(1, 0);
-    return true;
-  }
-  if (upper - lower > 1022) return true;
-  out->lut_prop = prop;
-  out->lut_base = int32_t(lower);
-  for (int64_t v = lower; v <= upper + 1; ++v) {
-    uint32_t idx = 0;
-    while (out->nodes[idx].property >= 0) idx = v > out->nodes[idx].value ? out->nodes[idx].a : out->nodes[idx].b;
-    out->lut.push_back(uint16_t(idx));
-  }
-  return true;
-}
-
 }  // namespace
 
 void CudaBackend::decode_modular(std::vector<ModularStreamJob>& jobs) {
   if (jobs.empty()) return;
-  struct TreeDev {
-    const MaNode* nodes = nullptr;  // full tree, uploaded only for the uncompacted fallback
-    DevEntropyCode code;
-    bool wp = false;
-  };
-  struct JobTables {  // device tables shared by every job with the same per-channel subtrees
-    const MaNode* nodes;
-    uint32_t num_nodes;
-    const uint16_t* luts;
-    uint32_t lut_total;
-    std::vector<DevChannelPlan> plans;
-    bool wp;
-  };
-  std::map<const MaTree*, TreeDev> trees;
-  std::map<std::tuple<const MaTree*, uint32_t, int, int64_t>, std::unique_ptr<ChannelTree>> channel_trees;
-  std::map<std::vector<const ChannelTree*>, JobTables> job_tables;
-  std::vector<DevModularJob> djobs(jobs.size());
-  std::vector<DevChannel> dchans;
-  std::vector<DevChannelPlan> dplans;
-  size_t max_smem = 0;
-  bool all_staged = true;
+  ModularLaunch L = build_modular_launch(jobs, [this](const View& v) { return dev_view(v); }, *this);
   for (size_t i = 0; i < jobs.size(); ++i) {
-    const ModularStreamJob& j = jobs[i];
-    auto it = trees.find(j.tree);
-    if (it == trees.end()) {
-      TreeDev td;
-      td.code = upload_code(j.tree->code);
-      it = trees.emplace(j.tree, td).first;
-    }
-    DevModularJob& d = djobs[i];
-    std::memset(&d, 0, sizeof(d));
-    d.bit_pos = j.bit_pos;
-    d.bit_limit = j.bit_limit;
-    d.code = it->second.code;
-    const WpHeader& w = j.wp;
-    const uint32_t wpv[11] = {w.p1, w.p2, w.p3a, w.p3b, w.p3c, w.p3d, w.p3e, w.w[0], w.w[1], w.w[2], w.w[3]};
-    std::memcpy(d.wp, wpv, sizeof(wpv));
-    d.stream_index = j.stream_index;
-    d.first_channel = uint32_t(dchans.size());
-    d.num_channels = uint32_t(j.channels.size());
-    uint32_t max_w = 0;
-    uint64_t samples = 0;
-    for (const ModularChannelTarget& c : j.channels) {
-      DevView v = dev_view(c.view);
-      dchans.push_back({static_cast<int32_t*>(v.ptr), v.stride, c.view.w, c.view.h, c.hshift, c.vshift});
-      max_w = std::max(max_w, c.view.w);
-      samples += uint64_t(c.view.w) * c.view.h;
-    }
-    d.dist_multiplier = max_w;
-    // per-channel subtrees (cached across the jobs of this call when they do not depend on the stream index)
-    std::vector<const ChannelTree*> key;
-    bool compact = true;
-    std::vector<int> nprevs(j.channels.size());
-    for (size_t ci = 0; ci < j.channels.size(); ++ci) {
-      const ModularChannelTarget& c = j.channels[ci];
-      int nprev = 0;
-      for (size_t pj = 0; pj < ci; ++pj) {
-        const ModularChannelTarget& q = j.channels[pj];
-        if (q.view.w && q.view.h && q.view.w == c.view.w && q.view.h == c.view.h && q.hshift == c.hshift && q.vshift == c.vshift) ++nprev;
-      }
-      nprevs[ci] = nprev = std::min(nprev, 16);
-      if (!compact) continue;
-      auto any = channel_trees.find({j.tree, uint32_t(ci), nprev, -1});
-      if (any == channel_trees.end()) any = channel_trees.find({j.tree, uint32_t(ci), nprev, int64_t(j.stream_index)});
-      if (any == channel_trees.end()) {
-        auto ct = std::make_unique<ChannelTree>();
-        if (!build_channel_tree(*j.tree, uint32_t(ci), j.stream_index, nprev, ct.get())) {
-          compact = false;
-          continue;
-        }
-        const int64_t skey = ct->stream_dependent ? int64_t(j.stream_index) : -1;
-        any = channel_trees.emplace(std::make_tuple(j.tree, uint32_t(ci), nprev, skey), std::move(ct)).first;
-      }
-      // Channels whose reachable subtrees are identical node for node (a tree that never tests the channel index, e.g.
-      // a Squeeze image's 36 global channels under one weighted-predictor chain) share one staged copy: the first
-      // channel tree with that content stands for all of them.
-      const ChannelTree* canon = any->second.get();
-      for (const ChannelTree* prev : key)
-        if (prev != canon && prev->lut_prop == canon->lut_prop && prev->lut_base == canon->lut_base && prev->lut == canon->lut &&
-            prev->nodes.size() == canon->nodes.size() &&
-            std::memcmp(prev->nodes.data(), canon->nodes.data(), canon->nodes.size() * sizeof(MaNode)) == 0) {
-          canon = prev;
-          break;
-        }
-      key.push_back(canon);
-    }
-    if (compact) {
-      auto jt = job_tables.find(key);
-      if (jt == job_tables.end()) {
-        JobTables t;
-        std::vector<MaNode> nodes;
-        std::vector<uint16_t> luts;
-        t.wp = false;
-        std::map<const ChannelTree*, DevChannelPlan> seen;  // channels that reach the same subtree share its copy
-        for (const ChannelTree* ct : key) {
-          auto dup = seen.find(ct);
-          if (dup != seen.end()) {
-            t.plans.push_back(dup->second);
-            continue;
-          }
-          const uint32_t base = uint32_t(nodes.size());
-          DevChannelPlan plan;
-          plan.root = base;
-          plan.lut_prop = -1;
-          plan.lut_base = 0;
-          plan.lut_len = 0;
-          plan.lut_offset = uint32_t(luts.size());
-          for (MaNode n : ct->nodes) {
-            if (n.property >= 0) {
-              n.a += base;
-              n.b += base;
-              if (n.property == 15) t.wp = true;
-            } else if ((n.a & 0xff) == 6) {
-              t.wp = true;
-            }
-            nodes.push_back(n);
-          }
-          if (ct->lut_prop >= 0 && nodes.size() <= 65536) {
-            plan.lut_prop = ct->lut_prop;
-            plan.lut_base = ct->lut_base;
-            plan.lut_len = uint32_t(ct->lut.size());
-            for (uint16_t l : ct->lut) luts.push_back(uint16_t(l + base));
-          }
-          t.plans.push_back(plan);
-          seen.emplace(ct, plan);
-        }
-        t.num_nodes = uint32_t(nodes.size());
-        t.lut_total = uint32_t(luts.size());
-        luts.push_back(0);
-        luts.push_back(0);
-        t.nodes = static_cast<const MaNode*>(upload_temp(nodes.data(), nodes.size() * sizeof(MaNode)));
-        t.luts = static_cast<const uint16_t*>(upload_temp(luts.data(), luts.size() * 2));
-        jt = job_tables.emplace(key, std::move(t)).first;
-      }
-      const JobTables& t = jt->second;
-      d.tree = t.nodes;
-      d.num_tree_nodes = t.num_nodes;
-      d.luts = t.luts;
-      d.lut_total = t.lut_total;
-      d.use_wp = t.wp ? 1 : 0;
-      dplans.insert(dplans.end(), t.plans.begin(), t.plans.end());
-    } else {  // a channel's subtree is too large to copy per job: walk the frame's tree in global memory
-      TreeDev& td = it->second;
-      if (!td.nodes) {
-        td.nodes = static_cast<const MaNode*>(upload_temp(j.tree->nodes.data(), j.tree->nodes.size() * sizeof(MaNode)));
-        td.wp = tree_uses_wp(*j.tree);
-      }
-      d.tree = td.nodes;
-      d.num_tree_nodes = uint32_t(j.tree->nodes.size());
-      d.use_wp = td.wp ? 1 : 0;
-      std::vector<uint16_t> luts;
-      for (size_t ci = 0; ci < j.channels.size(); ++ci)
-        dplans.push_back(build_channel_plan(*j.tree, uint32_t(ci), j.stream_index, nprevs[ci], &luts));
-      d.lut_total = uint32_t(luts.size());
-      luts.push_back(0);
-      luts.push_back(0);
-      d.luts = static_cast<const uint16_t*>(upload_temp(luts.data(), luts.size() * 2));
-    }
-    max_smem = std::max(max_smem, modular_job_smem_bytes(d, max_w));
-    all_staged = all_staged && modular_job_all_staged(d, max_w);
-    if (d.use_wp && max_w) {
-      d.wp_scratch = static_cast<int32_t*>(dmalloc(size_t(max_w) * 5 * 4));
-      temps_.push_back(d.wp_scratch);
-    }
-    if (d.code.lz77_enabled) {
-      size_t n = size_t(std::min<uint64_t>(1u << 20, std::max<uint64_t>(samples, 1)));
-      d.lz_window = static_cast<uint32_t*>(dmalloc(n * 4));
-      temps_.push_back(d.lz_window);
-    }
+    const ModularLaunch::JobNeeds& n = L.needs[i];
+    if (n.wp_scratch_bytes) temps_.push_back(L.jobs[i].wp_scratch = static_cast<int32_t*>(dmalloc(n.wp_scratch_bytes)));
+    if (n.lz_window_bytes) temps_.push_back(L.jobs[i].lz_window = static_cast<uint32_t*>(dmalloc(n.lz_window_bytes)));
   }
-  const DevModularJob* d_jobs = static_cast<const DevModularJob*>(upload_temp(djobs.data(), djobs.size() * sizeof(DevModularJob)));
-  const DevChannel* d_chans = static_cast<const DevChannel*>(upload_temp(dchans.data(), dchans.size() * sizeof(DevChannel)));
+  const DevModularJob* d_jobs = static_cast<const DevModularJob*>(upload_temp(L.jobs.data(), L.jobs.size() * sizeof(DevModularJob)));
+  const DevChannel* d_chans = static_cast<const DevChannel*>(upload_temp(L.channels.data(), L.channels.size() * sizeof(DevChannel)));
   uint64_t* d_end = static_cast<uint64_t*>(stage_scratch(jobs.size() * 8));
   int* d_status = static_cast<int*>(stage_scratch(jobs.size() * 4));
-  const DevChannelPlan* d_plans = static_cast<const DevChannelPlan*>(upload_temp(dplans.data(), dplans.size() * sizeof(DevChannelPlan)));
+  const DevChannelPlan* d_plans = static_cast<const DevChannelPlan*>(upload_temp(L.plans.data(), L.plans.size() * sizeof(DevChannelPlan)));
   unsigned long long* d_trace = nullptr;
   double host_launch = 0.0;
   if (trace_device) {
@@ -883,8 +607,8 @@ void CudaBackend::decode_modular(std::vector<ModularStreamJob>& jobs) {
     item.ref.end_bits = d_end;
     item.ref.status = d_status;
     item.num_jobs = int(jobs.size());
-    item.smem_bytes = max_smem;
-    item.all_staged = all_staged;
+    item.smem_bytes = L.smem_bytes;
+    item.all_staged = L.all_staged;
     uint8_t* h_end = h_result_;
     uint8_t* h_status = h_result_ + ((jobs.size() * 8 + 15) & ~size_t(15));
     JXLB_CHECK(size_t(h_status - h_result_) + jobs.size() * 4 <= result_cap_, kErrUnsupported, "too many stream jobs in one launch for the result buffer");
@@ -917,7 +641,7 @@ void CudaBackend::decode_modular(std::vector<ModularStreamJob>& jobs) {
     status = reinterpret_cast<const int*>(h_status);
   } else {
     begin_k("modular_decode");
-    launch_modular_decode(active_cs_, d_jobs, d_chans, d_plans, d_end, d_status, int(jobs.size()), max_smem, all_staged, S(), d_trace);
+    launch_modular_decode(active_cs_, d_jobs, d_chans, d_plans, d_end, d_status, int(jobs.size()), L.smem_bytes, L.all_staged, S(), d_trace);
     end_k();
     end = static_cast<const uint64_t*>(fetch_result(d_end, jobs.size() * 8));
     status = static_cast<const int*>(fetch_result(d_status, jobs.size() * 4));
@@ -1012,8 +736,7 @@ void CudaBackend::palette_inverse(const View& palette, const std::vector<View>& 
     for (size_t i = 0; i < targets.size(); ++i) p.target[i] = tv[i];
     p.mask = d_mask;
     p.d_pred = t.d_pred;
-    const uint32_t hdr[11] = {wph.p1, wph.p2, wph.p3a, wph.p3b, wph.p3c, wph.p3d, wph.p3e, wph.w[0], wph.w[1], wph.w[2], wph.w[3]};
-    for (int i = 0; i < 11; ++i) p.wp[i] = hdr[i];
+    pack_wp(wph, p.wp);
     int32_t* rows = nullptr;
     if (t.d_pred == 6) rows = static_cast<int32_t*>(dmalloc(targets.size() * ((5 * size_t(w) + 3) & ~size_t(3)) * 4));
     p.wp_rows = rows;
@@ -1037,32 +760,6 @@ void CudaBackend::modular_xyb_to_float(const View yxb[3], const float m[3]) {
   begin_k("modular_xyb");
   launch_modular_xyb(dev_view(yxb[0]), dev_view(yxb[1]), dev_view(yxb[2]), m[0], m[1], m[2], S());
   end_k();
-}
-
-DevFrame CudaBackend::dev_frame(const VarDctState& st) const {
-  DevFrame f;
-  f.width = st.width;
-  f.height = st.height;
-  f.bw = st.bw;
-  f.bh = st.bh;
-  f.cw = st.bw * 8;
-  f.ch = st.bh * 8;
-  f.w64 = (st.width + 63) / 64;
-  for (int c = 0; c < 3; ++c) {
-    f.lf_quant[c] = static_cast<int32_t*>(plane_ptr(st.lf_quant[c]));
-    f.lf[c] = static_cast<float*>(plane_ptr(st.lf[c]));
-    f.coeff[c] = static_cast<uint32_t*>(plane_ptr(st.coeff[c]));
-  }
-  f.x_from_y = static_cast<int32_t*>(plane_ptr(st.x_from_y));
-  f.b_from_y = static_cast<int32_t*>(plane_ptr(st.b_from_y));
-  f.sharpness = static_cast<int32_t*>(plane_ptr(st.sharpness));
-  f.blk_type = static_cast<int32_t*>(plane_ptr(st.blk_type));
-  f.blk_mul = static_cast<int32_t*>(plane_ptr(st.blk_mul));
-  f.epf_sigma = static_cast<float*>(plane_ptr(st.epf_sigma));
-  f.group_blocks = st.group_dim / 8;
-  for (int c = 0; c < 3; ++c) f.hshift[c] = uint8_t(st.hshift[c]), f.vshift[c] = uint8_t(st.vshift[c]);
-  f.subsampled = st.subsampled ? 1 : 0;
-  return f;
 }
 
 void CudaBackend::build_block_info(VarDctState& st, const std::vector<BlockInfoJob>& jobs) {
@@ -1092,68 +789,17 @@ void CudaBackend::build_block_info(VarDctState& st, const std::vector<BlockInfoJ
 
 void CudaBackend::decode_hf(VarDctState& st, std::vector<HfGroupJob>& jobs) {
   if (jobs.empty()) return;
-  const HfBlockContext& hbc = st.lfg->hf_block_ctx;
   const uint32_t pass = jobs[0].pass_idx;
   const HfPassSyntax& hp = st.hfg->passes[pass];
   // The coefficient kernels read plain hybrid-uint tokens; an LZ77-enabled HF code (legal, hf_coeff.rs:181-222 goes
   // through read_varint_with_multiplier_clustered, but no known encoder emits it) would decode silently wrong.
   const bool hf_lz77 = hp.code.lz77_enabled;  // reported after the launch: a stream that is invalid anyway keeps its own error
-  DevHfParams p;
-  std::memset(&p, 0, sizeof(p));
-  p.code = upload_code(hp.code);
-  // orders: natural (static) unless the pass carries a custom permutation
-  std::vector<uint32_t> custom;
-  bool any_custom = false;
-  for (int id = 0; id < 13; ++id)
-    for (int c = 0; c < 3; ++c) any_custom |= !hp.order[id][c].empty();
-  if (!any_custom) {
-    p.orders = d_natural_orders_;
-    for (int id = 0; id < 13; ++id)
-      for (int c = 0; c < 3; ++c) p.order_offset[id * 3 + c] = natural_order_offset_[id];
-  } else {
-    for (int id = 0; id < 13; ++id)
-      for (int c = 0; c < 3; ++c) {
-        p.order_offset[id * 3 + c] = uint32_t(custom.size());
-        if (hp.order[id][c].empty()) {
-          std::vector<uint32_t> o = natural_order(uint32_t(id));
-          custom.insert(custom.end(), o.begin(), o.end());
-        } else {
-          custom.insert(custom.end(), hp.order[id][c].begin(), hp.order[id][c].end());
-        }
-      }
-    p.orders = static_cast<const uint32_t*>(upload_temp(custom.data(), custom.size() * 4));
-  }
-  p.block_ctx_map = static_cast<const uint8_t*>(upload_temp(hbc.block_ctx_map.data(), hbc.block_ctx_map.size()));
-  p.block_ctx_map_size = uint32_t(hbc.block_ctx_map.size());
+  DevHfParams p = build_hf_params(st, pass, *this, d_natural_orders_, natural_order_offset_);
   {
     const char* lim = std::getenv("JXLB_HF_ANS_SMEM");  // tuning knob (bytes); default: stage up to 128 KB
     p.ans_smem_limit = lim ? uint32_t(std::atoi(lim)) : 128u * 1024u;
   }
-  std::vector<int32_t> thr;
-  for (int c = 0; c < 3; ++c) {
-    p.num_lf_thr[c] = uint32_t(hbc.lf_thresholds[c].size());
-    thr.insert(thr.end(), hbc.lf_thresholds[c].begin(), hbc.lf_thresholds[c].end());
-  }
-  thr.push_back(0);
-  p.lf_thresholds = static_cast<const int32_t*>(upload_temp(thr.data(), thr.size() * 4));
-  p.has_lf_quant = st.use_lf_frame ? 0 : 1;
-  std::vector<uint32_t> qf = hbc.qf_thresholds;
-  p.num_qf_thr = uint32_t(qf.size());
-  qf.push_back(0);
-  p.qf_thresholds = static_cast<const uint32_t*>(upload_temp(qf.data(), qf.size() * 4));
-  p.num_block_clusters = hbc.num_block_clusters;
-  p.num_hf_presets = st.hfg->num_hf_presets;
-  p.coeff_shift = pass < st.fh->passes.shift.size() ? st.fh->passes.shift[pass] : 0;
-  p.group_dim_blocks = st.group_dim / 8;
-  p.groups_per_row = st.groups_per_row;
-  // Thread-per-stream kernel: streams of similar length share a warp (longest first), so that a warp's lanes
-  // finish together; `perm` maps the launch order back to `jobs`.
-  std::vector<uint32_t> perm(jobs.size());
-  for (size_t i = 0; i < jobs.size(); ++i) perm[i] = uint32_t(i);
-  if (hf_streams_per_cta >= 64)
-    std::stable_sort(perm.begin(), perm.end(), [&](uint32_t a, uint32_t b) {
-      return jobs[a].bit_limit - jobs[a].bit_pos > jobs[b].bit_limit - jobs[b].bit_pos;
-    });
+  const std::vector<uint32_t> perm = hf_launch_order(jobs, hf_streams_per_cta >= 64);  // launch order -> `jobs`
   std::vector<DevHfJob> dj;
   for (uint32_t i : perm) dj.push_back({jobs[i].bit_pos, jobs[i].bit_limit, jobs[i].group_idx});
   const DevHfJob* d_jobs = static_cast<const DevHfJob*>(upload_temp(dj.data(), dj.size() * sizeof(DevHfJob)));
@@ -1363,39 +1009,16 @@ bool CudaBackend::filters_colour_fused(const View v[3], const RestorationFilter&
     out[c] = in[c];
     out[c].ptr = out_ptr[c];
   }
-  DevFusedFilterParams p;
-  std::memset(&p, 0, sizeof(p));
-  p.gab_enabled = rf.gab_enabled ? 1 : 0;
-  for (int c = 0; c < 3; ++c) {
-    p.gab_w[c][0] = rf.gab_weights[c][0];
-    p.gab_w[c][1] = rf.gab_weights[c][1];
-    p.epf.channel_scale[c] = rf.epf.channel_scale[c];
-  }
-  p.epf_iters = int(rf.epf.iters);
-  p.epf.pass0_sigma_scale = rf.epf.pass0_sigma_scale;
-  p.epf.pass2_sigma_scale = rf.epf.pass2_sigma_scale;
-  p.epf.border_sad_mul = rf.epf.border_sad_mul;
-  p.epf.sigma_for_modular = rf.epf.sigma_for_modular;
+  const float* d_sigma = nullptr;
+  uint32_t sigma_stride = 0;
   if (!sigma_is_constant && rf.epf.iters > 0) {
     const PlaneRec& s = planes_.at(sigma.plane);
-    p.sigma = static_cast<const float*>(s.ptr);
-    p.sigma_stride = s.w;
+    d_sigma = static_cast<const float*>(s.ptr);
+    sigma_stride = s.w;
   }
-  if (colour) {
-    p.colour = 1;
-    for (int i = 0; i < 3; ++i) {
-      p.col.opsin_bias[i] = colour->opsin_bias[i];
-      p.col.cbrt_opsin_bias[i] = colour->cbrt_opsin_bias[i];
-    }
-    p.col.itscale = colour->itscale;
-    for (int i = 0; i < 9; ++i) p.col.matrix[i] = colour->matrix[i];
-    p.col.apply_srgb_tf = colour->apply_srgb_tf ? 1 : 0;
-    p.col.apply_bt709_tf = colour->apply_bt709_tf ? 1 : 0;
-    JXLB_CHECK(!colour->second_stage && colour->gamma == 0.0f, kErrInvalidArg, "the fused filter kernel converts to sRGB-gamut targets only");
-    p.col.second_stage = p.col.to_luma = 0;
-    p.col.gamma = 0.0f;
-    p.col.pq_intensity_target = 0.0f;
-  }
+  JXLB_CHECK(!colour || (!colour->second_stage && colour->gamma == 0.0f), kErrInvalidArg,
+             "the fused filter kernel converts to sRGB-gamut targets only");
+  const DevFusedFilterParams p = fused_filter_params(rf, d_sigma, sigma_stride, colour);
   begin_k("filters_fused");
   if (!(debug_skip() & 4)) launch_filters_fused(in, out, p, S());
   end_k();

@@ -11,6 +11,7 @@
 
 #include "host/backend.h"
 #include "kernels/kernels.h"
+#include "launch_tables.h"
 
 namespace jxlb {
 
@@ -43,7 +44,7 @@ class LfBatchService {
 
 struct StopDecode {};  // thrown by stage_marker() when a stage entry point has what it asked for
 
-class CudaBackend : public Backend {
+class CudaBackend : public Backend, private TableSink {
  public:
   // own_stream = false: a pipeline decoder. It borrows the stream of a heavy slot (on_heavy_stage -> set_stream) and
   // runs its LF stage through `lf_service` without any stream.
@@ -151,10 +152,6 @@ class CudaBackend : public Backend {
     void* ptr;
     uint32_t w, h;
   };
-  struct DevTable {  // device copy of an EntropyCode
-    DevEntropyCode code;
-    std::vector<void*> allocs;
-  };
   void* dmalloc(size_t bytes);
   void dfree(void* p);
   // Host tables for the next launch. They are gathered in a pinned staging block that mirrors a device block of the
@@ -163,13 +160,15 @@ class CudaBackend : public Backend {
   // calls, each taking the driver's context lock that every other decoder thread of the process wants too. The block is
   // recycled at every sync(). Oversized requests fall back to a pool allocation + direct copy (freed by release_temps).
   void* upload_temp(const void* src, size_t bytes);
+  const void* put(const void* src, size_t bytes) override { return upload_temp(src, bytes); }  // launch tables
   void* stage_scratch(size_t bytes);  // device scratch from the same block (no host data), zeroed by nobody
   void flush_uploads();
   void release_temps();
   // results of a stage (end positions, status words): device -> pinned host, readable after the next sync()
   void* fetch_result(const void* dsrc, size_t bytes);
-  DevEntropyCode upload_code(const EntropyCode& c);
-  DevFrame dev_frame(const VarDctState& st) const;
+  DevFrame dev_frame(const VarDctState& st) const {
+    return make_dev_frame(st, [this](int id) { return plane_ptr(id); });
+  }
   void ensure_static_tables();
   void begin_k(const char* name);
   void end_k();
@@ -225,7 +224,6 @@ class CudaBackend : public Backend {
   std::map<int, PlaneRec> planes_;
   int next_id_ = 0;
   std::vector<void*> temps_;
-  std::vector<std::vector<uint8_t>> host_keep_;  // host staging kept alive until the next sync
   // static tables
   uint32_t* d_natural_orders_ = nullptr;
   uint32_t natural_order_offset_[13];

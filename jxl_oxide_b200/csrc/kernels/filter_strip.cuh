@@ -287,6 +287,9 @@ JXLB_FS void strip_xyb_px(float o[3], const DevColorParams& p, const float* pow_
 }
 static inline int strip_tf_of(const DevFusedFilterParams& p) {  // host side: which instantiation a frame needs
   return !p.colour ? 0 : (p.col.apply_srgb_tf ? 1 : (p.col.apply_bt709_tf ? 2 : 0)); }
+static inline void strip_gab_norm(const DevFusedFilterParams& p, float gw[3]) {  // host side: phase_gab's `gw` argument
+  for (int c = 0; c < 3; ++c) gw[c] = 1.0f / ((1.0f + p.gab_w[c][0] * 4.0f) + p.gab_w[c][1] * 4.0f);
+}
 
 // ---- phase 3: step-1 weighted sums, A + D -> B (the dead `in` planes) on [3, 61) x [3, 29); when step 1 is the frame's last
 // EPF step (LAST: epf_iters == 1) the output tile [4, 60) x [4, 28) goes through the colour stage to the output planes ----

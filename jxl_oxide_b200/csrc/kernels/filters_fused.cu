@@ -650,7 +650,7 @@ void launch_filters_fused(const DevView in[3], const DevView out[3], DevFusedFil
     }
     if (ok) {
       float gw[3];
-      for (int c = 0; c < 3; ++c) gw[c] = 1.0f / ((1.0f + p.gab_w[c][0] * 4.0f) + p.gab_w[c][1] * 4.0f);
+      fstrip::strip_gab_norm(p, gw);
       dim3 sgrid((r.x1 - r.x0 + fstrip::kTX - 1) / fstrip::kTX, (r.y1 - r.y0 + fstrip::kTY - 1) / fstrip::kTY);
       const int tf = fstrip::strip_tf_of(p);
       const size_t sm = fstrip::kSmemFloats * 4;

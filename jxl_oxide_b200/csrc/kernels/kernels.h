@@ -73,14 +73,11 @@ void launch_modular_decode(const uint8_t* codestream, const DevModularJob* jobs,
                            const DevChannelPlan* plans, uint64_t* end_bits, int* status, int num_jobs,
                            size_t smem_bytes, bool all_tables_staged, cudaStream_t stream,
                            unsigned long long* trace = nullptr);
-bool modular_job_all_staged(const DevModularJob& job, uint32_t max_width);
 void launch_signal_word(uint32_t* host_mapped_word, uint32_t value, cudaStream_t stream);
 void launch_modular_decode_batch(const DevModularBatchRef* refs, int total, size_t smem_bytes, bool all_tables_staged,
                                  cudaStream_t stream);
 // tracing aid: writes the device's %globaltimer (ns)
 void launch_read_globaltimer(unsigned long long* out, cudaStream_t stream);
-// bytes of dynamic shared memory a job wants for its tree / entropy tables / WP rows / LUTs
-size_t modular_job_smem_bytes(const DevModularJob& job, uint32_t max_width);
 void launch_squeeze_inverse(DevView avg, DevView res, DevView out, bool horizontal, cudaStream_t stream);
 // The channels of one Squeeze step in one launch (channels may differ in size; zero-sized outputs are skipped).
 void launch_squeeze_inverse_batch(const DevView* avg, const DevView* res, const DevView* out, int n, bool horizontal,

@@ -7,6 +7,7 @@
 #include <type_traits>
 
 #include "kernels.h"
+#include "modular_plan.cuh"
 #include "stream_common.cuh"
 
 // Test hooks of the host emulation (tests/emu/modular_emu.cc); no-ops in the kernel.
@@ -19,9 +20,6 @@
 
 namespace jxlb {
 namespace {
-
-constexpr uint32_t kFastChunk = 128;       // columns per warp-computed row prologue of the weighted-predictor fast loop
-constexpr uint32_t kFastMaxLeaves = 1024;  // a LUT spans at most 1024 property values (cuda_backend.cu)
 
 __device__ __forceinline__ uint32_t wp_weight32(const uint32_t* div, uint32_t err_sum, uint32_t maxweight) {
   const uint32_t t = (err_sum + 1) >> 5;

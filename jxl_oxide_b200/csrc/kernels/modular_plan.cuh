@@ -1,6 +1,6 @@
-// Host-built per-channel plans of the Modular stream kernel (modular_stream.cu) for a frame's whole MA tree: the
-// fallback when a channel's reachable subtree is too large to compact (cuda_backend.cu), and the plans the host
-// emulation in tests/emu/ runs the kernel's per-stream code with.
+// What the host has to know about the Modular stream kernel (modular_stream.cu) to build its launch tables
+// (launch_tables.cc): the shared-memory layout of a job, whether a launch stages every table, and the per-channel plans
+// for a frame's whole MA tree (the fallback when a channel's reachable subtree is too large to compact).
 #pragma once
 #include <algorithm>
 #include <cstdint>
@@ -10,17 +10,86 @@
 
 namespace jxlb {
 
+constexpr uint32_t kFastChunk = 128;       // columns per warp-computed row prologue of the weighted-predictor fast loop
+constexpr uint32_t kFastMaxLeaves = 1024;  // a LUT spans at most 1024 property values (launch_tables.cc)
+
+constexpr uint32_t kSmemTreeBytes = 64 * 1024;
+constexpr uint32_t kSmemAnsBytes = 48 * 1024;
+constexpr uint32_t kSmemPrefixBytes = 24 * 1024;
+constexpr uint32_t kSmemLutBytes = 8 * 1024;
+constexpr uint32_t kSmemWpMaxWidth = 1024;
+
+struct SmemLayout {
+  uint32_t tree, ans, prefix, prefix_meta, configs, luts, wp, div, fast_pro, fast_leaves, fast_rows, total;
+};
+
+__host__ __device__ inline SmemLayout modular_layout(uint32_t num_nodes, const DevEntropyCode& code, uint32_t lut_total,
+                                                      uint32_t use_wp, uint32_t max_w) {
+  SmemLayout L;
+  uint32_t off = 0;
+  auto take = [&](uint32_t bytes) {
+    uint32_t o = off;
+    off += (bytes + 15) & ~15u;
+    return o;
+  };
+  L.div = take(65 * 4);
+  uint32_t tree_bytes = num_nodes * 16;
+  L.tree = tree_bytes <= kSmemTreeBytes ? take(tree_bytes) : 0xffffffffu;
+  L.configs = take(code.num_clusters * 4);
+  if (code.use_prefix) {
+    L.ans = 0xffffffffu;
+    uint32_t pb = code.prefix_table_size * 4;
+    L.prefix = pb <= kSmemPrefixBytes ? take(pb) : 0xffffffffu;
+    L.prefix_meta = take(code.num_clusters * 8);
+  } else {
+    uint32_t ab = (code.num_clusters << code.log_alphabet_size) * 8;
+    L.ans = (ab <= kSmemAnsBytes) ? take(ab) : 0xffffffffu;
+    L.prefix = 0xffffffffu;
+    L.prefix_meta = 0xffffffffu;
+  }
+  uint32_t lb = lut_total * 2;
+  L.luts = lb <= kSmemLutBytes ? take(lb + 4) : 0xffffffffu;
+  L.wp = (use_wp && max_w <= kSmemWpMaxWidth) ? take(max_w * 5 * 4) : 0xffffffffu;
+  // weighted-predictor fast loop: row prologue (4 x int4 per column), packed leaves, second pair of error rows
+  L.fast_pro = L.fast_leaves = L.fast_rows = 0xffffffffu;
+  if (L.wp != 0xffffffffu) {
+    L.fast_pro = take(kFastChunk * 64);
+    L.fast_leaves = take((lut_total < kFastMaxLeaves ? lut_total : kFastMaxLeaves) * 16);
+    L.fast_rows = take(max_w * 5 * 4);
+  }
+  L.total = off;
+  return L;
+}
+
+// bytes of dynamic shared memory a job wants for its tree / entropy tables / WP rows / LUTs
+inline size_t modular_job_smem_bytes(const DevModularJob& job, uint32_t max_width) {
+  return modular_layout(job.num_tree_nodes, job.code, job.lut_total, job.use_wp, max_width).total;
+}
+
+// Whether modular_stream_kernel stages every table of this job (tree, entropy tables, leaf LUTs, predictor rows).
+inline bool modular_job_all_staged(const DevModularJob& job, uint32_t max_width) {
+  const SmemLayout L = modular_layout(job.num_tree_nodes, job.code, job.lut_total, job.use_wp, max_width);
+  if (L.tree == 0xffffffffu || L.luts == 0xffffffffu) return false;
+  if (job.code.use_prefix ? L.prefix == 0xffffffffu : L.ans == 0xffffffffu) return false;
+  if (job.use_wp && L.wp == 0xffffffffu) return false;
+  return !job.code.lz77_enabled;
+}
+
 // Resolves the MA-tree nodes that test properties which are constant for a whole channel
 // (channel index, stream index, previous channels that do not exist), like
-// MaTreeNode::next_decision_node (crates/jxl-modular/src/ma.rs:424-470).
-inline uint32_t resolve_static(const MaTree& t, uint32_t idx, uint32_t ci, uint32_t stream, int nprev) {
+// MaTreeNode::next_decision_node (crates/jxl-modular/src/ma.rs:424-470). Sets *stream_dependent when
+// a stream-index test was taken.
+inline uint32_t resolve_static(const MaTree& t, uint32_t idx, uint32_t ci, uint32_t stream, int nprev,
+                               bool* stream_dependent = nullptr) {
   for (;;) {
     const MaNode& n = t.nodes[idx];
     if (n.property < 0) return idx;
     int32_t v;
     if (n.property == 0) v = int32_t(ci);
-    else if (n.property == 1) v = int32_t(stream);
-    else if (n.property >= 16 && (n.property - 16) / 4 >= nprev) v = 0;
+    else if (n.property == 1) {
+      v = int32_t(stream);
+      if (stream_dependent) *stream_dependent = true;
+    } else if (n.property >= 16 && (n.property - 16) / 4 >= nprev) v = 0;
     else return idx;
     idx = v > n.value ? n.a : n.b;
   }

@@ -22,54 +22,6 @@ namespace jxlb {
 
 namespace {
 
-constexpr uint32_t kSmemTreeBytes = 64 * 1024;
-constexpr uint32_t kSmemAnsBytes = 48 * 1024;
-constexpr uint32_t kSmemPrefixBytes = 24 * 1024;
-constexpr uint32_t kSmemLutBytes = 8 * 1024;
-constexpr uint32_t kSmemWpMaxWidth = 1024;
-
-struct SmemLayout {
-  uint32_t tree, ans, prefix, prefix_meta, configs, luts, wp, div, fast_pro, fast_leaves, fast_rows, total;
-};
-
-__host__ __device__ inline SmemLayout modular_layout(uint32_t num_nodes, const DevEntropyCode& code, uint32_t lut_total,
-                                                      uint32_t use_wp, uint32_t max_w) {
-  SmemLayout L;
-  uint32_t off = 0;
-  auto take = [&](uint32_t bytes) {
-    uint32_t o = off;
-    off += (bytes + 15) & ~15u;
-    return o;
-  };
-  L.div = take(65 * 4);
-  uint32_t tree_bytes = num_nodes * 16;
-  L.tree = tree_bytes <= kSmemTreeBytes ? take(tree_bytes) : 0xffffffffu;
-  L.configs = take(code.num_clusters * 4);
-  if (code.use_prefix) {
-    L.ans = 0xffffffffu;
-    uint32_t pb = code.prefix_table_size * 4;
-    L.prefix = pb <= kSmemPrefixBytes ? take(pb) : 0xffffffffu;
-    L.prefix_meta = take(code.num_clusters * 8);
-  } else {
-    uint32_t ab = (code.num_clusters << code.log_alphabet_size) * 8;
-    L.ans = (ab <= kSmemAnsBytes) ? take(ab) : 0xffffffffu;
-    L.prefix = 0xffffffffu;
-    L.prefix_meta = 0xffffffffu;
-  }
-  uint32_t lb = lut_total * 2;
-  L.luts = lb <= kSmemLutBytes ? take(lb + 4) : 0xffffffffu;
-  L.wp = (use_wp && max_w <= kSmemWpMaxWidth) ? take(max_w * 5 * 4) : 0xffffffffu;
-  // weighted-predictor fast loop: row prologue (4 x int4 per column), packed leaves, second pair of error rows
-  L.fast_pro = L.fast_leaves = L.fast_rows = 0xffffffffu;
-  if (L.wp != 0xffffffffu) {
-    L.fast_pro = take(kFastChunk * 64);
-    L.fast_leaves = take((lut_total < kFastMaxLeaves ? lut_total : kFastMaxLeaves) * 16);
-    L.fast_rows = take(max_w * 5 * 4);
-  }
-  L.total = off;
-  return L;
-}
-
 // The execution policy of decode_stream_channels on the device: the 32 lanes of the stream's warp.
 struct DeviceWarp {
   static constexpr uint32_t kLanes = 32;
@@ -281,10 +233,6 @@ void launch_palette_delta(DevPaletteDeltaParams p, int num_c, cudaStream_t strea
   palette_delta_kernel<<<num_c, 32, 0, stream>>>(p);
 }
 
-size_t modular_job_smem_bytes(const DevModularJob& job, uint32_t max_width) {
-  return modular_layout(job.num_tree_nodes, job.code, job.lut_total, job.use_wp, max_width).total;
-}
-
 void launch_modular_decode(const uint8_t* cs, const DevModularJob* jobs, const DevChannel* channels,
                            const DevChannelPlan* plans, uint64_t* end_bits, int* status, int num_jobs, size_t smem_bytes,
                            bool all_tables_staged, cudaStream_t stream, unsigned long long* trace) {
@@ -314,15 +262,6 @@ void launch_modular_decode_batch(const DevModularBatchRef* refs, int total, size
   (void)attr_set;
   if (all_tables_staged) modular_stream_batch_kernel<true><<<total, 32, smem_bytes, stream>>>(refs, total);
   else modular_stream_batch_kernel<false><<<total, 32, smem_bytes, stream>>>(refs, total);
-}
-
-// Whether modular_stream_kernel stages every table of this job (tree, entropy tables, leaf LUTs, predictor rows).
-bool modular_job_all_staged(const DevModularJob& job, uint32_t max_width) {
-  const SmemLayout L = modular_layout(job.num_tree_nodes, job.code, job.lut_total, job.use_wp, max_width);
-  if (L.tree == 0xffffffffu || L.luts == 0xffffffffu) return false;
-  if (job.code.use_prefix ? L.prefix == 0xffffffffu : L.ans == 0xffffffffu) return false;
-  if (job.use_wp && L.wp == 0xffffffffu) return false;
-  return !job.code.lz77_enabled;
 }
 
 void launch_signal_word(uint32_t* host_mapped_word, uint32_t value, cudaStream_t stream) {

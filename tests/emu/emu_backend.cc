@@ -1,8 +1,8 @@
 // TEST INFRASTRUCTURE — NOT PART OF THE PRODUCT.
 //
 // Host emulation of the thread-per-stream HF coefficient kernel (kernels/hf_lanes.cuh). The oracle backend
-// is reused for everything else; decode_hf() builds the same DevFrame / DevHfParams / job list the CUDA
-// backend uploads (cuda_backend.cu: dev_frame, upload_code, decode_hf) but over host memory, and then runs
+// is reused for everything else; decode_hf() builds its DevFrame, DevHfParams and launch order with the CUDA
+// backend's own code (launch_tables.cc), over host memory and the same natural-order table, and then runs
 // hf_lane_decode() -- the very function every device thread runs -- once per stream, with the interleaved
 // non-zero-row layout of a 32-thread CTA. tests/test_emu_lanes.py compares the resulting coefficient planes,
 // end positions and final pixels with the plain oracle.
@@ -25,6 +25,7 @@ inline void emu_trip(bool is_coefficient) {
 #include "../../jxl_oxide_b200/csrc/kernels/filter_strip.cuh"
 #include "../../oracle/oracle_backend.h"
 #include "../../jxl_oxide_b200/csrc/host/planner.h"
+#include "host_sink.h"
 
 namespace {
 // strip filter emulation: [0] frames that took the path, [1] pixels compared, [2] pixels that differ from the oracle's stages
@@ -116,7 +117,7 @@ namespace jxlo {
 
 class EmuBackend : public OracleBackend {
  public:
-  explicit EmuBackend(int threads) : OracleBackend(threads) {}
+  explicit EmuBackend(int threads) : OracleBackend(threads), natural_orders_(natural_order_table(natural_offset_)) {}
   void set_codestream(const uint8_t* data, size_t size) override {
     OracleBackend::set_codestream(data, size);
     // the device copy is zero padded (the word-ahead bit reader touches up to 3 words past the last bit)
@@ -129,83 +130,18 @@ class EmuBackend : public OracleBackend {
 
  private:
   std::vector<uint64_t> storage_;  // 8-byte aligned
+  uint32_t natural_offset_[13];
+  std::vector<uint32_t> natural_orders_;  // the device-resident natural-order table
 };
-
-namespace {
-template <typename T>
-T* pl(OracleBackend& be, int id) {
-  return id < 0 ? nullptr : reinterpret_cast<T*>(be.plane(id).data.data());
-}
-}  // namespace
 
 void EmuBackend::decode_hf(VarDctState& st, std::vector<HfGroupJob>& jobs) {
   if (jobs.empty()) return;
   const uint8_t* cs = reinterpret_cast<const uint8_t*>(storage_.data());
-  DevFrame f;
-  std::memset(&f, 0, sizeof(f));
-  f.width = st.width, f.height = st.height, f.bw = st.bw, f.bh = st.bh;
-  f.cw = st.bw * 8, f.ch = st.bh * 8;
-  f.w64 = (st.width + 63) / 64;
-  for (int c = 0; c < 3; ++c) {
-    f.lf_quant[c] = pl<int32_t>(*this, st.lf_quant[c]);
-    f.coeff[c] = pl<uint32_t>(*this, st.coeff[c]);
-    f.hshift[c] = uint8_t(st.hshift[c]), f.vshift[c] = uint8_t(st.vshift[c]);
-  }
-  f.blk_type = pl<int32_t>(*this, st.blk_type);
-  f.blk_mul = pl<int32_t>(*this, st.blk_mul);
-  f.group_blocks = st.group_dim / 8;
-  f.subsampled = st.subsampled ? 1 : 0;
-
-  const HfBlockContext& hbc = st.lfg->hf_block_ctx;
+  const DevFrame f = make_dev_frame(st, [this](int id) -> void* { return id < 0 ? nullptr : plane(id).data.data(); });
   const uint32_t pass = jobs[0].pass_idx;
-  const HfPassSyntax& hp = st.hfg->passes[pass];
-  const EntropyCode& code = hp.code;
-  DevHfParams p;
-  std::memset(&p, 0, sizeof(p));
-  std::vector<uint32_t> cfg;
-  for (const HybridUintConfig& h : code.configs) cfg.push_back(h.packed());
-  std::vector<uint32_t> meta;
-  for (const PrefixMeta& m : code.prefix_meta) {
-    meta.push_back(m.table_offset);
-    meta.push_back(m.root_bits);
-  }
-  p.code.cluster_map = code.cluster_map.data();
-  p.code.configs = cfg.data();
-  p.code.log_alphabet_size = code.log_alphabet_size;
-  p.code.use_prefix = code.use_prefix ? 1 : 0;
-  if (std::getenv("JXLE_TRACE")) std::fprintf(stderr, "[emu] decode_hf pass %u: %zu streams, %s, %u clusters, %u presets, subsampled %d\n", pass, jobs.size(), code.use_prefix ? "prefix" : "ANS", code.num_clusters, st.hfg->num_hf_presets, int(st.subsampled));
-  p.code.num_clusters = code.num_clusters;
-  p.code.cluster_map_size = uint32_t(code.cluster_map.size());
-  p.code.prefix = code.prefix_table.data();
-  p.code.prefix_meta = meta.data();
-  p.code.ans = code.ans_table.data();
-  std::vector<uint32_t> orders;
-  for (int id = 0; id < 13; ++id)
-    for (int c = 0; c < 3; ++c) {
-      p.order_offset[id * 3 + c] = uint32_t(orders.size());
-      std::vector<uint32_t> o = hp.order[id][c].empty() ? natural_order(uint32_t(id)) : hp.order[id][c];
-      orders.insert(orders.end(), o.begin(), o.end());
-    }
-  p.orders = orders.data();
-  p.block_ctx_map = hbc.block_ctx_map.data();
-  p.block_ctx_map_size = uint32_t(hbc.block_ctx_map.size());
-  std::vector<int32_t> thr;
-  for (int c = 0; c < 3; ++c) {
-    p.num_lf_thr[c] = uint32_t(hbc.lf_thresholds[c].size());
-    thr.insert(thr.end(), hbc.lf_thresholds[c].begin(), hbc.lf_thresholds[c].end());
-  }
-  thr.push_back(0);
-  p.lf_thresholds = thr.data();
-  p.has_lf_quant = st.use_lf_frame ? 0 : 1;
-  std::vector<uint32_t> qf = hbc.qf_thresholds;
-  p.num_qf_thr = uint32_t(qf.size());
-  qf.push_back(0);
-  p.qf_thresholds = qf.data();
-  p.num_block_clusters = hbc.num_block_clusters;
-  p.num_hf_presets = st.hfg->num_hf_presets;
-  p.coeff_shift = pass < st.fh->passes.shift.size() ? st.fh->passes.shift[pass] : 0;
-  p.group_dim_blocks = st.group_dim / 8;
-  p.groups_per_row = st.groups_per_row;
+  HostTableSink sink;
+  const DevHfParams p = build_hf_params(st, pass, sink, natural_orders_.data(), natural_offset_);
+  if (std::getenv("JXLE_TRACE")) std::fprintf(stderr, "[emu] decode_hf pass %u: %zu streams, %s, %u clusters, %u presets, subsampled %d\n", pass, jobs.size(), p.code.use_prefix ? "prefix" : "ANS", p.code.num_clusters, st.hfg->num_hf_presets, int(st.subsampled));
 
   // "shared memory" tables of one CTA
   uint8_t ctx[128] = {0};
@@ -219,23 +155,18 @@ void EmuBackend::decode_hf(VarDctState& st, std::vector<HfGroupJob>& jobs) {
   T.tinfo = tinfo;
   T.order_offset = p.order_offset;
   T.ctx = ctx;
-  T.cfg = cfg.data();
+  T.cfg = p.code.configs;
   T.bctx = p.block_ctx_map;
   T.cmap = p.code.cluster_map;
   T.cmap_stride = 495 * p.num_block_clusters;
-  T.cv.configs = cfg.data();
+  T.cv.configs = p.code.configs;
   T.cv.ans = p.code.ans;
   T.cv.prefix = p.code.prefix;
   T.cv.prefix_meta = p.code.prefix_meta;
   T.cv.log_alphabet_size = p.code.log_alphabet_size;
   T.cv.use_prefix = p.code.use_prefix;
 
-  // launch order of the CUDA backend: longest section first
-  std::vector<uint32_t> perm(jobs.size());
-  for (size_t i = 0; i < jobs.size(); ++i) perm[i] = uint32_t(i);
-  std::stable_sort(perm.begin(), perm.end(), [&](uint32_t a, uint32_t b) {
-    return jobs[a].bit_limit - jobs[a].bit_pos > jobs[b].bit_limit - jobs[b].bit_pos;
-  });
+  const std::vector<uint32_t> perm = hf_launch_order(jobs, true);
   // the pre-pass kernel: one "thread" per 8x8 cell
   std::vector<uint32_t> blk_ctx(size_t(f.bw) * f.bh);
   for (uint32_t by = 0; by < f.bh; ++by)
@@ -354,34 +285,10 @@ bool EmuBackend::filters_colour_fused(const View v[3], const RestorationFilter& 
   for (int c = 0; c < 3; ++c)
     if (v[c].x0 != 0 || v[c].y0 != 0 || int(v[c].w) != width || int(v[c].h) != height) return false;
 
-  DevFusedFilterParams p;
-  std::memset(&p, 0, sizeof(p));
-  p.gab_enabled = 1;
-  for (int c = 0; c < 3; ++c) {
-    p.gab_w[c][0] = rf.gab_weights[c][0];
-    p.gab_w[c][1] = rf.gab_weights[c][1];
-    p.epf.channel_scale[c] = rf.epf.channel_scale[c];
-  }
-  p.epf_iters = int(rf.epf.iters);
-  p.epf.pass0_sigma_scale = rf.epf.pass0_sigma_scale;
-  p.epf.pass2_sigma_scale = rf.epf.pass2_sigma_scale;
-  p.epf.border_sad_mul = rf.epf.border_sad_mul;
-  p.epf.sigma_for_modular = rf.epf.sigma_for_modular;
-  if (!sigma_is_constant) {
-    Plane& sp = plane(sigma.plane);
-    p.sigma = sp.f32();
-    p.sigma_stride = sp.w;
-  }
-  if (colour) {
-    p.colour = 1;
-    for (int i = 0; i < 3; ++i) p.col.opsin_bias[i] = colour->opsin_bias[i], p.col.cbrt_opsin_bias[i] = colour->cbrt_opsin_bias[i];
-    p.col.itscale = colour->itscale;
-    for (int i = 0; i < 9; ++i) p.col.matrix[i] = colour->matrix[i];
-    p.col.apply_srgb_tf = colour->apply_srgb_tf ? 1 : 0;
-    p.col.apply_bt709_tf = colour->apply_bt709_tf ? 1 : 0;
-  }
+  const DevFusedFilterParams p = fused_filter_params(rf, sigma_is_constant ? nullptr : plane(sigma.plane).f32(),
+                                                     sigma_is_constant ? 0 : plane(sigma.plane).w, colour);
   float gw[3];
-  for (int c = 0; c < 3; ++c) gw[c] = 1.0f / ((1.0f + p.gab_w[c][0] * 4.0f) + p.gab_w[c][1] * 4.0f);
+  strip_gab_norm(p, gw);
 
   const float* in[3];
   uint32_t in_stride[3], out_stride[3];

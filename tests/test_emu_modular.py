@@ -2,10 +2,12 @@
 
 tests/emu/modular_emu.cc compiles the per-stream code of modular_stream_kernel for the host -- the channel dispatch,
 the general loop, the single-leaf loop and the weighted predictor's fast loop with its row prologue -- and plugs it
-into the oracle's planner in place of the oracle's own Modular decoder. Decoded samples reach every pixel, and a wrong
-end position breaks the parse of what follows the stream, so equal frames pin both. The LF shapes include channels 1,
-2 and 129 samples wide (a last prologue chunk of one column) and rows of 1 and 2 samples, and a forced range trip runs
-the fast loop's fallback. The device launch itself is covered by the GPU parity tests.
+into the oracle's planner in place of the oracle's own Modular decoder. It decodes launches built by the CUDA backend's
+own table code (launch_tables.cc): compacted and shared channel subtrees by default, the whole-tree plans when the node
+limit is lowered to 0. Decoded samples reach every pixel, and a wrong end position breaks the parse of what follows the
+stream, so equal frames pin both. The LF shapes include channels 1, 2 and 129 samples wide (a last prologue chunk of
+one column) and rows of 1 and 2 samples, and a forced range trip runs the fast loop's fallback. The device launch
+itself is covered by the GPU parity tests.
 """
 import ctypes
 import os
@@ -20,7 +22,7 @@ import oracle_lib
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EMU = os.path.join(ROOT, "tests", "emu")
 GOLDEN = os.path.join(ROOT, "tests", "golden")
-SRCS = ["modular_emu.cc"] + [os.path.join("..", "..", "oracle", f) for f in
+SRCS = ["modular_emu.cc", "launch_tables_host.cc"] + [os.path.join("..", "..", "oracle", f) for f in
                              ("oracle_capi.cc", "oracle_modular.cc", "oracle_vardct.cc", "oracle_render.cc")] + \
        [os.path.join("..", "..", "jxl_oxide_b200", "csrc", "host", f) for f in
         ("entropy.cc", "headers.cc", "modular_syntax.cc", "frame_syntax.cc", "planner.cc", "icc.cc")]
@@ -35,11 +37,16 @@ def emu(tmp_path_factory):
     L = oracle_lib._load(out, None)
     L.jxlme_stats.argtypes = [ctypes.POINTER(ctypes.c_uint64), ctypes.c_int]
     L.jxlme_force_trip.argtypes = [ctypes.c_uint64]
+    L.jxlme_max_channel_tree_nodes.argtypes = [ctypes.c_uint64]
+    L.jxlme_max_channel_tree_nodes.restype = ctypes.c_uint64
     return L
 
 
+# [0] streams, [1] fast-loop channels, [2] of those decoded again after a range trip, [3] single-leaf channels,
+# [4] jobs built compact, [5] jobs built with the whole-tree plans, [6] channels sharing an earlier channel's subtree,
+# [7] jobs of launches without the fast loop (a table not staged)
 def _stats(L):
-    v = (ctypes.c_uint64 * 4)()
+    v = (ctypes.c_uint64 * 8)()
     L.jxlme_stats(v, 1)
     return list(v)
 
@@ -53,12 +60,24 @@ def _decode(L, data):
         oracle_lib._EMU_LIB = saved
 
 
-def _same(L, data):
+def _same(L, data, whole_tree=False):
     _stats(L)
     want = oracle_lib.OracleImage(data, threads=4)
-    got = _decode(L, data)
+    if whole_tree:
+        limit = L.jxlme_max_channel_tree_nodes(0)
+        try:
+            got = _decode(L, data)
+        finally:
+            L.jxlme_max_channel_tree_nodes(limit)
+    else:
+        got = _decode(L, data)
     stats = _stats(L)
     assert stats[0] > 0, "the emulated Modular path did not run"
+    assert stats[4] + stats[5] == stats[0]
+    if whole_tree:
+        assert stats[5] > 0, "no job was built with the whole-tree plans"
+    else:
+        assert stats[4] == stats[0], "a job was not built with compacted channel subtrees"
     assert got.num_frames == want.num_frames
     for i in range(want.num_frames):
         a, b = want.frame(i)[0], got.frame(i)[0]
@@ -92,12 +111,29 @@ def test_emulated_fast_loop_fallback_after_range_trip(emu, trip_at):
 
 
 def test_emulated_modular_streams_match_oracle_on_synthetic_modular_frame(emu):
-    _same(emu, bench.synth_frame(1000, 600, 7, extra=("--modular",)))
+    stats = _same(emu, bench.synth_frame(1000, 600, 7, extra=("--modular",)))
+    assert stats[6] > 0, "no channels shared a subtree copy"
 
 
-@pytest.mark.parametrize("name", ["grayalpha", "squeeze_edge", "issue_311", "patches_lossless", "lossless_pfm",
-                                  "lz77_flower", "delta_palette"])
-def test_emulated_modular_streams_match_oracle_on_fixture(emu, name):
+FIXTURES = ["grayalpha", "squeeze_edge", "issue_311", "patches_lossless", "lossless_pfm", "lz77_flower", "delta_palette"]
+
+
+def _fixture(name):
     d = os.path.join(GOLDEN, name)
-    data = open(os.path.join(d, sorted(f for f in os.listdir(d) if f.endswith(".jxl"))[0]), "rb").read()
-    _same(emu, data)
+    return open(os.path.join(d, sorted(f for f in os.listdir(d) if f.endswith(".jxl"))[0]), "rb").read()
+
+
+@pytest.mark.parametrize("name", FIXTURES)
+def test_emulated_modular_streams_match_oracle_on_fixture(emu, name):
+    stats = _same(emu, _fixture(name))
+    if name == "squeeze_edge":  # a Squeeze image's channels under one tree that never tests the channel index
+        assert stats[6] > 0, "no channels shared a subtree copy"
+    if name == "lz77_flower":  # the LZ77 window lives in global memory: the launch is not all staged
+        assert stats[7] == stats[0] and stats[1] == 0, "the fast loop was not disabled"
+
+
+# Node limit 0: every job with a channel subtree of more than one node walks the frame's whole tree (single-leaf channels
+# still compact, so squeeze_edge keeps every job compact).
+@pytest.mark.parametrize("name", [n for n in FIXTURES if n != "squeeze_edge"] + ["synthetic"])
+def test_emulated_modular_streams_match_oracle_with_whole_tree_plans(emu, name):
+    _same(emu, bench.synth_frame(2056, 600, 3) if name == "synthetic" else _fixture(name), whole_tree=True)
