@@ -19,7 +19,7 @@ import os
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("JXLB_LIB") or os.path.join(_HERE, "libjxlb200.so")  # JXLB_LIB: experiment builds (build.build_variant)
+LIB_PATH = os.path.join(_HERE, "libjxlb200.so")
 
 OK, ERR_BITSTREAM, ERR_UNSUPPORTED, ERR_EOF, ERR_CUDA, ERR_INVALID_ARG, ERR_DEVICE_DECODE, ERR_OUT_OF_MEMORY = range(8)
 
@@ -345,7 +345,7 @@ class Decoder:
         self._L.jxlb_set_fuse_filters(self._h, int(on))
 
     def set_hf_streams_per_cta(self, streams):
-        """HF streams per CTA: 0 (default, = 16), 8, 16, 32: one warp per stream; 4: round-1 kernel; 64 / 128: one thread per stream."""
+        """HF streams per CTA: 0 (default, = 16), 4 (= 8), 8, 16, 32: one warp per stream; 64 / 128: one thread per stream."""
         if self._L.jxlb_set_hf_streams_per_cta(self._h, int(streams)) != 0:
             raise ValueError("streams per CTA must be 0, 4, 8, 16, 32, 64 or 128")
 

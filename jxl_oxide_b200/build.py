@@ -72,27 +72,6 @@ def build(force=False, verbose=False):
     return OUT
 
 
-def build_variant(name, defines, sources=("kernels/vardct.cu", "kernels/filters_fused.cu")):
-    """Experiment builds: libjxlb200_<name>.so under _variants/ with -D<define> on the listed sources (the other objects
-    are shared with the main build). Select one at run time with JXLB_LIB=<path> (jxl_oxide_b200/__init__.py)."""
-    build()
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    vdir = os.path.join(HERE, "_variants")
-    os.makedirs(vdir, exist_ok=True)
-    objs = []
-    for src in SOURCES:
-        if src in sources:
-            obj = os.path.join(OBJ, name + "_" + src.replace("/", "_") + ".o")
-            subprocess.check_call([nvcc] + NVCC_FLAGS + ["-D" + d for d in defines] + ["-x", "cu", "-c", os.path.join(CSRC, src), "-o", obj], cwd=CSRC)
-        else:
-            obj = _obj_path(src)
-        objs.append(obj)
-    out = os.path.join(vdir, f"libjxlb200_{name}.so")
-    subprocess.check_call([nvcc, "--shared"] + ARCH + ["-Xcompiler", "-fPIC,-pthread"] + objs +
-                          ["-o", out, "-lcudart"], cwd=CSRC)
-    return out
-
-
 if __name__ == "__main__":
     build(force="--force" in sys.argv, verbose="-v" in sys.argv)
     print(OUT)

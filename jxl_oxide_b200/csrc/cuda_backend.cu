@@ -26,16 +26,6 @@ CudaBackend::CudaBackend(int device, bool own_stream) : device_(device), own_str
   if (e != cudaSuccess || count == 0)
     fail(kErrCuda, "no CUDA device available: the jxl_oxide_b200 hot path has no CPU fallback");
   CUDA_CHECK(cudaSetDevice(device_));
-  {
-    // The inverse transforms read 32-byte row segments of varblocks whose neighbours (of another size class) are fetched by
-    // another kernel at another time; with the default L2 fetch granularity every such read drags in the rest of its line.
-    // JXLB_L2_FETCH = 32 / 64 / 128 sets the device limit.
-    static const int l2_fetch = [] {
-      const char* e = std::getenv("JXLB_L2_FETCH");
-      return e ? std::atoi(e) : 0;
-    }();
-    if (l2_fetch > 0) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, size_t(l2_fetch));
-  }
   if (own_stream_) CUDA_CHECK(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
   CUDA_CHECK(cudaEventCreateWithFlags(&sync_event_, cudaEventBlockingSync | cudaEventDisableTiming));
   stage_cap_ = size_t(2) << 20;
@@ -54,23 +44,19 @@ CudaBackend::CudaBackend(int device, bool own_stream) : device_(device), own_str
   // A private stream-ordered pool per decoder: freed planes are reused by this decoder's next frame
   // (release threshold = never trim), and an allocation never has to wait on another decoder's
   // stream the way reuse inside the shared default pool can.
-  if (!std::getenv("JXLB_SHARED_POOL")) {
-    cudaMemPoolProps props;
-    std::memset(&props, 0, sizeof(props));
-    props.allocType = cudaMemAllocationTypePinned;
-    props.handleTypes = cudaMemHandleTypeNone;
-    props.location.type = cudaMemLocationTypeDevice;
-    props.location.id = device_;
-    CUDA_CHECK(cudaMemPoolCreate(&pool_, &props));
-  } else {
-    CUDA_CHECK(cudaDeviceGetDefaultMemPool(&pool_, device_));
-  }
+  cudaMemPoolProps props;
+  std::memset(&props, 0, sizeof(props));
+  props.allocType = cudaMemAllocationTypePinned;
+  props.handleTypes = cudaMemHandleTypeNone;
+  props.location.type = cudaMemLocationTypeDevice;
+  props.location.id = device_;
+  CUDA_CHECK(cudaMemPoolCreate(&pool_, &props));
   uint64_t keep = UINT64_MAX;
   CUDA_CHECK(cudaMemPoolSetAttribute(pool_, cudaMemPoolAttrReleaseThreshold, &keep));
   // All kernels of the library ask for the same (maximum shared memory) L1/shared split: an SM only
   // changes its split when idle, so kernels with different splits cannot share an SM, and the
   // long-running one-warp entropy CTAs would otherwise fence other streams' kernels off their SMs.
-  if (!std::getenv("JXLB_NO_CARVEOUT")) CUDA_CHECK(cudaDeviceSetCacheConfig(cudaFuncCachePreferShared));
+  CUDA_CHECK(cudaDeviceSetCacheConfig(cudaFuncCachePreferShared));
   if (const char* lanes = std::getenv("JXLB_HF_LANES")) {
     const int n = std::atoi(lanes);
     hf_streams_per_cta = n <= 0 ? 0 : (n <= 4 ? 4 : (n <= 8 ? 8 : (n <= 16 ? 16 : (n <= 32 ? 32 : (n <= 64 ? 64 : 128)))));
@@ -99,7 +85,7 @@ CudaBackend::~CudaBackend() {
   if (h_flag_) cudaFreeHost(const_cast<uint32_t*>(h_flag_));
   if (stream_ && own_stream_) cudaStreamDestroy(stream_);
   if (lf_arena_) cudaFree(lf_arena_);
-  if (pool_ && !std::getenv("JXLB_SHARED_POOL")) cudaMemPoolDestroy(pool_);
+  if (pool_) cudaMemPoolDestroy(pool_);
 }
 
 cudaStream_t CudaBackend::S() {
@@ -137,13 +123,11 @@ void CudaBackend::end_lease() {
 
 void* CudaBackend::lf_arena_alloc(size_t bytes) {
   if (!lf_arena_) {
-    const char* e = std::getenv("JXLB_LF_ARENA_MB");
-    lf_arena_cap_ = size_t(e ? std::atoi(e) : 64) << 20;
     CUDA_CHECK(cudaSetDevice(device_));
-    CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&lf_arena_), lf_arena_cap_));
+    CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&lf_arena_), kLfArenaBytes));
   }
   const size_t need = (bytes + 255) & ~size_t(255);
-  if (lf_arena_off_ + need > lf_arena_cap_) return nullptr;
+  if (lf_arena_off_ + need > kLfArenaBytes) return nullptr;
   void* p = lf_arena_ + lf_arena_off_;
   lf_arena_off_ += need;
   return p;
@@ -516,16 +500,6 @@ void CudaBackend::phase_mark(const char* name) {
   phase_t0_ = now;
 }
 
-// JXLB_DEBUG_SKIP (bit 0: HF decode, 1: dequant + transforms, 2: fused filters): tools/pipe_probe.py's "which stage
-// bounds the pipeline" experiment. The decoded pixels are garbage with any bit set; never set in tests or the bench.
-static int debug_skip() {
-  static const int v = [] {
-    const char* e = std::getenv("JXLB_DEBUG_SKIP");
-    return e ? std::atoi(e) : 0;
-  }();
-  return v;
-}
-
 void CudaBackend::stage_marker(const char* name, const View* views, int n) {
   if (!stop_stage.empty() && stop_stage == name) {
     // stage entry points (jxlb_decode_hf_groups, jxlb_dequant_idct, jxlb_modular_decode_groups): hand the stage's planes
@@ -794,19 +768,16 @@ void CudaBackend::decode_hf(VarDctState& st, std::vector<HfGroupJob>& jobs) {
   // The coefficient kernels read plain hybrid-uint tokens; an LZ77-enabled HF code (legal, hf_coeff.rs:181-222 goes
   // through read_varint_with_multiplier_clustered, but no known encoder emits it) would decode silently wrong.
   const bool hf_lz77 = hp.code.lz77_enabled;  // reported after the launch: a stream that is invalid anyway keeps its own error
-  DevHfParams p = build_hf_params(st, pass, *this, d_natural_orders_, natural_order_offset_);
-  {
-    const char* lim = std::getenv("JXLB_HF_ANS_SMEM");  // tuning knob (bytes); default: stage up to 128 KB
-    p.ans_smem_limit = lim ? uint32_t(std::atoi(lim)) : 128u * 1024u;
-  }
-  const std::vector<uint32_t> perm = hf_launch_order(jobs, hf_streams_per_cta >= 64);  // launch order -> `jobs`
+  const DevHfParams p = build_hf_params(st, pass, *this, d_natural_orders_, natural_order_offset_);
+  const HfSchedule sched = hf_schedule(p, hf_streams_per_cta);
+  const std::vector<uint32_t> perm = hf_launch_order(jobs, sched.lanes);  // launch order -> `jobs`
   std::vector<DevHfJob> dj;
   for (uint32_t i : perm) dj.push_back({jobs[i].bit_pos, jobs[i].bit_limit, jobs[i].group_idx});
   const DevHfJob* d_jobs = static_cast<const DevHfJob*>(upload_temp(dj.data(), dj.size() * sizeof(DevHfJob)));
   uint64_t* d_end = static_cast<uint64_t*>(stage_scratch(jobs.size() * 8));
   int* d_status = static_cast<int*>(stage_scratch(jobs.size() * 4));
   uint32_t* d_blk_ctx = nullptr;
-  if (hf_streams_per_cta >= 64) {
+  if (sched.lanes) {
     d_blk_ctx = static_cast<uint32_t*>(dmalloc(size_t(st.bw) * st.bh * 4));
     temps_.push_back(d_blk_ctx);
     begin_k("hf_block_ctx");
@@ -814,15 +785,12 @@ void CudaBackend::decode_hf(VarDctState& st, std::vector<HfGroupJob>& jobs) {
     end_k();
   }
   begin_k("decode_hf");
-  if (debug_skip() & 1) {  // experiment: what the pipeline does without this kernel (results are garbage)
-    CUDA_CHECK(cudaMemsetAsync(d_end, 0, jobs.size() * 8, S()));
-    CUDA_CHECK(cudaMemsetAsync(d_status, 0, jobs.size() * 4, S()));
-  } else if (hf_streams_per_cta >= 64)
+  if (sched.lanes)
     launch_decode_hf_lanes(active_cs_, dev_frame(st), p, d_blk_ctx, d_jobs, d_end, d_status, int(jobs.size()), pass == 0 ? 1 : 0,
-                           hf_streams_per_cta, S());
+                           sched.per_cta, S());
   else
     launch_decode_hf(active_cs_, dev_frame(st), p, d_jobs, d_end, d_status, int(jobs.size()), pass == 0 ? 1 : 0,
-                     hf_streams_per_cta > 0 ? hf_streams_per_cta : 16, S());
+                     sched.per_cta, S());
   end_k();
   const uint64_t* end = static_cast<const uint64_t*>(fetch_result(d_end, jobs.size() * 8));
   const int* status = static_cast<const int*>(fetch_result(d_status, jobs.size() * 4));
@@ -929,7 +897,7 @@ void CudaBackend::hf_dequant_cfl(VarDctState& st) {
 void CudaBackend::hf_transform(VarDctState& st) {
   void* scratch = dmalloc(hf_transform_scratch_bytes(st.bw, st.bh));
   begin_k("hf_transform");
-  if (!(debug_skip() & 2)) launch_hf_transform(dev_frame(st), scratch, have_pending_dequant_ ? &pending_dequant_ : nullptr, S());
+  launch_hf_transform(dev_frame(st), scratch, have_pending_dequant_ ? &pending_dequant_ : nullptr, S());
   end_k();
   have_pending_dequant_ = false;
   dfree(scratch);
@@ -1020,7 +988,7 @@ bool CudaBackend::filters_colour_fused(const View v[3], const RestorationFilter&
              "the fused filter kernel converts to sRGB-gamut targets only");
   const DevFusedFilterParams p = fused_filter_params(rf, d_sigma, sigma_stride, colour);
   begin_k("filters_fused");
-  if (!(debug_skip() & 4)) launch_filters_fused(in, out, p, S());
+  launch_filters_fused(in, out, p, S());
   end_k();
   for (int c = 0; c < 3; ++c) {
     PlaneRec& r = planes_.at(v[c].plane);

@@ -137,8 +137,7 @@ class CudaBackend : public Backend, private TableSink {
   void pack_to_device(const DevPackParams& p, void* d_dst);
   bool fuse_dequant = true;  // dequant + chroma from luma inside the inverse transforms (off: separate kernel)
   bool fuse_filters = true;  // single-kernel Gaborish+EPF+colour (off: stage-by-stage, for stage parity tests)
-  // HF coefficient streams per CTA: 0 (= 4), 8, 16 = one warp per stream (decode_hf_fast_kernel); 32 / 64 / 128 = one
-  // thread per stream (decode_hf_lanes_kernel). Initialised from JXLB_HF_LANES.
+  // HF coefficient streams per CTA (jxlb_set_hf_streams_per_cta, hf_schedule). Initialised from JXLB_HF_LANES.
   int hf_streams_per_cta = 0;
   bool profile = false;
   bool host_phases = false;  // wall clock per planner phase only (no CUDA events): where a frame's latency goes under load
@@ -192,12 +191,13 @@ class CudaBackend : public Backend, private TableSink {
   cudaStream_t S();  // the decoder's stream, leased on first use when it has none of its own
   void* lf_arena_alloc(size_t bytes);
   bool in_lf_arena(const void* p) const {
-    return lf_arena_ && p >= static_cast<const void*>(lf_arena_) && p < static_cast<const void*>(lf_arena_ + lf_arena_cap_);
+    return lf_arena_ && p >= static_cast<const void*>(lf_arena_) && p < static_cast<const void*>(lf_arena_ + kLfArenaBytes);
   }
   int device_;
   bool own_stream_ = true;
-  uint8_t* lf_arena_ = nullptr;  // device block the LF-stage planes of a pipeline decoder are carved from
-  size_t lf_arena_cap_ = 0, lf_arena_off_ = 0;
+  static constexpr size_t kLfArenaBytes = size_t(64) << 20;
+  uint8_t* lf_arena_ = nullptr;  // device block of kLfArenaBytes the LF-stage planes of a pipeline decoder are carved from
+  size_t lf_arena_off_ = 0;
   size_t pending_cs_bytes_ = 0;        // encoded bytes staged in h_input_, not yet copied to d_codestream_
   std::vector<void*> deferred_free_;   // pool pointers released while the decoder had no stream
   uint8_t* h_stage_ = nullptr;   // pinned

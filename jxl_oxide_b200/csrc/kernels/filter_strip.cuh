@@ -59,11 +59,8 @@ JXLB_FS float fs_absdiff(float a, float b) { return fabsf(fs_sub(a, b)); }
 
 // The Gaborish and distance phases walk the three channels with the same code (a loop, not three unrolled copies): the
 // kernel is straight-line code that every warp executes once, so its size is instruction-fetch traffic (the fully unrolled
-// body stalls on instruction fetch). JXLB_STRIP_ROLL=0 unrolls them again.
-#ifndef JXLB_STRIP_ROLL
-#define JXLB_STRIP_ROLL 1
-#endif
-constexpr int kChanUnroll = JXLB_STRIP_ROLL ? 1 : 3;
+// body stalls on instruction fetch).
+constexpr int kChanUnroll = 1;
 
 constexpr int kWX = 64, kWY = 32;        // window (shared-memory plane) size
 constexpr int kM = 4;                    // margin

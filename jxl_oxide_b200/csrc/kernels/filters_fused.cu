@@ -591,8 +591,7 @@ void launch_filters_fused(const DevView in[3], const DevView out[3], DevFusedFil
   FusedMaps maps;
   std::memset(&maps, 0, sizeof(maps));
   v.use_tma = 0;
-  static const bool no_tma = std::getenv("JXLB_NO_TMA") != nullptr;
-  if (EncodeTiledFn enc = no_tma ? nullptr : tensor_map_encoder()) {
+  if (EncodeTiledFn enc = tensor_map_encoder()) {
     bool ok = true;
     for (int c = 0; c < 3 && ok; ++c) {
       ok = (reinterpret_cast<uintptr_t>(v.in[c]) & 15) == 0 && (size_t(v.in_stride[c]) * 4) % 16 == 0;
@@ -627,14 +626,13 @@ void launch_filters_fused(const DevView in[3], const DevView out[3], DevFusedFil
 
   // The default chains (Gaborish + EPF step 1, or steps 1 and 2) run the interior of the frame in the column-strip kernel and only the
   // tiles that touch the image border (mirroring, Gaborish edge formulas) in the general one.
-  static const bool no_strip = std::getenv("JXLB_NO_STRIP") != nullptr;
   const fstrip::StripRect r = fstrip::strip_rect(v.width, v.height);
   // The strip kernel's window origins are 28 + 56 * tx and, for the pulled-back last column of tiles, width - 64: TMA wants the
   // box to start on a 16-byte boundary in the innermost dimension (cp.async.bulk.tensor with an origin of 325 floats ends in
   // "illegal instruction"), so frames whose width is not a multiple of four samples stay in the general kernel, whose origins
   // are multiples of four by construction.
   const bool origins_aligned = (v.width & 3) == 0;
-  if (!no_strip && v.use_tma && origins_aligned && p.gab_enabled && (p.epf_iters == 1 || p.epf_iters == 2) && r.x1 > r.x0 && r.y1 > r.y0) {
+  if (v.use_tma && origins_aligned && p.gab_enabled && (p.epf_iters == 1 || p.epf_iters == 2) && r.x1 > r.x0 && r.y1 > r.y0) {
     FusedMaps smaps;
     std::memset(&smaps, 0, sizeof(smaps));
     bool ok = true;

@@ -1,7 +1,7 @@
 // HF coefficient decode, one *thread* per stream (jxl-vardct/src/hf_coeff.rs:21-252).
 //
-// decode_hf_fast_kernel (entropy.cu) walks every stream from a single lane of its warp; with 510 streams
-// per 8K frame and 24 frames in flight the SM schedulers saturate on one-lane warps (DESIGN.md section 7).
+// decode_hf_warp_kernel (entropy.cu) walks every stream from a single lane of its warp; with 510 streams
+// per 8K frame and 24 frames in flight the SM schedulers saturate on one-lane warps (DESIGN.md section 4).
 // Here a warp carries 32 independent streams. The chain of one stream is written as a flat state machine --
 // every trip of the loop decodes exactly one symbol (a block's non-zero count or one coefficient) -- so the
 // lanes of a warp re-converge on the expensive part (alias-table ANS step + hybrid-uint read) no matter

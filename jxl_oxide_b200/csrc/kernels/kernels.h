@@ -138,7 +138,6 @@ struct DevHfParams {
   uint32_t order_offset[13 * 3];  // [order_id * 3 + channel] into `orders`
   const uint8_t* block_ctx_map;
   uint32_t block_ctx_map_size;
-  uint32_t ans_smem_limit;  // stage the ANS alias tables in shared memory when they fit in this many bytes
   const int32_t* lf_thresholds;   // concatenated X, Y, B
   uint32_t num_lf_thr[3];
   uint32_t has_lf_quant;  // 0: the frame uses an LF frame, the LF part of every block context is 0
@@ -151,10 +150,15 @@ struct DevHfJob {
   uint64_t bit_pos, bit_limit;
   uint32_t group_idx;
 };
-// One warp per stream, `warps_per_cta` (4, 8 or 16) streams per CTA sharing the staged tables.
+// Shared memory of the HF coefficient kernels: the ANS alias tables are staged when they take at most kHfAnsSmemBytes,
+// the cluster maps of all HF presets together when they take at most kLaneCmapSmemBytes. The one-warp-per-stream kernel
+// always stages the cluster maps, so larger ones run one thread per stream (hf_schedule in launch_tables.h).
+constexpr uint32_t kHfAnsSmemBytes = 128 * 1024;
+constexpr uint32_t kLaneCmapSmemBytes = 32 * 1024;
+// One warp per stream, `warps_per_cta` (8, 16 or 32) streams per CTA sharing the staged tables.
 void launch_decode_hf(const uint8_t* codestream, DevFrame f, DevHfParams p, const DevHfJob* jobs, uint64_t* end_bits,
                       int* status, int num_jobs, int first_pass, int warps_per_cta, cudaStream_t stream);
-// Same contract, one thread per stream (kernels/hf_lanes.cuh); `streams_per_cta` in {32, 64, 128}.
+// Same contract, one thread per stream (kernels/hf_lanes.cuh); `streams_per_cta` in {64, 128}.
 // `blk_ctx` (bw x bh words) comes from launch_hf_block_ctx: transform type and context offset of every varblock origin.
 void launch_hf_block_ctx(DevFrame f, DevHfParams p, uint32_t* out, cudaStream_t stream);
 void launch_decode_hf_lanes(const uint8_t* codestream, DevFrame f, DevHfParams p, const uint32_t* blk_ctx, const DevHfJob* jobs,

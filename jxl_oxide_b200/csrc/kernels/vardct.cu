@@ -547,9 +547,7 @@ struct TransformLists {
   uint32_t* items[4];
   uint32_t* shape_items[kMediumShapes];
   uint32_t* small_items[kSmallTypes];
-  uint32_t flags;  // bit 0: idct_small prefetches the next block's coefficient rows into L2 (JXLB_L2_PREFETCH=1 sets it)
 };
-__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
 // One list slot per varblock. The lanes of a warp that append to the same list reserve their slots with ONE atomic
 // (match_any): a frame has half a million cells and a dozen counters, and one atomic per cell serialises on them.
@@ -849,20 +847,13 @@ __device__ __forceinline__ void cfl_factors(const DevFrame& f, const DevDequantP
   kb = __fadd_rn(p.base_correlation_b, __fdiv_rn(float(f.b_from_y[ti]), p.colour_factor));
 }
 
-// Experiment knobs (build.build_variant): defaults are the measured best (requesting the three channels together costs
-// idct_small registers and a third of its warps; medium trips of 8 rows beat 4 and 16).
-#ifndef JXLB_SMALL_PREFETCH
-#define JXLB_SMALL_PREFETCH 0  // idct_small: request the three channels' rows of a block together
-#endif
-#ifndef JXLB_MEDIUM_TRIP
-#define JXLB_MEDIUM_TRIP 8    // idct_medium: tile rows whose loads are in flight together (4, 8, 16, 32)
-#endif
-#ifndef JXLB_SMALL_MINB
-#define JXLB_SMALL_MINB 3      // idct_small: resident CTAs per SM asked of the register allocator
-#endif
-constexpr int kSmallGroups = 32;  // 8-thread groups per CTA
+// Measured: idct_small requesting the three channels' rows of a block together costs registers and a third of its warps;
+// idct_medium trips of 8 rows beat 4 and 16.
+constexpr int kMediumTrip = 8;      // idct_medium: tile rows whose loads are in flight together
+constexpr int kSmallMinBlocks = 3;  // idct_small: resident CTAs per SM asked of the register allocator
+constexpr int kSmallGroups = 32;    // 8-thread groups per CTA
 template <bool DEQ>
-__global__ void __launch_bounds__(kSmallGroups * 8, JXLB_SMALL_MINB) idct_small_kernel(DevFrame f, DevDequantParams dq, TransformLists lists) {
+__global__ void __launch_bounds__(kSmallGroups * 8, kSmallMinBlocks) idct_small_kernel(DevFrame f, DevDequantParams dq, TransformLists lists) {
   __shared__ float s_tile[kSmallGroups][72];      // 8 x 9
   __shared__ float s_special[kSmallGroups][192];  // 8 x 8 copy + 128 scratch
   const uint32_t group = threadIdx.x >> 3, r = threadIdx.x & 7;
@@ -878,32 +869,9 @@ __global__ void __launch_bounds__(kSmallGroups * 8, JXLB_SMALL_MINB) idct_small_
     const uint32_t item = items[DEQ ? work : work / 3];
     const uint32_t sbx = item & 0xffff, sby = item >> 16;
     const int32_t t = f.blk_type[size_t(sby) * f.bw + sbx];
-    if (DEQ && (lists.flags & 1)) {
-      // The rows this thread will read for the chroma channels of this block, and for the block it takes next, are
-      // requested into L2 now (no registers held): the loads below and in the next trip then wait for L2, not for DRAM.
-      const size_t here = (size_t(sby) * 8 + r) * f.cw + size_t(sbx) * 8;
-      prefetch_l2(f.coeff[0] + here);
-      prefetch_l2(f.coeff[2] + here);
-      const uint32_t next = work + gridDim.x * kSmallGroups;
-      if (next < total) {
-        const uint32_t ni = items[next];
-        const size_t there = (size_t(ni >> 16) * 8 + r) * f.cw + size_t(ni & 0xffff) * 8;
-        prefetch_l2(f.coeff[1] + there);
-      }
-    }
     DeqBlock db;
     float kx = 0.0f, kb = 0.0f, vy[8];
-    // DEQ (never subsampled: every channel keeps the block at (sbx, sby)): the coefficient rows of the three channels are
-    // requested together, before the first use - one exposed DRAM latency per block instead of three
-    float4 pre[3][2];
-    constexpr bool kPre = DEQ && JXLB_SMALL_PREFETCH;
     if (DEQ) {
-#pragma unroll
-      for (int c = 0; kPre && c < 3; ++c) {
-        const float* prow = reinterpret_cast<const float*>(f.coeff[c]) + (size_t(sby) * 8 + r) * f.cw + size_t(sbx) * 8;
-        pre[c][0] = *reinterpret_cast<const float4*>(prow);
-        pre[c][1] = *reinterpret_cast<const float4*>(prow + 4);
-      }
       db = deq_block(f, dq, t, sbx, sby);
       cfl_factors(f, dq, sbx * 8, sby * 8, kx, kb);
     }
@@ -913,13 +881,7 @@ __global__ void __launch_bounds__(kSmallGroups * 8, JXLB_SMALL_MINB) idct_small_
       uint32_t bx, by;  // where channel c keeps this block
       if (!channel_block(f, c, sbx, sby, bx, by)) continue;
       float* row = reinterpret_cast<float*>(f.coeff[c]) + (size_t(by) * 8 + r) * f.cw + size_t(bx) * 8;
-      float4 lo, hi;
-      if (kPre) {
-        lo = ci == 0 ? pre[1][0] : (ci == 1 ? pre[0][0] : pre[2][0]);
-        hi = ci == 0 ? pre[1][1] : (ci == 1 ? pre[0][1] : pre[2][1]);
-      } else {
-        lo = *reinterpret_cast<const float4*>(row), hi = *reinterpret_cast<const float4*>(row + 4);
-      }
+      const float4 lo = *reinterpret_cast<const float4*>(row), hi = *reinterpret_cast<const float4*>(row + 4);
       float v[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
       if (DEQ) {
         const float4 m0 = __ldg(reinterpret_cast<const float4*>(db.mat[c] + r * 8));
@@ -986,23 +948,18 @@ constexpr int kMediumWarps = 4;
 // One varblock of a warp's 32 x 32 tile (idct_medium_kernel).
 struct MediumSub {
   uint32_t bx[3], by[3];  // where channel c keeps the block (8x8 cells); by == 0xffffffff: the channel skips it
-  float mul[3];           // DeqBlock::mul
-  float kx[4], kb[4];     // chroma-from-luma factors of the (at most 2 x 2) 64x64 tiles the block touches
-  uint32_t tx0, ty0;      // the first of those tiles
 };
-// Varblocks of 16x8 ... 32x32 samples, one warp per 32 x 32 TILE of them: a tile holds (32 / w) x (32 / h) blocks of
-// the shape being walked (8 of 16x8, 4 of 16x16, 1 of 32x32), so the row pass (lane = tile row) and the column pass
-// (lane = tile column) keep all 32 lanes busy whatever the shape; with one block per warp a 16x8 block used 8 and 16
-// lanes of 32. Per block nothing changes: same loads, same operation order in the line transforms.
-template <bool DEQ>
+// Varblocks of 16x8 ... 32x32 samples of frames whose coefficients are already dequantised, one warp per 32 x 32 TILE of
+// them: a tile holds (32 / w) x (32 / h) blocks of the shape being walked (8 of 16x8, 4 of 16x16, 1 of 32x32), so the row
+// pass (lane = tile row) and the column pass (lane = tile column) keep all 32 lanes busy whatever the shape; with one
+// block per warp a 16x8 block used 8 and 16 lanes of 32. Per block nothing changes: same loads, same operation order in
+// the line transforms. `dq` is unused: the launch passes the same arguments to every transform kernel.
 __global__ void __launch_bounds__(kMediumWarps * 32) idct_medium_kernel(DevFrame f, DevDequantParams dq, TransformLists lists) {
   __shared__ float s_tile[kMediumWarps][32 * 33];
-  __shared__ float s_ytile[DEQ ? kMediumWarps : 1][DEQ ? 32 * 33 : 1];  // dequantised Y coefficients (chroma from luma)
   __shared__ float s_llf[kMediumWarps][8][16];
   __shared__ MediumSub s_sub[kMediumWarps][8];
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   float* tile = s_tile[warp];
-  float* ytile = s_ytile[DEQ ? warp : 0];
   MediumSub* sub = s_sub[warp];
 #pragma unroll 1
   for (int shape = 0; shape < kMediumShapes; ++shape) {
@@ -1017,12 +974,6 @@ __global__ void __launch_bounds__(kMediumWarps * 32) idct_medium_kernel(DevFrame
     const int logw = 31 - __clz(w), logh = 31 - __clz(h);
     const int lognx = 5 - logw, logny = 5 - logh, logp = lognx + logny;  // blocks across, down, per tile
     const int ny = 1 << logny;
-    const float* mat[3] = {nullptr, nullptr, nullptr};
-    if (DEQ) {
-      const uint32_t set = kDevTransformInfo[t][2], tr = kDevTransformInfo[t][4];
-#pragma unroll
-      for (int c = 0; c < 3; ++c) mat[c] = dq.matrices + dq.matrix_offset[(set * 3 + c) * 2 + tr];
-    }
     // this lane's tile column: block column sx, sample column x inside the block
     const int sx = int(lane) >> logw, x = int(lane) & (w - 1);
 #pragma unroll 1
@@ -1041,23 +992,12 @@ __global__ void __launch_bounds__(kMediumWarps * 32) idct_medium_kernel(DevFrame
           m.bx[c] = bx;
           m.by[c] = has ? by : 0xffffffffu;
         }
-        m.tx0 = (sbx * 8) >> 6, m.ty0 = (sby * 8) >> 6;
-        if (DEQ) {
-          const DeqBlock db = deq_block(f, dq, t, sbx, sby);
-#pragma unroll
-          for (int c = 0; c < 3; ++c) m.mul[c] = db.mul[c];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const uint32_t tx = min(m.tx0 + uint32_t(i & 1), f.w64 - 1), ty = min(m.ty0 + uint32_t(i >> 1), (f.ch + 63) / 64 - 1);
-            cfl_factors(f, dq, tx << 6, ty << 6, m.kx[i], m.kb[i]);
-          }
-        }
         sub[lane] = m;
       }
       __syncwarp();
 #pragma unroll 1
       for (int ci = 0; ci < 3; ++ci) {
-        const uint32_t c = DEQ ? (ci == 0 ? 1u : (ci == 1 ? 0u : 2u)) : uint32_t(ci);
+        const uint32_t c = uint32_t(ci);
         // the (up to 4) blocks of this lane's tile column
         float* col[4];
 #pragma unroll
@@ -1067,34 +1007,18 @@ __global__ void __launch_bounds__(kMediumWarps * 32) idct_medium_kernel(DevFrame
           if (sy < ny && s < nb && sub[s].by[c] != 0xffffffffu)
             col[sy] = reinterpret_cast<float*>(f.coeff[c]) + size_t(sub[s].by[c]) * 8 * f.cw + size_t(sub[s].bx[c]) * 8 + x;
         }
-        // 32 tile rows, kTrip per trip, all loads of a trip issued before the first use
-        constexpr int kTrip = JXLB_MEDIUM_TRIP;
+        // 32 tile rows, kMediumTrip per trip, all loads of a trip issued before the first use
 #pragma unroll 1
-        for (int y0 = 0; y0 < 32; y0 += kTrip) {
-          float raw[kTrip], mt[kTrip];
+        for (int y0 = 0; y0 < 32; y0 += kMediumTrip) {
+          float raw[kMediumTrip];
 #pragma unroll
-          for (int j = 0; j < kTrip; ++j) {
+          for (int j = 0; j < kMediumTrip; ++j) {
             const int Y = y0 + j, sy = Y >> logh, y = Y & (h - 1);
             const float* src = sy == 0 ? col[0] : (sy == 1 ? col[1] : (sy == 2 ? col[2] : col[3]));
             raw[j] = src ? src[size_t(y) * f.cw] : 0.0f;
-            if (DEQ) mt[j] = __ldg(mat[c] + (y << logw) + x);
           }
 #pragma unroll
-          for (int j = 0; j < kTrip; ++j) {
-            const int Y = y0 + j, sy = Y >> logh, y = Y & (h - 1);
-            float v = raw[j];
-            if (DEQ) {
-              const MediumSub& m = sub[min((sy << lognx) + sx, nb - 1)];
-              const float q = deq_one(__float_as_uint(v), mt[j], m.mul[c], dq.quant_bias[c], dq.quant_bias_numerator);
-              if (c == 1) {
-                ytile[Y * 33 + int(lane)] = v = q;
-              } else {
-                const int ti = int(((m.bx[c] * 8 + uint32_t(x)) >> 6) - m.tx0) + 2 * int(((m.by[c] * 8 + uint32_t(y)) >> 6) - m.ty0);
-                v = __fadd_rn(q, __fmul_rn(c == 0 ? m.kx[ti & 3] : m.kb[ti & 3], ytile[Y * 33 + int(lane)]));
-              }
-            }
-            tile[Y * 33 + int(lane)] = v;
-          }
+          for (int j = 0; j < kMediumTrip; ++j) tile[(y0 + j) * 33 + int(lane)] = raw[j];
         }
         // lowest frequencies from the LF image: lane s for block s, then 16 lanes place the (at most) 16 values of the tile
         if (int(lane) < nb && sub[lane].by[c] != 0xffffffffu) compute_llf_small(f, int(c), sub[lane].bx[c], sub[lane].by[c], bw, bh, s_llf[warp][lane]);
@@ -1139,10 +1063,9 @@ __global__ void __launch_bounds__(kMediumWarps * 32) idct_medium_kernel(DevFrame
 // look-ups of the generic body (which spent several times more instructions on indexing than on arithmetic) fold into
 // immediates. The shapes are walked one after the other by all CTAs in step, so one instantiation's code is hot at a time,
 // and the line transforms are the shared idct_line_smem<N>.
-#ifndef JXLB_MEDIUM_ROLL
-#define JXLB_MEDIUM_ROLL 0     // medium_walk: block rows / 8-row batches of a tile as loops instead of unrolled: less than
-#endif                         // half the instructions, but measured slower - the unrolled form wins
-constexpr int kMediumOuterUnroll = JXLB_MEDIUM_ROLL ? 1 : 32;
+// medium_walk unrolls the block rows and 8-row batches of a tile: as loops they take less than half the instructions, but
+// were measured slower.
+constexpr int kMediumOuterUnroll = 32;
 struct MediumBlk {
   uint32_t bx, by;     // block position in 8x8 cells (dequantising frames are never subsampled: the same for all channels)
   float mul[3];        // DeqBlock::mul
@@ -1258,10 +1181,8 @@ __device__ __forceinline__ void medium_walk(const DevFrame& f, const DevDequantP
   }
 }
 
-#ifndef JXLB_MEDIUM_MINB
-#define JXLB_MEDIUM_MINB 5  // the fastest of 4 / 5 / 6 when measured; not re-measured on the H100
-#endif
-__global__ void __launch_bounds__(kMediumWarps * 32, JXLB_MEDIUM_MINB) idct_medium_deq_kernel(DevFrame f, DevDequantParams dq, TransformLists lists) {
+constexpr int kMediumMinBlocks = 5;  // the fastest of 4 / 5 / 6 when measured; not re-measured on the H100
+__global__ void __launch_bounds__(kMediumWarps * 32, kMediumMinBlocks) idct_medium_deq_kernel(DevFrame f, DevDequantParams dq, TransformLists lists) {
   __shared__ float s_tile[kMediumWarps][32 * 33];
   __shared__ float s_ytile[kMediumWarps][32 * 33];  // dequantised Y coefficients (chroma from luma)
   __shared__ float s_llf[kMediumWarps][8][16];
@@ -1587,12 +1508,10 @@ void launch_idcts(DevFrame f, const DevDequantParams& dq, const TransformLists& 
   const int small_grid = int(std::min<size_t>((cells * per + kSmallGroups - 1) / kSmallGroups, size_t(num_sms) * 8));
   idct_small_kernel<DEQ><<<small_grid, kSmallGroups * 8, 0, stream>>>(f, dq, L);
   const int medium_grid = int(std::min<size_t>((cells / 2 * per + kMediumWarps) / kMediumWarps, size_t(num_sms) * 8));
-  static const bool generic_medium = std::getenv("JXLB_MEDIUM_GENERIC") != nullptr;
-  if (DEQ && !generic_medium) idct_medium_deq_kernel<<<medium_grid, kMediumWarps * 32, 0, stream>>>(f, dq, L);
-  else idct_medium_kernel<DEQ><<<medium_grid, kMediumWarps * 32, 0, stream>>>(f, dq, L);
+  if (DEQ) idct_medium_deq_kernel<<<medium_grid, kMediumWarps * 32, 0, stream>>>(f, dq, L);
+  else idct_medium_kernel<<<medium_grid, kMediumWarps * 32, 0, stream>>>(f, dq, L);
   const int large_grid = int(std::min<size_t>((cells / 32 + 1) * per, size_t(num_sms) * 4));
-  static const bool generic_large = std::getenv("JXLB_LARGE_GENERIC") != nullptr;
-  if (DEQ && !generic_large) idct_large64_deq_kernel<<<large_grid, kL64Threads, kL64SmemFloats * 4, stream>>>(f, dq, L.items[2], L.counts + 2);
+  if (DEQ) idct_large64_deq_kernel<<<large_grid, kL64Threads, kL64SmemFloats * 4, stream>>>(f, dq, L.items[2], L.counts + 2);
   else idct_large_kernel<DEQ><<<large_grid, kLargeThreads, (1024 + kLargeThreads * (2 * 64 + 1)) * 4, stream>>>(f, dq, L.items[2], L.counts + 2, 64);
   const int huge_grid = int(std::min<size_t>((cells / 128 + 1) * per, size_t(num_sms)));
   idct_large_kernel<DEQ><<<huge_grid, kLargeThreads, (1024 + kLargeThreads * (2 * 256 + 1)) * 4, stream>>>(f, dq, L.items[3], L.counts + 3, 256);
@@ -1622,9 +1541,6 @@ void launch_hf_transform(DevFrame f, void* scratch, const DevDequantParams* dq, 
       q += cells + 1;
     }
   }
-  // measured: no faster for idct_small, and more DRAM reads per frame: off by default
-  static const bool l2_prefetch = std::getenv("JXLB_L2_PREFETCH") != nullptr;
-  L.flags = l2_prefetch ? 1u : 0u;
   cudaMemsetAsync(L.counts, 0, 128, stream);
   dim3 cb(32, 8), cg((f.bw + 31) / 32, (f.bh + 7) / 8);
   classify_varblocks_kernel<<<cg, cb, 0, stream>>>(f, L);

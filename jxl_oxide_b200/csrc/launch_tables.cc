@@ -334,6 +334,15 @@ DevHfParams build_hf_params(const VarDctState& st, uint32_t pass, TableSink& sin
   return p;
 }
 
+HfSchedule hf_schedule(const DevHfParams& p, int streams_per_cta) {
+  const bool cmaps_fit = 495u * p.num_block_clusters * p.num_hf_presets <= kLaneCmapSmemBytes;
+  if (!cmaps_fit || streams_per_cta > 64) return {true, 128};
+  if (streams_per_cta == 64) return {true, 64};
+  if (streams_per_cta >= 32) return {false, 32};
+  if (streams_per_cta >= 16 || streams_per_cta == 0) return {false, 16};
+  return {false, 8};
+}
+
 std::vector<uint32_t> hf_launch_order(const std::vector<HfGroupJob>& jobs, bool longest_first) {
   std::vector<uint32_t> perm(jobs.size());
   for (size_t i = 0; i < jobs.size(); ++i) perm[i] = uint32_t(i);

@@ -45,9 +45,18 @@ ModularLaunch build_modular_launch(const std::vector<ModularStreamJob>& jobs,
 // The 13 natural coefficient orders back to back; offset[id] is where order `id` starts.
 std::vector<uint32_t> natural_order_table(uint32_t offset[13]);
 // Parameters of one HF pass. `natural_orders` is natural_order_table() where the kernel can read it, used unless the pass
-// carries a custom order. ans_smem_limit is left 0.
+// carries a custom order.
 DevHfParams build_hf_params(const VarDctState& st, uint32_t pass, TableSink& sink, const uint32_t* natural_orders,
                             const uint32_t natural_offset[13]);
+// Which kernel decodes the HF streams of one pass, and how many streams share a CTA: one thread per stream
+// (launch_decode_hf_lanes, `per_cta` 64 or 128) or one warp per stream (launch_decode_hf, `per_cta` 8, 16 or 32).
+struct HfSchedule {
+  bool lanes;
+  int per_cta;
+};
+// `streams_per_cta` is the decoder's setting (jxlb_set_hf_streams_per_cta): 0 (one warp per stream, 16 per CTA), 4 (the
+// same as 8), 8, 16, 32, 64 or 128. Cluster maps larger than kLaneCmapSmemBytes always run one thread per stream, 128 per CTA.
+HfSchedule hf_schedule(const DevHfParams& p, int streams_per_cta);
 // Launch order of the HF streams as indices into `jobs`. longest_first (the thread-per-stream kernel): longest section
 // first, so that streams of similar length share a warp.
 std::vector<uint32_t> hf_launch_order(const std::vector<HfGroupJob>& jobs, bool longest_first);

@@ -569,15 +569,11 @@ int32_t jxlb_pipeline_create(int32_t device, const jxlb_pipeline_config* cfg, jx
   p->heavy_frames = heavy;
   p->slabs.resize(size_t(heavy));
   if (cudaSetDevice(device) != cudaSuccess) return JXLB_ERR_CUDA;
-  {
-    // A pipeline owns its device's decode work: L2 fetches 32-byte sectors instead of whole 128-byte lines. The inverse
-    // transforms read 32-byte row segments of varblocks whose line neighbours belong to another size class, i.e. to another
-    // kernel at another time, so 32-byte fetches read less DRAM for the same kernel times. JXLB_L2_FETCH=0 leaves the limit alone,
-    // 64 / 128 set another value (also honoured by stand-alone decoders, which do not touch the limit by default).
-    const char* e = std::getenv("JXLB_L2_FETCH");
-    const int g = e ? std::atoi(e) : 32;
-    if (g > 0) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, size_t(g));
-  }
+  // A pipeline owns its device's decode work: L2 fetches 32-byte sectors instead of whole 128-byte lines. The inverse
+  // transforms read 32-byte row segments of varblocks whose line neighbours belong to another size class, i.e. to another
+  // kernel at another time, so 32-byte fetches read less DRAM for the same kernel times. A stand-alone decoder leaves the
+  // limit alone.
+  cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, 32);
   for (Slab& sl : p->slabs)
     if (cudaStreamCreateWithFlags(&sl.stream, cudaStreamNonBlocking) != cudaSuccess) return JXLB_ERR_CUDA;
   p->batcher.reset(new BatchService(device, cfg && cfg->batch_streams > 0 ? cfg->batch_streams : 6));

@@ -281,7 +281,7 @@ bool EmuBackend::filters_colour_fused(const View v[3], const RestorationFilter& 
   const bool colour_ok = !colour || (!colour->second_stage && colour->gamma == 0.0f);
   if (std::getenv("JXLE_TRACE"))
     std::fprintf(stderr, "[emu] filters: %d x %d, gab %d, epf iters %u, colour %d\n", width, height, int(rf.gab_enabled), rf.epf.iters, int(colour != nullptr));
-  if (!rf.gab_enabled || (rf.epf.iters != 1 && rf.epf.iters != 2) || r.x1 <= r.x0 || r.y1 <= r.y0 || !colour_ok || std::getenv("JXLE_NO_STRIP")) return false;
+  if (!rf.gab_enabled || (rf.epf.iters != 1 && rf.epf.iters != 2) || r.x1 <= r.x0 || r.y1 <= r.y0 || !colour_ok) return false;
   for (int c = 0; c < 3; ++c)
     if (v[c].x0 != 0 || v[c].y0 != 0 || int(v[c].w) != width || int(v[c].h) != height) return false;
 

@@ -18,9 +18,9 @@ from conftest import fixture_bytes
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(600, method="thread")]
 
 FIXTURES = ["opsin_inverse", "bike", "cafe", "issue_425", "genshin_ycbcr_420", "bench_oriented_brg", "minecraft_vardct_e7", "upsampling"]
-# streams per CTA: 8 / 16 (default) / 32 = one warp per stream, every preset's tables staged once per CTA
-# (decode_hf_warp_kernel); 4 = the round-1 kernel (also the fall-back for oversized cluster maps); 64 = one thread per stream
-SCHEDULES = [4, 32, 64]
+# streams per CTA: 8 and 32 run one warp per stream with every preset's tables staged once per CTA (decode_hf_warp_kernel;
+# the default 16 runs in every other GPU test), 64 one thread per stream (decode_hf_lanes_kernel)
+SCHEDULES = [8, 32, 64]
 
 
 @pytest.fixture(scope="module")
@@ -134,8 +134,9 @@ def test_epf_iteration_counts(dec, oracle, iters):
 
 @pytest.mark.parametrize("streams", [0, 16, 32, 128])
 def test_hf_presets_on_the_device(dec, oracle, streams):
-    """Several HF presets (synthetic: no reference fixture has more than one): the default kernel stages one preset's
-    cluster-map slice per warp, the thread-per-stream kernel all of them per CTA."""
+    """Several HF presets (synthetic: no reference fixture has more than one). Their cluster maps (5 x 495 x 15 B = 37 KB)
+    exceed what the one-warp-per-stream kernel stages, so every value here, 0, 16 and 32 included, runs the
+    thread-per-stream kernel, which reads them from global memory."""
     data = bench.synth_frame(1000, 600, 7, extra=("--hf-presets", "5", "--passes", "2"))
     if streams:
         _check(dec, oracle, data, streams)
