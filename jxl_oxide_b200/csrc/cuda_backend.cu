@@ -776,18 +776,22 @@ void CudaBackend::decode_hf(VarDctState& st, std::vector<HfGroupJob>& jobs) {
   const DevHfJob* d_jobs = static_cast<const DevHfJob*>(upload_temp(dj.data(), dj.size() * sizeof(DevHfJob)));
   uint64_t* d_end = static_cast<uint64_t*>(stage_scratch(jobs.size() * 8));
   int* d_status = static_cast<int*>(stage_scratch(jobs.size() * 4));
-  uint32_t* d_blk_ctx = nullptr;
+  uint2* d_list = nullptr;
+  uint32_t* d_counts = nullptr;
   if (sched.lanes) {
-    d_blk_ctx = static_cast<uint32_t*>(dmalloc(size_t(st.bw) * st.bh * 4));
-    temps_.push_back(d_blk_ctx);
+    const size_t groups = hf_block_list_count(dev_frame(st), p);
+    const size_t records = groups * p.group_dim_blocks * p.group_dim_blocks;
+    d_list = static_cast<uint2*>(dmalloc(records * sizeof(uint2) + groups * 4));
+    temps_.push_back(d_list);
+    d_counts = reinterpret_cast<uint32_t*>(d_list + records);
     begin_k("hf_block_ctx");
-    launch_hf_block_ctx(dev_frame(st), p, d_blk_ctx, S());
+    launch_hf_block_list(dev_frame(st), p, d_list, d_counts, S());
     end_k();
   }
   begin_k("decode_hf");
   if (sched.lanes)
-    launch_decode_hf_lanes(active_cs_, dev_frame(st), p, d_blk_ctx, d_jobs, d_end, d_status, int(jobs.size()), pass == 0 ? 1 : 0,
-                           sched.per_cta, S());
+    launch_decode_hf_lanes(active_cs_, dev_frame(st), p, d_list, d_counts, d_jobs, d_end, d_status, int(jobs.size()),
+                           pass == 0 ? 1 : 0, sched.per_cta, S());
   else
     launch_decode_hf(active_cs_, dev_frame(st), p, d_jobs, d_end, d_status, int(jobs.size()), pass == 0 ? 1 : 0,
                      sched.per_cta, S());

@@ -51,117 +51,6 @@ __host__ __device__ inline HfSmem hf_layout(const DevHfParams& p) {
 //     symbol, which covers the ANS 16-bit refill and a prefix-code peek; only the rare long hybrid-uint tail checks again;
 //   * loads never pass the section's end (stop index), so corrupt streams are caught by the position check per channel.
 // Semantics: jxl-vardct/src/hf_coeff.rs:21-252, jxl-coding/src/{ans.rs:276-330, prefix.rs:335-357, lib.rs:572-605}.
-__device__ __forceinline__ uint32_t sm_addr(const void* p) { return uint32_t(__cvta_generic_to_shared(p)); }
-__device__ __forceinline__ uint32_t lds8(uint32_t a) {
-  uint32_t v;
-  asm("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(a));
-  return v;
-}
-__device__ __forceinline__ uint32_t lds32(uint32_t a) {
-  uint32_t v;
-  asm("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(a));
-  return v;
-}
-__device__ __forceinline__ uint2 lds64(uint32_t a) {
-  uint2 v;
-  asm("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(a));
-  return v;
-}
-
-struct HfBits {  // LSB-first reader, 64-bit buffer + one word in flight, word-indexed
-  const uint32_t* base;
-  uint32_t widx, stop_idx;
-  uint64_t buf;
-  uint32_t ahead;
-  int nbits;
-  __device__ __forceinline__ void init(const uint8_t* d, uint64_t bit_pos, uint64_t bit_limit) {
-    base = reinterpret_cast<const uint32_t*>(d);
-    const uint32_t w = uint32_t(bit_pos >> 5), skip = uint32_t(bit_pos & 31);
-    stop_idx = uint32_t((bit_limit + 31) >> 5) + 2;
-    buf = uint64_t(__ldg(base + w)) >> skip;
-    nbits = 32 - int(skip);
-    buf |= uint64_t(__ldg(base + w + 1)) << nbits;
-    nbits += 32;
-    ahead = __ldg(base + w + 2);
-    widx = w + 3;
-  }
-  __device__ __forceinline__ void refill() {  // nbits <= 32 -> nbits > 32
-    buf |= uint64_t(ahead) << nbits;
-    nbits += 32;
-    ahead = widx <= stop_idx ? __ldg(base + widx) : 0u;
-    ++widx;
-  }
-  __device__ __forceinline__ void top_up() {
-    if (nbits < 32) refill();
-  }
-  __device__ __forceinline__ uint32_t take(uint32_t n) {  // n <= 32 bits that are known to be buffered
-    const uint32_t v = uint32_t(buf) & (n >= 32 ? 0xffffffffu : ((1u << n) - 1));
-    buf >>= n;
-    nbits -= int(n);
-    return v;
-  }
-  __device__ __forceinline__ uint64_t pos() const { return uint64_t(widx - 1) * 32 - uint64_t(nbits); }
-};
-
-struct HfTables {  // 32-bit shared addresses (ans: only when ANS_SMEM) + global fall-backs
-  uint32_t cfg, ans;
-  const uint64_t* ans_g;
-  const uint32_t* prefix;
-  const uint32_t* prefix_meta;
-  uint32_t log_alphabet_size, log_bucket, use_prefix;
-};
-
-// One symbol of cluster `cl` -> hybrid-uint value. Requires >= 32 buffered bits on entry.
-template <bool ANS_SMEM>
-__device__ __forceinline__ uint32_t hf_read_value(const HfTables& T, HfBits& br, uint32_t& ans_state, uint32_t cl) {
-  const uint32_t cfg = lds32(T.cfg + cl * 4);
-  uint32_t token;
-  if (T.use_prefix) {  // prefix.rs:335-357
-    const uint32_t off = __ldg(T.prefix_meta + cl * 2), root_bits = __ldg(T.prefix_meta + cl * 2 + 1);
-    const uint32_t peeked = uint32_t(br.buf) & 0x7fffu;
-    uint32_t e = __ldg(T.prefix + off + (peeked & ((1u << root_bits) - 1)));
-    if (e & 0x80000000u) {
-      const uint32_t sb = (e >> 16) & 0xff;
-      e = __ldg(T.prefix + off + (1u << root_bits) + (e & 0xffff) + ((peeked >> root_bits) & ((1u << sb) - 1)));
-    }
-    br.take((e >> 16) & 0xff);
-    token = e & 0xffff;
-  } else {  // ans.rs:276-330
-    const uint32_t state = ans_state;
-    const uint32_t idx = state & 0xfff;
-    const uint32_t i = idx >> T.log_bucket;
-    const uint32_t pos = idx & ((1u << T.log_bucket) - 1);
-    uint2 b;
-    if (ANS_SMEM) {
-      b = lds64(T.ans + (((cl << T.log_alphabet_size) + i) << 3));
-    } else {
-      const uint64_t g = __ldg(T.ans_g + ((size_t(cl) << T.log_alphabet_size) + i));
-      b = make_uint2(uint32_t(g), uint32_t(g >> 32));
-    }
-    const bool map_to_alias = pos >= ((b.x >> 8) & 0xff);
-    const uint32_t hi = map_to_alias ? b.y : 0u;
-    const uint32_t offset = (hi & 0xffff) + pos;
-    const uint32_t dist = (b.x >> 16) ^ (hi >> 16);
-    token = map_to_alias ? (b.x & 0xff) : i;
-    uint32_t next = (state >> 12) * dist + offset;
-    if (next < (1u << 16)) next = (next << 16) | br.take(16);
-    ans_state = next;
-  }
-  // hybrid uint (lib.rs:572-605)
-  const uint32_t split_exponent = cfg & 0xff;
-  const uint32_t split = 1u << split_exponent;
-  if (token < split) return token;
-  const uint32_t msb = (cfg >> 8) & 0xff, lsb = (cfg >> 16) & 0xff;
-  const uint32_t in_token = msb + lsb;
-  const uint32_t n = (split_exponent - in_token + ((token - split) >> in_token)) & 31;
-  br.top_up();
-  const uint32_t rest = br.take(n);
-  const uint32_t low = token & ((1u << lsb) - 1);
-  uint32_t t = (token >> lsb) & ((1u << msb) - 1);
-  t |= 1u << msb;
-  return uint32_t((((uint64_t(t) << n) | rest) << lsb) | low);
-}
-
 template <bool SUB, int W, bool ANS_SMEM>
 __global__ void __launch_bounds__(W * 32) decode_hf_warp_kernel(const uint8_t* __restrict__ cs, DevFrame f, DevHfParams p,
                                                                 const DevHfJob* __restrict__ jobs,
@@ -196,16 +85,16 @@ __global__ void __launch_bounds__(W * 32) decode_hf_warp_kernel(const uint8_t* _
   const int job_idx = blockIdx.x * W + int(warp);
   if (job_idx >= num_jobs || lane != 0) return;
 
-  HfTables T;
-  T.cfg = sm_addr(s_cfg);
-  T.ans = ANS_SMEM ? sm_addr(smem + L.ans) : 0;
+  HfTables<HfLds> T;
+  T.cfg = HfLds::addr(s_cfg);
+  T.ans = ANS_SMEM ? HfLds::addr(smem + L.ans) : 0;
   T.ans_g = p.code.ans;
   T.prefix = p.code.prefix;
   T.prefix_meta = p.code.prefix_meta;
   T.log_alphabet_size = p.code.log_alphabet_size;
   T.log_bucket = 12 - p.code.log_alphabet_size;
   T.use_prefix = p.code.use_prefix;
-  const uint32_t a_ctx = sm_addr(s_ctx), a_bctx = sm_addr(s_bctx);
+  const uint32_t a_ctx = HfLds::addr(s_ctx), a_bctx = HfLds::addr(s_bctx);
 
   const DevHfJob job = jobs[job_idx];
   HfBits br;
@@ -219,7 +108,7 @@ __global__ void __launch_bounds__(W * 32) decode_hf_warp_kernel(const uint8_t* _
     hfp = 0;
   }
   const uint32_t nbc = p.num_block_clusters;
-  const uint32_t a_cmap = sm_addr(smem + L.cmap) + hfp * L.cmap_stride;
+  const uint32_t a_cmap = HfLds::addr(smem + L.cmap) + hfp * L.cmap_stride;
   const uint32_t lf_idx_mul = (p.num_lf_thr[0] + 1) * (p.num_lf_thr[1] + 1) * (p.num_lf_thr[2] + 1);
   const uint32_t hf_idx_mul = p.num_qf_thr + 1;
   br.top_up();
@@ -281,7 +170,7 @@ __global__ void __launch_bounds__(W * 32) decode_hf_warp_kernel(const uint8_t* _
           }
         }
         const uint32_t idx = (ch_idx * hf_idx_mul + hf_idx) * lf_idx_mul + lf_idx;
-        const uint32_t block_ctx = lds8(a_bctx + idx);
+        const uint32_t block_ctx = HfLds::u8(a_bctx + idx);
         uint32_t predicted;
         const uint32_t nz_here = nz_row[c][sx];
         const uint32_t nz_left = sx ? nz_row[c][sx - 1] : 0;
@@ -290,7 +179,7 @@ __global__ void __launch_bounds__(W * 32) decode_hf_warp_kernel(const uint8_t* _
         else predicted = (nz_here + nz_left + 1) >> 1;
         const uint32_t pidx = predicted >= 8 ? 4 + predicted / 2 : predicted;
         br.top_up();
-        uint32_t non_zeros = hf_read_value<ANS_SMEM>(T, br, ans_state, lds8(a_cmap + block_ctx + pidx * nbc));
+        uint32_t non_zeros = hf_read_value<HfLds, ANS_SMEM>(T, br, ans_state, HfLds::u8(a_cmap + block_ctx + pidx * nbc));
         if (non_zeros > (63u << num_blocks_log)) {
           err = kDevInvalid;
           break;
@@ -305,15 +194,15 @@ __global__ void __launch_bounds__(W * 32) decode_hf_warp_kernel(const uint8_t* _
         uint32_t* plane = f.coeff[c];
         const size_t base = (size_t(sby0 + sy) * 8) * f.cw + size_t(sbx0 + sx) * 8;
         // context term of the remaining-non-zeros count; changes only after a non-zero coefficient
-        uint32_t nzc2 = lds8(a_ctx + 64 + ((non_zeros - 1) >> num_blocks_log)) * 2;
+        uint32_t nzc2 = HfLds::u8(a_ctx + 64 + ((non_zeros - 1) >> num_blocks_log)) * 2;
         for (uint32_t k = num_blocks, i = 0; k < size; ++k, ++i) {
-          const uint32_t cctx = nzc2 + lds8(a_ctx + (i >> num_blocks_log)) * 2 + prev_nonzero;
+          const uint32_t cctx = nzc2 + HfLds::u8(a_ctx + (i >> num_blocks_log)) * 2 + prev_nonzero;
           if (cctx >= 458) {
             err = kDevInvalid;
             break;
           }
           br.top_up();
-          const uint32_t ucoeff = hf_read_value<ANS_SMEM>(T, br, ans_state, lds8(a_blk + cctx));
+          const uint32_t ucoeff = hf_read_value<HfLds, ANS_SMEM>(T, br, ans_state, HfLds::u8(a_blk + cctx));
           if (ucoeff == 0) {
             prev_nonzero = 0;
             continue;
@@ -332,7 +221,7 @@ __global__ void __launch_bounds__(W * 32) decode_hf_warp_kernel(const uint8_t* _
           else *dst += cvv;
           prev_nonzero = 1;
           if (--non_zeros == 0) break;
-          nzc2 = lds8(a_ctx + 64 + ((non_zeros - 1) >> num_blocks_log)) * 2;
+          nzc2 = HfLds::u8(a_ctx + 64 + ((non_zeros - 1) >> num_blocks_log)) * 2;
         }
         if (br.pos() > job.bit_limit) err = kDevOverrun;
       }
@@ -344,44 +233,41 @@ __global__ void __launch_bounds__(W * 32) decode_hf_warp_kernel(const uint8_t* _
 }
 
 // ---------------------------------------------------------------------------------------------
-// One thread per stream (hf_lanes.cuh). A CTA of `blockDim.x` threads carries blockDim.x streams and
-// stages, once: context LUTs, hybrid-uint configs, block-context map, the cluster maps of every HF preset
-// (global memory when they exceed kLaneCmapSmemBytes), the ANS alias tables (same rule as above) and 96
-// bytes of non-zero-count row per stream.
-struct HfLaneSmem {
-  uint32_t ctxlut, small, configs, bctx, cmap, cmap_stride, nz, ans, total;
-};
-__host__ __device__ inline HfLaneSmem hf_lane_layout(const DevHfParams& p, uint32_t nthreads) {
-  HfLaneSmem L;
-  uint32_t off = 0;
-  auto take = [&](uint32_t bytes) {
-    uint32_t o = off;
-    off += (bytes + 15) & ~15u;
-    return o;
-  };
-  L.ctxlut = take(128);
-  L.small = take((27 + 39) * 4);
-  L.configs = take(p.code.num_clusters * 4);
-  L.bctx = take(p.block_ctx_map_size);
-  L.cmap_stride = 495 * p.num_block_clusters;
-  const uint32_t cmap_bytes = L.cmap_stride * p.num_hf_presets;
-  L.cmap = cmap_bytes <= kLaneCmapSmemBytes ? take(cmap_bytes) : 0xffffffffu;
-  L.nz = take(96 * nthreads);
-  uint32_t ab = p.code.use_prefix ? 0 : (p.code.num_clusters << p.code.log_alphabet_size) * 8;
-  L.ans = (!p.code.use_prefix && ab <= kHfAnsSmemBytes) ? take(ab) : 0xffffffffu;
-  L.total = off;
-  return L;
+// One thread per stream (hf_lanes.cuh). A CTA of `blockDim.x` threads carries blockDim.x streams and stages, once, the
+// tables of hf_lane_layout(). Its streams start from their groups' varblock lists (hf_block_list_kernel).
+
+// One CTA per group: the group's cells in raster order, 256 at a time, compacted with a ballot and a prefix over warps.
+template <bool SUB>
+__global__ void __launch_bounds__(256) hf_block_list_kernel(DevFrame f, DevHfParams p, uint2* __restrict__ list,
+                                                            uint32_t* __restrict__ counts) {
+  __shared__ uint32_t s_warp[8];
+  const uint32_t g = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const HfGroupRect r = hf_group_rect(f, p, g);
+  const uint32_t n = r.width * r.height;
+  uint2* out = list + size_t(g) * p.group_dim_blocks * p.group_dim_blocks;
+  uint32_t base = 0;
+  for (uint32_t i0 = 0; i0 < n; i0 += 256) {
+    uint2 rec;
+    const bool has = i0 + tid < n && hf_block_record<SUB>(f, p, r, i0 + tid, rec);
+    const uint32_t ballot = __ballot_sync(0xffffffffu, has);
+    if (lane == 0) s_warp[warp] = __popc(ballot);
+    __syncthreads();
+    uint32_t before = base, total = 0;
+    for (uint32_t w = 0; w < 8; ++w) {
+      before += w < warp ? s_warp[w] : 0;
+      total += s_warp[w];
+    }
+    if (has) out[before + __popc(ballot & ((1u << lane) - 1))] = rec;
+    base += total;
+    __syncthreads();
+  }
+  if (tid == 0) counts[g] = base;
 }
 
-template <bool SUB>
-__global__ void __launch_bounds__(256) hf_block_ctx_kernel(DevFrame f, DevHfParams p, uint32_t* __restrict__ out) {
-  const uint32_t bx = blockIdx.x * 32 + (threadIdx.x & 31), by = blockIdx.y * 8 + (threadIdx.x >> 5);
-  if (bx < f.bw && by < f.bh) out[size_t(by) * f.bw + bx] = hf_block_ctx_cell<SUB>(f, p, bx, by);
-}
-
-template <bool SUB>
+template <bool SUB, bool STAGED>
 __global__ void __launch_bounds__(128) decode_hf_lanes_kernel(const uint8_t* __restrict__ cs, DevFrame f, DevHfParams p,
-                                                              const uint32_t* __restrict__ blk_ctx,
+                                                              const uint2* __restrict__ list,
+                                                              const uint32_t* __restrict__ counts,
                                                               const DevHfJob* __restrict__ jobs,
                                                               uint64_t* __restrict__ end_bits, int* __restrict__ status,
                                                               int num_jobs, int first_pass) {
@@ -400,20 +286,31 @@ __global__ void __launch_bounds__(128) decode_hf_lanes_kernel(const uint8_t* __r
   uint32_t* s_small = reinterpret_cast<uint32_t*>(smem + L.small);
   for (uint32_t i = tid; i < 27; i += nthreads) s_small[i] = hf_pack_tinfo(i);
   for (uint32_t i = tid; i < 39; i += nthreads) s_small[27 + i] = p.order_offset[i];
-  HfLaneTables T;
-  T.tinfo = s_small;
-  T.order_offset = s_small + 27;
-  T.ctx = s_ctx;
-  T.cfg = s_cfg;
-  T.bctx = s_bctx;
-  T.cmap = p.code.cluster_map;
+  HfLaneView<HfLds> T;
+  T.tinfo = HfLds::addr(s_small);
+  T.order_offset = HfLds::addr(s_small + 27);
+  T.ctx = HfLds::addr(s_ctx);
+  T.bctx = HfLds::addr(s_bctx);
+  T.nz = HfLds::addr(smem + L.nz + tid);
+  T.nz_stride = nthreads;
   T.cmap_stride = L.cmap_stride;
+  T.cmap = 0;
+  T.cmap_ptr = p.code.cluster_map;
   if (L.cmap != 0xffffffffu) {
     uint8_t* s_cmap = smem + L.cmap;
     const uint32_t n = L.cmap_stride * p.num_hf_presets;
     for (uint32_t i = tid; i < n; i += nthreads) s_cmap[i] = __ldg(p.code.cluster_map + i);
-    T.cmap = s_cmap;
+    T.cmap = HfLds::addr(s_cmap);
+    T.cmap_ptr = s_cmap;
   }
+  T.code.cfg = HfLds::addr(s_cfg);
+  T.code.ans = 0;
+  T.code.ans_g = p.code.ans;
+  T.code.prefix = p.code.prefix;
+  T.code.prefix_meta = p.code.prefix_meta;
+  T.code.log_alphabet_size = p.code.log_alphabet_size;
+  T.code.log_bucket = 12 - p.code.log_alphabet_size;
+  T.code.use_prefix = p.code.use_prefix;
   T.cv.log_alphabet_size = p.code.log_alphabet_size;
   T.cv.use_prefix = p.code.use_prefix;
   T.cv.configs = s_cfg;
@@ -425,42 +322,58 @@ __global__ void __launch_bounds__(128) decode_hf_lanes_kernel(const uint8_t* __r
     const uint32_t quads = (p.code.num_clusters << p.code.log_alphabet_size) / 2;  // 2 buckets per 16 bytes
     const uint4* src = reinterpret_cast<const uint4*>(p.code.ans);
     for (uint32_t i = tid; i < quads; i += nthreads) s_ans[i] = __ldg(src + i);
+    T.code.ans = HfLds::addr(s_ans);
     T.cv.ans = reinterpret_cast<const uint64_t*>(s_ans);
   }
   __syncthreads();
   const int job_idx = blockIdx.x * int(nthreads) + int(tid);
   if (job_idx >= num_jobs) return;
   const DevHfJob job = jobs[job_idx];
-  hf_lane_decode<SUB>(cs, f, p, T, blk_ctx, job, smem + L.nz + tid, nthreads, first_pass, end_bits + job_idx,
-                      status + job_idx);
+  const uint32_t gb = p.group_dim_blocks;
+  hf_lane_stream<SUB, STAGED>(cs, f, p, T, list + size_t(job.group_idx) * gb * gb, __ldg(counts + job.group_idx), job,
+                              first_pass, end_bits + job_idx, status + job_idx);
 }
 
 }  // namespace
 
-void launch_hf_block_ctx(DevFrame f, DevHfParams p, uint32_t* out, cudaStream_t stream) {
-  const dim3 grid((f.bw + 31) / 32, (f.bh + 7) / 8);
-  if (f.subsampled) hf_block_ctx_kernel<true><<<grid, 256, 0, stream>>>(f, p, out);
-  else hf_block_ctx_kernel<false><<<grid, 256, 0, stream>>>(f, p, out);
+size_t hf_block_list_count(DevFrame f, DevHfParams p) {
+  const uint32_t gb = p.group_dim_blocks;
+  return size_t((f.bh + gb - 1) / gb) * p.groups_per_row;
 }
 
-void launch_decode_hf_lanes(const uint8_t* cs, DevFrame f, DevHfParams p, const uint32_t* blk_ctx, const DevHfJob* jobs,
-                            uint64_t* end_bits, int* status, int num_jobs, int first_pass, int streams_per_cta,
-                            cudaStream_t stream) {
+void launch_hf_block_list(DevFrame f, DevHfParams p, uint2* list, uint32_t* counts, cudaStream_t stream) {
+  const uint32_t groups = uint32_t(hf_block_list_count(f, p));
+  if (f.subsampled) hf_block_list_kernel<true><<<groups, 256, 0, stream>>>(f, p, list, counts);
+  else hf_block_list_kernel<false><<<groups, 256, 0, stream>>>(f, p, list, counts);
+}
+
+void launch_decode_hf_lanes(const uint8_t* cs, DevFrame f, DevHfParams p, const uint2* list, const uint32_t* counts,
+                            const DevHfJob* jobs, uint64_t* end_bits, int* status, int num_jobs, int first_pass,
+                            int streams_per_cta, cudaStream_t stream) {
   if (num_jobs <= 0) return;
   // C++ function-local statics are initialised once, thread-safely: no worker thread launches before the limits are set
   static const bool attr_set = [] {
-    cudaFuncSetAttribute(decode_hf_lanes_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(decode_hf_lanes_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(decode_hf_lanes_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(decode_hf_lanes_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(decode_hf_lanes_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(decode_hf_lanes_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     return true;
   }();
   (void)attr_set;
   const int nthreads = streams_per_cta <= 64 ? 64 : 128;
   const HfLaneSmem L = hf_lane_layout(p, uint32_t(nthreads));
   const int ctas = (num_jobs + nthreads - 1) / nthreads;
-  if (f.subsampled)
-    decode_hf_lanes_kernel<true><<<ctas, nthreads, L.total, stream>>>(cs, f, p, blk_ctx, jobs, end_bits, status, num_jobs, first_pass);
-  else
-    decode_hf_lanes_kernel<false><<<ctas, nthreads, L.total, stream>>>(cs, f, p, blk_ctx, jobs, end_bits, status, num_jobs, first_pass);
+#define JXLB_HF_LANES(SUB_, STAGED_)                                                                                 \
+  decode_hf_lanes_kernel<SUB_, STAGED_><<<ctas, nthreads, L.total, stream>>>(cs, f, p, list, counts, jobs, end_bits, \
+                                                                             status, num_jobs, first_pass)
+  if (hf_lane_staged(p, L)) {
+    if (f.subsampled) JXLB_HF_LANES(true, true);
+    else JXLB_HF_LANES(false, true);
+  } else {
+    if (f.subsampled) JXLB_HF_LANES(true, false);
+    else JXLB_HF_LANES(false, false);
+  }
+#undef JXLB_HF_LANES
 }
 
 namespace {

@@ -159,11 +159,13 @@ constexpr uint32_t kLaneCmapSmemBytes = 32 * 1024;
 void launch_decode_hf(const uint8_t* codestream, DevFrame f, DevHfParams p, const DevHfJob* jobs, uint64_t* end_bits,
                       int* status, int num_jobs, int first_pass, int warps_per_cta, cudaStream_t stream);
 // Same contract, one thread per stream (kernels/hf_lanes.cuh); `streams_per_cta` in {64, 128}.
-// `blk_ctx` (bw x bh words) comes from launch_hf_block_ctx: transform type and context offset of every varblock origin.
-void launch_hf_block_ctx(DevFrame f, DevHfParams p, uint32_t* out, cudaStream_t stream);
-void launch_decode_hf_lanes(const uint8_t* codestream, DevFrame f, DevHfParams p, const uint32_t* blk_ctx, const DevHfJob* jobs,
-                            uint64_t* end_bits, int* status, int num_jobs, int first_pass, int streams_per_cta,
-                            cudaStream_t stream);
+// `list` / `counts` come from launch_hf_block_list: per group (hf_block_list_count of them), its varblock origins in
+// raster order with their transform type and context offset, group_dim_blocks^2 records apart, and their number.
+size_t hf_block_list_count(DevFrame f, DevHfParams p);
+void launch_hf_block_list(DevFrame f, DevHfParams p, uint2* list, uint32_t* counts, cudaStream_t stream);
+void launch_decode_hf_lanes(const uint8_t* codestream, DevFrame f, DevHfParams p, const uint2* list, const uint32_t* counts,
+                            const DevHfJob* jobs, uint64_t* end_bits, int* status, int num_jobs, int first_pass,
+                            int streams_per_cta, cudaStream_t stream);
 
 struct DevLfDequantJob {
   DevLfGroupRect rect;

@@ -22,7 +22,7 @@ def model(name, data):
     print(f"{name}: {streams} streams in {warps} warps, {symbols} symbols ({symbols / max(streams, 1):.0f} per stream)")
     print(f"  warp trips {warp_trips} -> {symbols / max(warp_trips, 1):.1f} symbols per trip "
           f"(lane efficiency {symbols / max(warp_trips * 32, 1):.2f}); one-lane-per-warp kernel: {symbols} trips")
-    print(f"  trips with a lane on a non-zero count (block walk runs): {hdr_trips / max(warp_trips, 1):.2f}, "
+    print(f"  trips with a lane on a non-zero count (it may take its next varblock record): {hdr_trips / max(warp_trips, 1):.2f}, "
           f"with a lane on a coefficient: {coef_trips / max(warp_trips, 1):.2f}")
 
 
