@@ -184,6 +184,24 @@ int32_t jxlb_dequant_idct(jxlb_decoder* dec, const uint8_t* data, size_t size, f
  * channels = NULL first to size the buffers. */
 int32_t jxlb_modular_decode_groups(jxlb_decoder* dec, const uint8_t* data, size_t size, int32_t* const* channels,
                                    uint32_t num_channels, uint32_t stride, uint32_t* num_coded, uint32_t* dims, uint32_t dims_cap);
+/* ---- JPEG bitstream reconstruction (crates/jxl-oxide/src/lib.rs:797-904, crate jxl-jbr). A JPEG transcode carries a
+ * `jbrd` box; with it and the quantised coefficients of frame 0 the original .jpg is rebuilt byte for byte. Sequential
+ * scans only: progressive ones return JXLB_ERR_UNSUPPORTED. The box's data section is Brotli-compressed and read through
+ * the system libbrotlidec.so.1 (loaded on first use; JXLB_ERR_UNSUPPORTED when it is missing). ---- */
+/* JxlImage::jpeg_reconstruction_status for a complete file: 0 unavailable (no jbrd box), 1 available, 2 invalid
+ * (frame 0 is not a normal VarDCT frame, the box is malformed or truncated, or metadata it needs is missing).
+ * Host only: needs no decoder and no device; JXLB_ERR_INVALID_ARG (5) for a null pointer. */
+int32_t jxlb_jpeg_reconstruction_status(const uint8_t* data, size_t size);
+/* JxlImage::reconstruct_jpeg (lib.rs:852-904, jxl-jbr/src/reconstruct.rs, reconstruct/scan.rs): decodes frame 0 up to its
+ * quantised coefficients on the device, encodes the scans there (kernels/jpeg.cu) and writes the markers around them.
+ * The decoder keeps the file until its next decode or jxlb_release_frames; `jpeg_size` receives its length. Without a
+ * jbrd box: JXLB_ERR_UNSUPPORTED ("unavailable"); a box that does not fit the frame, a wrong data-section length or a
+ * symbol missing from its Huffman table: JXLB_ERR_BITSTREAM. The decode's device planes are freed before it returns,
+ * and the allocation budget of jxlb_decoder_create_ex applies. */
+int32_t jxlb_reconstruct_jpeg(jxlb_decoder* dec, const uint8_t* data, size_t size, size_t* jpeg_size);
+/* Copies the reconstructed file (jpeg_size bytes) to host memory. JXLB_ERR_INVALID_ARG when there is none or
+ * `dst_bytes` is too small. */
+int32_t jxlb_jpeg_copy(const jxlb_decoder* dec, uint8_t* dst, size_t dst_bytes);
 /* features::upsample (crates/jxl-render/src/features/upsampling.rs:45-132) with the default weight tables
  * (crates/jxl-image/src/lib.rs upsampling weights): `in` (w x h, stride in floats) -> `out` ((w * factor) x (h * factor)),
  * factor 2, 4 or 8; both DEVICE pointers. */

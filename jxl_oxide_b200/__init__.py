@@ -34,6 +34,7 @@ EXPORTED_SYMBOLS = [
     "jxlb_gaborish", "jxlb_epf", "jxlb_xyb_to_rgb", "jxlb_squeeze_inverse", "jxlb_rct_inverse", "jxlb_blend",
     "jxlb_pipeline_create", "jxlb_pipeline_destroy", "jxlb_pipeline_last_error", "jxlb_pipeline_preload", "jxlb_pipeline_submit",
     "jxlb_pipeline_wait", "jxlb_pipeline_release_output", "jxlb_pipeline_launch_count", "jxlb_pipeline_workers", "jxlb_pipeline_decoder",
+    "jxlb_jpeg_reconstruction_status", "jxlb_reconstruct_jpeg", "jxlb_jpeg_copy",
 ]
 
 
@@ -154,6 +155,12 @@ def load_library():
     L.jxlb_pipeline_workers.argtypes = [vp]
     L.jxlb_pipeline_decoder.argtypes = [vp, i32]
     L.jxlb_pipeline_decoder.restype = vp
+    L.jxlb_jpeg_reconstruction_status.argtypes = [ctypes.c_char_p, ctypes.c_size_t]
+    L.jxlb_jpeg_reconstruction_status.restype = i32
+    L.jxlb_reconstruct_jpeg.argtypes = [vp, ctypes.c_char_p, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t)]
+    L.jxlb_reconstruct_jpeg.restype = i32
+    L.jxlb_jpeg_copy.argtypes = [vp, vp, ctypes.c_size_t]
+    L.jxlb_jpeg_copy.restype = i32
     _lib = L
     return L
 
@@ -185,6 +192,15 @@ class Decoder:
         arr = (_Section * len(sections))(*[_Section(s, len(s)) for s in sections])
         opt = _Options(output_colour, max_frames)
         self._check(self._L.jxlb_decode_frame_sections(self._h, header, len(header), arr, len(sections), ctypes.byref(opt)))
+
+    def reconstruct_jpeg(self, data: bytes) -> bytes:
+        """JxlImage::reconstruct_jpeg: the original JPEG file of a JPEG transcode (a `jbrd` box), scans encoded on the GPU.
+        Releases this decoder's frames. JxlError UNSUPPORTED when the file has no reconstruction data."""
+        n = ctypes.c_size_t()
+        self._check(self._L.jxlb_reconstruct_jpeg(self._h, data, len(data), ctypes.byref(n)))
+        buf = ctypes.create_string_buffer(max(n.value, 1))
+        self._check(self._L.jxlb_jpeg_copy(self._h, buf, n.value))
+        return buf.raw[:n.value]
 
     def _stage_planes(self, fn, data, dtype):
         import torch
@@ -554,6 +570,8 @@ class JxlImage:
     """Mirror of jxl_oxide::JxlImage for the decode hot path."""
 
     def __init__(self, data: bytes, device=0, output_colour=0):
+        self._data = bytes(data)
+        self._jpeg_dec = None
         self._dec = Decoder(device)
         self._dec.decode(data, output_colour=output_colour)
         info = self._dec.image_info()
@@ -581,3 +599,19 @@ class JxlImage:
     @property
     def decoder(self):
         return self._dec
+
+    def jpeg_reconstruction_status(self):
+        """0 unavailable (no jbrd box), 1 available, 2 invalid (JxlImage::jpeg_reconstruction_status)."""
+        return jpeg_reconstruction_status(self._data)
+
+    def reconstruct_jpeg(self) -> bytes:
+        """The original JPEG file, rebuilt from the bytes this image was read from (on a decoder of its own, so the
+        decoded frames stay available)."""
+        if self._jpeg_dec is None:
+            self._jpeg_dec = Decoder(self._dec.device)
+        return self._jpeg_dec.reconstruct_jpeg(self._data)
+
+
+def jpeg_reconstruction_status(data: bytes) -> int:
+    """0 unavailable (no jbrd box), 1 available, 2 invalid; host-side parsing only, no device needed."""
+    return int(load_library().jxlb_jpeg_reconstruction_status(data, len(data)))

@@ -14,8 +14,8 @@ OUT = os.path.join(HERE, "libjxlb200.so")
 
 SOURCES = [
     "capi.cu", "cuda_backend.cu", "launch_tables.cc", "pipeline.cu",
-    "kernels/modular.cu", "kernels/modular_stream.cu", "kernels/entropy.cu", "kernels/blockinfo.cu", "kernels/vardct.cu", "kernels/filters.cu", "kernels/filters_fused.cu",
-    "host/entropy.cc", "host/headers.cc", "host/modular_syntax.cc", "host/frame_syntax.cc", "host/planner.cc", "host/icc.cc",
+    "kernels/modular.cu", "kernels/modular_stream.cu", "kernels/entropy.cu", "kernels/blockinfo.cu", "kernels/vardct.cu", "kernels/filters.cu", "kernels/filters_fused.cu", "kernels/jpeg.cu",
+    "host/entropy.cc", "host/headers.cc", "host/modular_syntax.cc", "host/frame_syntax.cc", "host/planner.cc", "host/icc.cc", "host/jbrd.cc",
 ]
 
 # -fmad=false: the reference's generic float path never contracts a*b+c (SimdVector::muladd is
@@ -68,7 +68,7 @@ def build(force=False, verbose=False):
     with concurrent.futures.ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as ex:
         objs = list(ex.map(compile_one, srcs))
     subprocess.check_call([nvcc, "--shared"] + ARCH + ["-Xcompiler", "-fPIC,-pthread"] + objs +
-                          ["-o", OUT, "-lcudart"], cwd=CSRC)
+                          ["-o", OUT, "-lcudart", "-ldl"], cwd=CSRC)
     return OUT
 
 

@@ -24,6 +24,8 @@ int32_t guarded(jxlb_decoder* dec, F f) {
 }
 
 void release(jxlb_decoder* dec) {
+  dec->jpeg.clear();
+  dec->jpeg.shrink_to_fit();
   if (!dec->have_result) return;
   for (DecodedFrame& f : dec->res.frames)
     for (View& v : f.channels) dec->be->free_plane(v.plane);
@@ -167,6 +169,49 @@ int32_t jxlb_decode_hf_groups(jxlb_decoder* dec, const uint8_t* data, size_t siz
   if (rc == JXLB_OK && width) *width = dims[0];
   if (rc == JXLB_OK && height) *height = dims[1];
   return rc;
+}
+
+int32_t jxlb_jpeg_reconstruction_status(const uint8_t* data, size_t size) {
+  if (!data) return JXLB_ERR_INVALID_ARG;
+  try {
+    return jpeg_reconstruction_status(data, size);
+  } catch (const Error&) {  // a malformed container
+    return 2;
+  }
+}
+
+int32_t jxlb_reconstruct_jpeg(jxlb_decoder* dec, const uint8_t* data, size_t size, size_t* jpeg_size) {
+  if (!dec || !data) return JXLB_ERR_INVALID_ARG;
+  if (jpeg_size) *jpeg_size = 0;
+  CudaBackend& be = *dec->be;
+  const int32_t rc = guarded(dec, [&] {
+    release(dec);
+    JpegJob job = prepare_jpeg_job(data, size);
+    dec->codestream = extract_codestream(data, size);
+    DecodeOptions o;
+    o.max_frames = 1;
+    be.jpeg_job = &job;
+    bool done = false;
+    try {
+      DecodeResult res = decode_codestream(be, dec->codestream.data(), dec->codestream.size(), o);
+      for (DecodedFrame& f : res.frames)
+        for (View& v : f.channels) be.free_plane(v.plane);
+    } catch (const JpegDone&) {
+      done = true;
+    }
+    be.jpeg_job = nullptr;
+    JXLB_CHECK(done, kErrBitstream, "the first frame is not a VarDCT frame: its JPEG reconstruction data is invalid");
+    dec->jpeg = std::move(job.out);
+  });
+  be.jpeg_job = nullptr;
+  if (rc == JXLB_OK && jpeg_size) *jpeg_size = dec->jpeg.size();
+  return rc;
+}
+
+int32_t jxlb_jpeg_copy(const jxlb_decoder* dec, uint8_t* dst, size_t dst_bytes) {
+  if (!dec || !dst || dec->jpeg.empty() || dst_bytes < dec->jpeg.size()) return JXLB_ERR_INVALID_ARG;
+  std::memcpy(dst, dec->jpeg.data(), dec->jpeg.size());
+  return JXLB_OK;
 }
 
 int32_t jxlb_dequant_idct(jxlb_decoder* dec, const uint8_t* data, size_t size, float* const planes[3], uint32_t stride,

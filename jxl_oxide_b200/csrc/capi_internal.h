@@ -15,6 +15,7 @@ struct jxlb_decoder {
   bool have_result = false;
   std::string error;
   std::vector<uint8_t> codestream;
+  std::vector<uint8_t> jpeg;  // the last jxlb_reconstruct_jpeg result
   struct Slot {
     std::vector<uint8_t> codestream;
     uint8_t* dptr = nullptr;

@@ -1186,4 +1186,109 @@ void CudaBackend::xyb_to_rgb(const View v[3], const ColorParams& p) {
   end_k();
 }
 
+// ---- JPEG reconstruction: the scans of the jbrd box encoded from the frame's quantised coefficients ----
+void CudaBackend::vardct_coefficients(const VarDctState& st) {
+  if (!jpeg_job) return;
+  assemble_jpeg(*jpeg_job, st, [&](const JpegScanPlan& plan, uint64_t, std::vector<uint8_t>* out) { return encode_jpeg_scan(st, plan, out); });
+  throw JpegDone();
+}
+
+uint64_t CudaBackend::encode_jpeg_scan(const VarDctState& st, const JpegScanPlan& plan, std::vector<uint8_t>* out) {
+  DevJpegScan p = plan.dev;
+  for (int c = 0; c < 3; ++c) {
+    const DevView cv = dev_view(View{st.coeff[c], 0, 0, 1, 1}), lv = dev_view(View{st.lf_quant[c], 0, 0, 1, 1});
+    p.coeff[c] = static_cast<const int32_t*>(cv.ptr);
+    p.lfq[c] = static_cast<const int32_t*>(lv.ptr);
+    p.coeff_stride = cv.stride;
+    p.lfq_stride = lv.stride;
+  }
+  const DevView xv = dev_view(View{st.x_from_y, 0, 0, 1, 1}), bv = dev_view(View{st.b_from_y, 0, 0, 1, 1});
+  p.cfl[0] = static_cast<const int32_t*>(xv.ptr);
+  p.cfl[1] = static_cast<const int32_t*>(bv.ptr);
+  p.cfl_stride = xv.stride;
+  const uint32_t nb = p.num_blocks, ni = p.num_intervals;
+  const uint32_t zero = 0;
+  const uint32_t* huff = static_cast<const uint32_t*>(upload_temp(plan.huff, sizeof(plan.huff)));
+  const uint32_t* ezr_b = static_cast<const uint32_t*>(upload_temp(p.num_ezr ? plan.ezr_block.data() : &zero, 4 * std::max(p.num_ezr, 1u)));
+  const uint32_t* ezr_c = static_cast<const uint32_t*>(upload_temp(p.num_ezr ? plan.ezr_count.data() : &zero, 4 * std::max(p.num_ezr, 1u)));
+  const std::vector<uint8_t>& padding = jpeg_job->header.padding;
+  const uint8_t* pad = static_cast<const uint8_t*>(upload_temp(padding.empty() ? reinterpret_cast<const uint8_t*>(&zero) : padding.data(),
+                                                               std::max<size_t>(padding.size(), 4)));
+  // scratch planes: freed on every path out of here
+  std::vector<int> planes;
+  struct Free {
+    CudaBackend* be;
+    std::vector<int>* ids;
+    ~Free() {
+      for (int id : *ids) be->free_plane(id);
+    }
+  } free_guard{this, &planes};
+  auto scratch = [&](size_t bytes, bool zero_fill) {
+    planes.push_back(alloc_plane(uint32_t((bytes + 3) / 4 + 1), 1, zero_fill));
+    return plane_ptr(planes.back());
+  };
+  const size_t temp_bytes = jpeg_scan_temp_bytes(std::max(nb, ni) + 1);
+  void* temp = scratch(temp_bytes, false);
+  uint64_t* lens = static_cast<uint64_t*>(scratch(8 * (size_t(nb) + 1), false));
+  uint64_t* boff = static_cast<uint64_t*>(scratch(8 * (size_t(nb) + 1), false));
+  uint64_t* iv = static_cast<uint64_t*>(scratch(8 * 4 * (size_t(ni) + 1), false));
+  uint64_t *ib = iv, *ibx = iv + (ni + 1), *ip = iv + 2 * (ni + 1), *ipx = iv + 3 * (ni + 1);
+  uint32_t* err = static_cast<uint32_t*>(scratch(4, true));
+  cudaStream_t s = S();
+
+  begin_k("jpeg_lengths");
+  launch_jpeg_lengths(p, huff, ezr_b, ezr_c, lens, err, s);
+  end_k();
+  begin_k("jpeg_prefix_sum");
+  launch_jpeg_scan_u64(lens, boff, nb + 1, temp, temp_bytes, s);
+  end_k();
+  begin_k("jpeg_intervals");
+  launch_jpeg_intervals(p, boff, ib, ip, s);
+  end_k();
+  begin_k("jpeg_prefix_sum");
+  launch_jpeg_scan_u64(ib, ibx, ni + 1, temp, temp_bytes, s);
+  end_k();
+  begin_k("jpeg_prefix_sum");
+  launch_jpeg_scan_u64(ip, ipx, ni + 1, temp, temp_bytes, s);
+  end_k();
+  const uint64_t* h_total = static_cast<const uint64_t*>(fetch_result(ibx + ni, 8));
+  const uint64_t* h_pad = static_cast<const uint64_t*>(fetch_result(ipx + ni, 8));
+  const uint32_t* h_err = static_cast<const uint32_t*>(fetch_result(err, 4));
+  sync();
+  JXLB_CHECK(!(*h_err & kJpegErrHuffman), kErrBitstream, "a JPEG symbol has no code in its Huffman table");
+  const uint64_t total = *h_total, pad_bits = *h_pad;
+  JXLB_CHECK(total / 4 < (uint64_t(1) << 31), kErrUnsupported, "JPEG scan too large");
+  const uint32_t nw = uint32_t((total + 3) / 4);
+
+  uint32_t* words = static_cast<uint32_t*>(scratch(4 * (size_t(nw) + 1), true));
+  uint32_t* cnt = static_cast<uint32_t*>(scratch(4 * (size_t(nw) + 1), false));
+  uint32_t* ffoff = static_cast<uint32_t*>(scratch(4 * (size_t(nw) + 1), false));
+  const size_t temp2_bytes = jpeg_scan_temp_bytes(nw + 1);
+  void* temp2 = temp2_bytes > temp_bytes ? scratch(temp2_bytes, false) : temp;
+  uint8_t* bytes = static_cast<uint8_t*>(scratch(2 * total + 2 * size_t(ni), false));
+  begin_k("jpeg_emit");
+  launch_jpeg_emit(p, huff, ezr_b, ezr_c, boff, ibx, ipx, pad, words, err, s);
+  end_k();
+  begin_k("jpeg_ff_count");
+  launch_jpeg_ff_count(words, total, nw, cnt, s);
+  end_k();
+  begin_k("jpeg_prefix_sum");
+  launch_jpeg_scan_u32(cnt, ffoff, nw + 1, temp2, std::max(temp_bytes, temp2_bytes), s);
+  end_k();
+  begin_k("jpeg_stuff");
+  launch_jpeg_stuff(words, total, nw, ffoff, ibx, ni, bytes, s);
+  end_k();
+  const uint32_t* h_ff = static_cast<const uint32_t*>(fetch_result(ffoff + nw, 4));
+  h_err = static_cast<const uint32_t*>(fetch_result(err, 4));
+  sync();
+  JXLB_CHECK(!(*h_err & kJpegErrPadding), kErrBitstream, "the jbrd box has fewer padding bits than the scans need");
+  JXLB_CHECK(!*h_err, kErrBitstream, "a JPEG symbol has no code in its Huffman table");
+  const size_t n = size_t(total) + *h_ff + 2 * (size_t(ni) - 1);
+  const size_t at = out->size();
+  out->resize(at + n);
+  CUDA_CHECK(cudaMemcpyAsync(out->data() + at, bytes, n, cudaMemcpyDeviceToHost, s));
+  sync();
+  return p.pad_avail_bits ? pad_bits : 0;
+}
+
 }  // namespace jxlb

@@ -10,6 +10,7 @@
 #include <vector>
 
 #include "host/backend.h"
+#include "host/jbrd.h"
 #include "kernels/kernels.h"
 #include "launch_tables.h"
 
@@ -86,6 +87,10 @@ class CudaBackend : public Backend, private TableSink {
                             const ColorParams* colour) override;
   void stage_marker(const char* name, const View* views, int n) override;
   void phase_mark(const char* name) override;
+  // JPEG reconstruction (jxlb_reconstruct_jpeg): with a job set, the frame's coefficients are encoded as the job's JPEG
+  // scans (kernels/jpeg.cu) and the decode ends with JpegDone.
+  void vardct_coefficients(const VarDctState& st) override;
+  JpegJob* jpeg_job = nullptr;
 
   // Heavy stage of a frame (everything that needs full-resolution planes): the planner announces it with the bytes it
   // is about to allocate; a pipeline (csrc/pipeline.cu) hooks in here to bound the number of frames past this point
@@ -169,6 +174,7 @@ class CudaBackend : public Backend, private TableSink {
     return make_dev_frame(st, [this](int id) { return plane_ptr(id); });
   }
   void ensure_static_tables();
+  uint64_t encode_jpeg_scan(const VarDctState& st, const JpegScanPlan& plan, std::vector<uint8_t>* out);
   void begin_k(const char* name);
   void end_k();
   struct PendingTiming {

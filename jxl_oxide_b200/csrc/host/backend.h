@@ -209,6 +209,9 @@ class Backend {
                                     bool /*sigma_is_constant*/, const ColorParams* /*colour*/) {
     return false;
   }
+  // Called once the quantised LF and HF coefficients of a VarDCT frame are complete, before anything dequantises them:
+  // where JPEG reconstruction (host/jbrd.h) takes the frame.
+  virtual void vardct_coefficients(const VarDctState& /*st*/) {}
   // Called by the planner at stage boundaries; a backend may snapshot planes for tests.
   virtual void stage_marker(const char* /*name*/, const View* /*views*/, int /*n*/) {}
   // Profiling hook: the planner finished the named host phase (wall clock since the previous mark).

@@ -626,6 +626,8 @@ HfGlobalSyntax parse_hf_global(BitReader& br, const ImageHeader& ih, const Frame
     for (uint32_t set = 0; set < 17; ++set) {
       MatrixParams p = defaults ? default_params(set) : parse_matrix_params(br, set, 1 + 3 * fh.num_lf_groups() + set, raw_decoder);
       build_matrix(p, set, dq->matrices[set]);
+      if (set == 0 && p.mode == MatrixParams::kRaw && std::round(1.0f / p.raw_denominator) == 2040.0f)
+        for (int c = 0; c < 3; ++c) dq->jpeg[c] = p.raw[c];
       uint32_t w, h;
       DequantMatrices::matrix_size(set, &w, &h);
       for (int c = 0; c < 3; ++c) {

@@ -95,6 +95,9 @@ struct DequantMatrices {
   // matrices[set][channel] : width*height floats (row-major, `width` = dequant_matrix_size().0)
   std::vector<float> matrices[17][3];
   std::vector<float> matrices_tr[17][3];
+  // JPEG transcodes: the raw DCT8 table's integer values per channel when its denominator is 1/2040, else empty
+  // (jpeg_quant_values, dequant.rs:616-629, 718-720)
+  std::vector<int32_t> jpeg[3];
   static void matrix_size(uint32_t set, uint32_t* w, uint32_t* h);
 };
 

@@ -1042,6 +1042,7 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
 }
 
 void FramePlanner::render_vardct(DecodedFrame*) {
+  be_.vardct_coefficients(st_);
   // LF: dequant, chroma-from-luma, adaptive smoothing (vardct/mod.rs:163-201, util.rs:254-290)
   std::vector<LfDequantJob> jobs;
   const uint32_t lfd = fh_.lf_group_dim();

@@ -8,6 +8,7 @@
 #include "../host/headers.h"
 #include "../host/modular_syntax.h"
 #include "common.cuh"
+#include "jpeg_blocks.cuh"
 
 namespace jxlb {
 
@@ -272,5 +273,20 @@ struct DevFusedFilterParams {
 };
 void launch_filters_fused(const DevView in[3], const DevView out[3], DevFusedFilterParams p, cudaStream_t stream);
 bool fused_filters_supported(uint32_t width, uint32_t height);
+
+// JPEG reconstruction: scan encoding of one scan (kernels/jpeg.cu, per-block code in jpeg_blocks.cuh). Bit offsets and
+// byte counts are 64-bit exclusive sums over n + 1 entries (the last one is the total).
+size_t jpeg_scan_temp_bytes(uint32_t max_items);
+void launch_jpeg_lengths(const DevJpegScan& p, const uint32_t* huff, const uint32_t* ezr_block, const uint32_t* ezr_count,
+                         uint64_t* lens, uint32_t* err, cudaStream_t s);
+void launch_jpeg_scan_u64(const uint64_t* in, uint64_t* out, uint32_t n, void* temp, size_t temp_bytes, cudaStream_t s);
+void launch_jpeg_scan_u32(const uint32_t* in, uint32_t* out, uint32_t n, void* temp, size_t temp_bytes, cudaStream_t s);
+void launch_jpeg_intervals(const DevJpegScan& p, const uint64_t* boff, uint64_t* ibytes, uint64_t* ipad, cudaStream_t s);
+void launch_jpeg_emit(const DevJpegScan& p, const uint32_t* huff, const uint32_t* ezr_block, const uint32_t* ezr_count,
+                      const uint64_t* boff, const uint64_t* ibx, const uint64_t* ipx, const uint8_t* pad, uint32_t* words,
+                      uint32_t* err, cudaStream_t s);
+void launch_jpeg_ff_count(const uint32_t* words, uint64_t total_bytes, uint32_t nw, uint32_t* cnt, cudaStream_t s);
+void launch_jpeg_stuff(const uint32_t* words, uint64_t total_bytes, uint32_t nw, const uint32_t* ffoff, const uint64_t* ibx,
+                       uint32_t nint, uint8_t* out, cudaStream_t s);
 
 }  // namespace jxlb
