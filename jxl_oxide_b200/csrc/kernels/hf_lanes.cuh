@@ -215,7 +215,7 @@ struct HfLaneView {
   using Addr = typename Mem::Addr;
   // Lanes index these with their own block's transform type / channel: from constant memory (kTInfo, the kernel
   // parameter bank) such a lookup costs one replay per distinct address, from shared memory it is one access.
-  Addr tinfo;         // [27] hf_pack_tinfo(): width | blocks << 8 | order id << 16 | transposed << 24
+  Addr tinfo;         // [27] hf_pack_tinfo(): width | log2(blocks) << 8 | order id << 16 | transposed << 24
   Addr order_offset;  // [13 * 3] copy of DevHfParams::order_offset
   Addr ctx;           // [0..63): coefficient frequency context, [64..127): non-zero-count context
   Addr bctx;          // block context map
@@ -232,9 +232,18 @@ struct HfLaneView {
 };
 
 __device__ __forceinline__ uint32_t hf_umin(uint32_t a, uint32_t b) { return a < b ? a : b; }
+// One transform type's record in `tinfo`: width in blocks | log2(number of blocks) << 8 | order id << 16 | transposed << 24.
+// The block count is stored as its logarithm (every varblock is a power of two of 8x8 blocks): DCT256 covers 1024 blocks,
+// which does not fit a byte.
 __device__ __forceinline__ uint32_t hf_pack_tinfo(uint32_t t) {
-  return uint32_t(kTInfo[t][0]) | (uint32_t(kTInfo[t][0]) * kTInfo[t][1]) << 8 | uint32_t(kTInfo[t][3]) << 16 |
-         uint32_t(kTInfo[t][4]) << 24;
+  const uint32_t blocks_log = 31u - uint32_t(__clz(int(uint32_t(kTInfo[t][0]) * kTInfo[t][1])));
+  return uint32_t(kTInfo[t][0]) | blocks_log << 8 | uint32_t(kTInfo[t][3]) << 16 | uint32_t(kTInfo[t][4]) << 24;
+}
+struct HfTinfo {
+  uint32_t w8, num_blocks_log, order_id, transpose;
+};
+__device__ __forceinline__ HfTinfo hf_unpack_tinfo(uint32_t ti) {
+  return HfTinfo{ti & 0xff, (ti >> 8) & 0xff, (ti >> 16) & 0xff, ti >> 24};
 }
 
 // Block context of one 8x8 cell (hf_coeff.rs:100-127): everything a stream needs to know about a varblock before its
@@ -373,12 +382,12 @@ __device__ __forceinline__ void hf_lane_stream(const uint8_t* __restrict__ cs, c
           if (--left) next = __ldg(list++);
           x = rec.y & 0xffff;
           y = rec.y >> 16;
-          const uint32_t ti = Mem::u32(T.tinfo + (rec.x & 0xff) * 4);
-          w8 = ti & 0xff;
-          num_blocks = (ti >> 8) & 0xff;
-          order_id = (ti >> 16) & 0xff;
-          transpose = ti >> 24;
-          num_blocks_log = 31u - uint32_t(__clz(int(num_blocks)));
+          const HfTinfo ti = hf_unpack_tinfo(Mem::u32(T.tinfo + (rec.x & 0xff) * 4));
+          w8 = ti.w8;
+          num_blocks_log = ti.num_blocks_log;
+          num_blocks = 1u << num_blocks_log;
+          order_id = ti.order_id;
+          transpose = ti.transpose;
           blk_ctx_idx = rec.x >> 8;
           ci = 0;
         }

@@ -113,6 +113,28 @@ extern "C" uint64_t jxle_hybrid_uint_selftest(uint64_t seed, uint32_t steps) {
   return 0;
 }
 
+// The packed records of the thread-per-stream HF decoder read back to what they were packed from: the transform-type
+// record of every type against kTransformInfo, and the varblock record at the largest values its fields can take
+// (type 26; context offset hf_idx * lf_idx_mul + lf_idx with 15 quant-field and 3 x 15 LF thresholds; x, y inside a
+// 1024-sample group). Returns 0 when all agree, otherwise 1 + the type that differs, or 100 + which record check failed.
+extern "C" int jxle_hf_record_check() {
+  using namespace jxlb;
+  for (uint32_t t = 0; t < kNumTransformTypes; ++t) {
+    const HfTinfo ti = hf_unpack_tinfo(hf_pack_tinfo(t));
+    const TransformTypeInfo& want = kTransformInfo[t];
+    if (ti.w8 != want.w8 || (1u << ti.num_blocks_log) != uint32_t(want.w8) * want.h8 || ti.order_id != want.order_id ||
+        ti.transpose != want.transpose)
+      return int(1 + t);
+  }
+  const uint32_t max_offset = 15u * (16u * 16u * 16u) + (16u * 16u * 16u - 1u);
+  const uint32_t max_type = kNumTransformTypes - 1, max_xy = 1024 / 8 - 1;
+  const uint2 rec = hf_block_rec(max_type | max_offset << 8, max_xy, max_xy);
+  if (rec.x == kHfNoBlock) return 100;
+  if ((rec.x & 0xff) != max_type || (rec.x >> 8) != max_offset) return 101;
+  if ((rec.y & 0xffff) != max_xy || (rec.y >> 16) != max_xy) return 102;
+  return 0;
+}
+
 namespace jxlo {
 
 class EmuBackend : public OracleBackend {

@@ -43,6 +43,12 @@ def test_strip_filter_matches_oracle_on_synthetic_frames(size, seed):
     _check(bench.synth_frame(size[0], size[1], seed), 3 * (size[0] - 100) * (size[1] - 100))
 
 
+@pytest.mark.parametrize("size,seed", [((1000, 600), 7), ((2600, 700), 5)])
+def test_strip_filter_matches_oracle_on_all_transform_types(size, seed):
+    # tools/synth_enc.cc --all-types: EPF sigma over 64x64 .. 256x256 varblocks (one quantisation value per varblock)
+    _check(bench.synth_frame(size[0], size[1], seed, extra=("--all-types",)), 3 * (size[0] - 100) * (size[1] - 100))
+
+
 def test_strip_filter_single_epf_step():
     # epf_iters == 1: step 1 is the last step and writes through the colour stage
     _check(bench.synth_frame(520, 392, 11, extra=("--epf-iters", "1")), 3 * 400 * 280)

@@ -70,8 +70,36 @@ def test_emulated_lanes_match_oracle_on_fixture(name):
 @pytest.mark.parametrize("extra", [(), ("--passes", "2"), ("--passes", "3"), ("--lf-frame",), ("--hf-presets", "3"),
                                    ("--hf-presets", "5", "--passes", "2")])
 def test_emulated_lanes_match_oracle_on_synthetic_frames(extra):
-    # ragged right / bottom groups, all 27 transform types, several groups per warp
+    # ragged right / bottom groups, 17 of the 27 transform types (DCT64 the largest), several groups per warp
     _same(bench.synth_frame(1000, 600, 7, extra=extra))
+
+
+# tools/synth_enc.cc --all-types: every one of the 27 transform types, DCT128 .. DCT256 (128 to 1024 blocks, order ids
+# 10-12) included, also in partial groups at the ragged edges; 2600 wide: on both sides of an LF-group boundary
+ALL_TYPES_FRAMES = [((1000, 600), 7), ((2600, 700), 5)]
+
+
+@pytest.mark.parametrize("extra", [(), ("--passes", "2"), ("--passes", "3"), ("--hf-presets", "5")],
+                         ids=["staged", "passes2", "passes3", "presets5_general"])
+@pytest.mark.parametrize("size,seed", ALL_TYPES_FRAMES)
+def test_emulated_lanes_match_oracle_on_all_transform_types(size, seed, extra):
+    # one HF preset: the staged variant (cluster maps and ANS tables in shared memory); five presets' cluster maps
+    # (37 KB) exceed the staging budget and select the general variant
+    _same(bench.synth_frame(size[0], size[1], seed, extra=("--all-types",) + extra))
+
+
+@pytest.mark.parametrize("ttype", [19, 21, 22, 23, 24, 25, 26])
+def test_emulated_lanes_match_oracle_on_one_transform_type(ttype):
+    # a frame tiled with DCT64x32 or one of the six largest types wherever it fits (DCT8 elsewhere)
+    _same(bench.synth_frame(1000, 600, 3, extra=("--only-type", str(ttype))))
+
+
+def test_lane_records_hold_every_transform_type():
+    """The transform-type records of the lanes decoder unpack to kTransformInfo for all 27 types (DCT256's 1024 blocks
+    included), and its varblock record keeps type, context offset and position at their largest values."""
+    L = oracle_lib.emu_lib()
+    L.jxle_hf_record_check.restype = ctypes.c_int
+    assert L.jxle_hf_record_check() == 0
 
 
 def test_emulated_lanes_reject_truncated_streams():

@@ -136,7 +136,8 @@ def test_stage_entry_points_match_pipeline(dec, oracle):
 @pytest.mark.parametrize("size,seed,extra", [((1000, 600), 5, ()), ((1544, 1032), 6, ("--lf-gradient",)),
                                              ((1000, 600), 7, ("--lf-frame",)), ((1000, 600), 5, ("--passes", "3"))])
 def test_synthetic_vardct_frames_bit_exact(dec, oracle, size, seed, extra):
-    """Frames from tools/synth_enc.cc (the bench workload generator): all 27 transform families,
+    """Frames from tools/synth_enc.cc (the bench workload generator): 17 of the 27 transform types, up to DCT64
+    (tests/test_zz_gpu_transforms.py has all 27),
     WP- or gradient-coded LF, EPF 2 iterations; an LF frame; HF coefficients split over three passes
     (pass_group.rs:150-170: later passes add `value << shift` to the coefficients of earlier ones)."""
     import bench

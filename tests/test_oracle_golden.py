@@ -442,6 +442,33 @@ def test_dct_known_answers(oracle, n, forward):
     assert np.abs(got - want).max() <= 1
 
 
+@pytest.mark.parametrize("n", [64, 128, 256])
+@pytest.mark.parametrize("forward", [True, False])
+def test_dct_known_answers_large(oracle, n, forward):
+    """The 64-, 128- and 256-point transforms of DCT64 .. DCT256 against the f64 closed form, on dense uniform +-1 inputs
+    as in the 2^-16 test above. That criterion does not hold here (the 256-point inverse is up to ~17 such units off), so
+    the bound is float32 roundoff: the recursion has log2(n) butterfly levels, each rounding an add and a multiply by a
+    constant, and a level's rounding error is scaled by its secant factor 1 / (2 cos(.)) before it reaches the output.
+    Allowed: 8 units of 2^-24 per level, relative to the l1 norm of the terms an output sums (sum_k alpha_k |c_k| for the
+    inverse, sqrt(2) / n sum_i |x_i| for the forward transform); the measured worst case is under half of that."""
+    L = oracle.lib()
+    L.jxlo_dct_2d.argtypes = [ctypes.c_void_p, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_int]
+    m = np.cos(np.pi * (np.arange(n)[:, None] + 0.5) * np.arange(n)[None, :] / n)  # m[i, k]: sample i of basis k
+    alpha = np.r_[1.0, np.full(n - 1, math.sqrt(2.0))]
+    rng = np.random.default_rng(n * 2 + int(forward))
+    for _ in range(16):
+        x = rng.uniform(-1.0, 1.0, size=n).astype(np.float32)
+        buf = x.copy()
+        L.jxlo_dct_2d(buf.ctypes.data, n, 1, int(forward))
+        x64 = x.astype(np.float64)
+        if forward:
+            want, l1 = (m.T @ x64) * alpha / n, math.sqrt(2.0) / n * np.abs(x64).sum()
+        else:
+            want, l1 = m @ (alpha * x64), (alpha * np.abs(x64)).sum()
+        bound = 8 * math.log2(n) * 2.0 ** -24 * l1
+        assert np.abs(buf.astype(np.float64) - want).max() <= bound
+
+
 def test_threads_do_not_change_results(oracle):
     data = fixture_bytes("opsin_inverse", "input.jxl")
     a, _, _ = oracle.OracleImage(data, threads=1).frame(0)

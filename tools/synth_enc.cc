@@ -11,6 +11,9 @@
 // coefficient orders, one HF preset, ANS everywhere.
 // The entropy-code headers it writes are read back with the product's own parser to derive the
 // exact alias tables, so encoder and decoder cannot disagree about symbol mapping.
+// For tests, --all-types puts every one of the 27 transform types into the frame (the largest ones also in the partial
+// groups at the right / bottom edges and next to LF-group boundaries), --only-type T tiles the frame with one type, and
+// --dump-blocks FILE writes the varblock layout; without these flags the output does not change.
 //
 // Not part of the product; not a general-purpose encoder (it does not transform an input image).
 #include <algorithm>
@@ -578,7 +581,89 @@ struct Args {
   uint32_t hf_presets = 1; // HF presets (hf_pass.rs): group g uses preset g % N, each preset has its own (rotated) cluster map
   std::string dump_raw;    // --modular: also write the source image (3 planes, int32 little endian) for lossless checks
   bool modular = false;    // a Modular lossless frame (RGB 8 bit, RCT + default Squeeze, weighted predictor) instead of VarDCT
+  bool all_types = false;  // every one of the 27 transform types in the frame (forced_layout), the rest drawn from all 27
+  int only_type = -1;      // tile every group with this transform type wherever it fits, DCT8 elsewhere
+  std::string dump_blocks; // write the varblock layout as text lines "x y type" (8x8 cells) in the order HfMetadata codes them
 };
+
+// Varblocks placed before the random layout is drawn (--all-types / --only-type): the transform type at each block's
+// top-left cell, -1 elsewhere. Groups are 32 x 32 cells.
+std::vector<int8_t> forced_layout(const Args& a, uint32_t bw, uint32_t bh) {
+  std::vector<int8_t> forced(size_t(bw) * bh, -1);
+  std::vector<int8_t> covered(size_t(bw) * bh, 0);
+  const uint32_t gcols = (bw + 31) / 32, grows = (bh + 31) / 32;
+  auto place = [&](int t, uint32_t x, uint32_t y) {
+    const uint32_t w = kTransformInfo[t].w8, h = kTransformInfo[t].h8;
+    if (x / 32 != (x + w - 1) / 32 || y / 32 != (y + h - 1) / 32 || x + w > bw || y + h > bh)
+      fprintf(stderr, "forced varblock %d at (%u, %u) does not fit its group\n", t, x, y), exit(2);
+    for (uint32_t dy = 0; dy < h; ++dy)
+      for (uint32_t dx = 0; dx < w; ++dx) {
+        if (covered[size_t(y + dy) * bw + x + dx]) fprintf(stderr, "forced varblocks overlap at (%u, %u)\n", x + dx, y + dy), exit(2);
+        covered[size_t(y + dy) * bw + x + dx] = 1;
+      }
+    forced[size_t(y) * bw + x] = int8_t(t);
+  };
+  auto group_size = [&](uint32_t gx, uint32_t gy, uint32_t* w, uint32_t* h) {
+    *w = std::min(32u, bw - gx * 32), *h = std::min(32u, bh - gy * 32);
+  };
+  if (a.only_type >= 0) {
+    const uint32_t w = kTransformInfo[a.only_type].w8, h = kTransformInfo[a.only_type].h8;
+    for (uint32_t gy = 0; gy < grows; ++gy)
+      for (uint32_t gx = 0; gx < gcols; ++gx) {
+        uint32_t gw, gh;
+        group_size(gx, gy, &gw, &gh);
+        for (uint32_t y = 0; y + h <= gh; y += h)
+          for (uint32_t x = 0; x + w <= gw; x += w) place(a.only_type, gx * 32 + x, gy * 32 + y);
+      }
+    return forced;
+  }
+  // The first three full groups hold a catalogue of all 27 types: DCT256 | DCT256x128, DCT128, DCT128x64, DCT64x32,
+  // DCT32x64 | DCT128x256, DCT64x128, DCT64 and a row of the 18 types of at most 32 x 32 samples.
+  std::vector<uint32_t> full;
+  for (uint32_t gy = 0; gy < grows && full.size() < 3; ++gy)
+    for (uint32_t gx = 0; gx < gcols && full.size() < 3; ++gx) {
+      uint32_t gw, gh;
+      group_size(gx, gy, &gw, &gh);
+      if (gw == 32 && gh == 32) full.push_back(gy * gcols + gx);
+    }
+  if (full.size() < 3) fprintf(stderr, "--all-types needs a frame with at least three full 256 x 256 groups\n"), exit(2);
+  auto origin = [&](uint32_t g, uint32_t* x, uint32_t* y) { *x = g % gcols * 32, *y = g / gcols * 32; };
+  uint32_t x0, y0;
+  origin(full[0], &x0, &y0);
+  place(kDct256, x0, y0);
+  origin(full[1], &x0, &y0);
+  place(kDct256x128, x0, y0);
+  place(kDct128, x0 + 16, y0);
+  place(kDct128x64, x0 + 16, y0 + 16);
+  place(kDct64x32, x0 + 24, y0 + 16);
+  place(kDct32x64, x0 + 24, y0 + 24);
+  origin(full[2], &x0, &y0);
+  place(kDct128x256, x0, y0);
+  place(kDct64x128, x0, y0 + 16);
+  place(kDct64, x0 + 16, y0 + 16);
+  const int small[] = {kDct32, kDct32x16, kDct16x32, kDct32x8, kDct8x32, kDct16, kDct16x8, kDct8x16, kDct8, kHornuss, kDct2,
+                       kDct4, kDct4x8, kDct8x4, kAfv0, kAfv1, kAfv2, kAfv3};
+  uint32_t sx = x0;
+  for (int t : small) place(t, sx, y0 + 24), sx += kTransformInfo[t].w8;
+  // Partial groups at the right / bottom edges and the groups on either side of an LF-group boundary (every 8 groups)
+  // get the largest type of at least 64 x 64 samples that fits at their origin.
+  const int big[] = {kDct256, kDct256x128, kDct128x256, kDct128, kDct128x64, kDct64x128, kDct64, kDct64x32, kDct32x64};
+  for (uint32_t gy = 0; gy < grows; ++gy)
+    for (uint32_t gx = 0; gx < gcols; ++gx) {
+      const uint32_t g = gy * gcols + gx;
+      if (std::find(full.begin(), full.end(), g) != full.end()) continue;
+      uint32_t gw, gh;
+      group_size(gx, gy, &gw, &gh);
+      const bool lf_edge = gx % 8 == 7 || (gx % 8 == 0 && gx) || gy % 8 == 7 || (gy % 8 == 0 && gy);
+      if (gw == 32 && gh == 32 && !lf_edge) continue;
+      for (int t : big)
+        if (kTransformInfo[t].w8 <= gw && kTransformInfo[t].h8 <= gh) {
+          place(t, gx * 32, gy * 32);
+          break;
+        }
+    }
+  return forced;
+}
 
 // ---- Modular lossless frame (BASELINE config #4): forward RCT (YCoCg, type 6), forward Squeeze with the default
 // parameter schedule (jxl-modular/src/transform.rs:285-341), channels split into the global / LF-group / pass-group
@@ -887,10 +972,15 @@ int main(int argc, char** argv) {
     else if (s == "--hf-presets") a.hf_presets = std::max(1, atoi(next().c_str()));
     else if (s == "--modular") a.modular = true;
     else if (s == "--dump-raw") a.dump_raw = next();
+    else if (s == "--all-types") a.all_types = true;
+    else if (s == "--only-type") a.only_type = atoi(next().c_str());
+    else if (s == "--dump-blocks") a.dump_blocks = next();
     else if (s == "-o") a.out = next();
     else fprintf(stderr, "unknown arg %s\n", s.c_str()), exit(2);
   }
   if (a.modular) return encode_modular(a);
+  if (a.only_type >= int(kNumTransformTypes) || (a.only_type >= 0 && a.all_types))
+    fprintf(stderr, "--only-type takes a transform type 0..26 (not with --all-types)\n"), exit(2);
   std::mt19937 rng(a.seed);
   auto uni = [&](double lo, double hi) { return lo + (hi - lo) * (double(rng()) / 4294967296.0); };
   const uint32_t W = a.width, H = a.height;
@@ -907,6 +997,17 @@ int main(int argc, char** argv) {
   const int mix_types[] = {kDct8, kDct8, kDct8, kDct16x8, kDct8x16, kDct16, kDct16, kDct32x16, kDct16x32, kDct32, kDct4x8, kDct8x4,
                            kAfv0, kDct4, kDct2, kHornuss, kDct64, kDct32x8, kDct8x32, kAfv3};
   std::vector<int8_t> occ(size_t(bw) * bh, 0);
+  std::vector<int8_t> forced;
+  if (a.all_types || a.only_type >= 0) {
+    forced = forced_layout(a, bw, bh);
+    for (uint32_t y = 0; y < bh; ++y)
+      for (uint32_t x = 0; x < bw; ++x) {
+        const int t = forced[size_t(y) * bw + x];
+        if (t < 0) continue;
+        for (uint32_t dy = 0; dy < kTransformInfo[t].h8; ++dy)
+          for (uint32_t dx = 0; dx < kTransformInfo[t].w8; ++dx) occ[size_t(y + dy) * bw + x + dx] = 1;
+      }
+  }
   std::vector<std::vector<Block>> lf_blocks(num_lf);
   std::vector<int32_t> blk_type(size_t(bw) * bh, -1), blk_mul(size_t(bw) * bh, 0);
   for (uint32_t lg = 0; lg < num_lf; ++lg) {
@@ -914,10 +1015,11 @@ int main(int argc, char** argv) {
     uint32_t lw = std::min(256u, bw - lx0), lh = std::min(256u, bh - ly0);
     for (uint32_t y = 0; y < lh; ++y)
       for (uint32_t x = 0; x < lw; ++x) {
-        if (occ[size_t(ly0 + y) * bw + lx0 + x]) continue;
-        int type = kDct8;
-        for (int attempt = 0; attempt < 4; ++attempt) {
-          int t = mix_types[rng() % (sizeof(mix_types) / sizeof(int))];
+        const int forced_type = forced.empty() ? -1 : forced[size_t(ly0 + y) * bw + lx0 + x];
+        if (forced_type < 0 && occ[size_t(ly0 + y) * bw + lx0 + x]) continue;
+        int type = forced_type < 0 ? kDct8 : forced_type;
+        for (int attempt = 0; forced_type < 0 && a.only_type < 0 && attempt < 4; ++attempt) {
+          int t = a.all_types ? int(rng() % kNumTransformTypes) : mix_types[rng() % (sizeof(mix_types) / sizeof(int))];
           uint32_t dw = kTransformInfo[t].w8, dh = kTransformInfo[t].h8;
           bool ok = (x % 32) + dw <= 32 && (y % 32) + dh <= 32 && x + dw <= lw && y + dh <= lh;
           for (uint32_t dy = 0; ok && dy < dh; ++dy)
@@ -935,6 +1037,13 @@ int main(int argc, char** argv) {
         blk_type[size_t(ly0 + y) * bw + lx0 + x] = type;
         blk_mul[size_t(ly0 + y) * bw + lx0 + x] = hf_mul;
       }
+  }
+  if (!a.dump_blocks.empty()) {
+    FILE* bf = fopen(a.dump_blocks.c_str(), "w");
+    if (!bf) return perror("fopen"), 1;
+    for (const auto& blocks : lf_blocks)
+      for (const Block& b : blocks) fprintf(bf, "%u %u %u\n", unsigned(b.x), unsigned(b.y), unsigned(b.type));
+    fclose(bf);
   }
   // LF quantised values: smooth field + small noise (Y large range, X/B small)
   std::vector<int32_t> lfq[3];
