@@ -93,6 +93,7 @@ cudaStream_t CudaBackend::S() {
     // A pipeline decoder has no stream of its own: the LF stage runs through the batch service, everything else on the
     // stream of a heavy slot. Whatever needs a stream before the planner announces the heavy stage takes the slot now.
     JXLB_CHECK(bool(on_need_stream), kErrCuda, "decoder has no CUDA stream");
+    if (!heavy_announced_ && (profile || host_phases)) ++profile_acc["host:slot_before_heavy"].first;  // taken early
     on_need_stream();
     JXLB_CHECK(stream_ != nullptr, kErrCuda, "no CUDA stream was leased to the decoder");
     if (pending_cs_bytes_) {  // encoded bytes staged for a batch that never came
@@ -537,6 +538,7 @@ const char* dev_status_message(int s) {
     case kDevOverrun: return "entropy-coded stream reads past the end of its section";
     case kDevInvalid: return "semantic validation of a decoded stream failed";
     case kDevUnsupported: return "chroma subsampling with varblocks larger than 8x8 is not supported";
+    case kDevBadLayout: return "invalid HfMetadata block layout";
     default: return "unknown device decode error";
   }
 }
@@ -635,10 +637,13 @@ void CudaBackend::decode_modular(std::vector<ModularStreamJob>& jobs) {
   }
   release_temps();
   for (size_t i = 0; i < jobs.size(); ++i) {
-    if (status[i] != kDevOk)
+    if (status[i] != kDevOk && status[i] != kDevBadLayout)
       fail(status[i] == kDevOverrun ? kErrEof : kErrDeviceDecode,
            std::string("modular stream ") + std::to_string(jobs[i].stream_index) + ": " + dev_status_message(status[i]));
     jobs[i].end_bit = size_t(end[i]);
+    // the stream's warp placed the LF group's varblocks (the planner reports a bad layout after the streams' errors)
+    jobs[i].placed = jobs[i].placement.group.nb_blocks != 0;
+    jobs[i].layout_ok = status[i] == kDevOk;
   }
 }
 
@@ -738,21 +743,12 @@ void CudaBackend::modular_xyb_to_float(const View yxb[3], const float m[3]) {
 
 void CudaBackend::build_block_info(VarDctState& st, const std::vector<BlockInfoJob>& jobs) {
   if (jobs.empty()) return;
-  std::vector<DevBlockInfoJob> dj;
-  for (const BlockInfoJob& j : jobs) {
-    const PlaneRec& raw = planes_.at(j.raw_plane);
-    dj.push_back({{j.rect.bx0, j.rect.by0, j.rect.bw, j.rect.bh}, static_cast<const int32_t*>(raw.ptr), raw.w, j.nb_blocks});
-  }
-  const EpfParams& epf = st.fh->restoration_filter.epf;
-  const DevBlockInfoJob* d_jobs = static_cast<const DevBlockInfoJob*>(upload_temp(dj.data(), dj.size() * sizeof(DevBlockInfoJob)));
-  const float* d_lut = static_cast<const float*>(upload_temp(epf.sharp_lut, sizeof(epf.sharp_lut)));
+  std::vector<DevPlacement> dp;
+  for (const BlockInfoJob& j : jobs) dp.push_back(make_dev_placement(varblock_placement(st, j), [this](const View& v) { return dev_view(v); }));
+  const DevPlacement* d_jobs = static_cast<const DevPlacement*>(upload_temp(dp.data(), dp.size() * sizeof(DevPlacement)));
   int* d_status = static_cast<int*>(stage_scratch(jobs.size() * 4));
-  float quant_mul_base = epf.quant_mul * 65536.0f / float(st.lfg->global_scale);
-  begin_k("build_block_info");
-  void* scratch = dmalloc(build_block_info_scratch_bytes(int(jobs.size())));
-  temps_.push_back(scratch);
-  launch_build_block_info(dev_frame(st), d_jobs, int(jobs.size()), quant_mul_base, d_lut, epf.iters > 0 ? 1 : 0, d_status,
-                          scratch, S());
+  begin_k("place_varblocks");
+  launch_place_varblocks(d_jobs, int(jobs.size()), d_status, S());
   end_k();
   const int* status = static_cast<const int*>(fetch_result(d_status, jobs.size() * 4));
   sync();

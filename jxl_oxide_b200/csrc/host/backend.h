@@ -29,6 +29,26 @@ struct ModularChannelTarget {
   int32_t hshift = 0, vshift = 0;
 };
 
+struct LfGroupRect {  // geometry of one LF group in 8x8-block units
+  uint32_t bx0 = 0, by0 = 0, bw = 0, bh = 0;
+};
+
+struct BlockInfoJob {  // HfMetadata post-processing (jxl-vardct/src/hf_metadata.rs:99-230)
+  LfGroupRect rect;
+  int raw_plane = -1;  // nb_blocks x 2
+  uint32_t nb_blocks = 0;
+};
+
+// The varblock placement of one LF group with everything it writes: the group's rectangle of the frame's blk_type /
+// blk_mul / epf_sigma planes (epf_sigma = quant_mul_base / hf_mul * sharp_lut[sharpness] when has_epf).
+struct VarblockPlacement {
+  BlockInfoJob group;  // nb_blocks == 0: no placement
+  int blk_type = -1, blk_mul = -1, epf_sigma = -1, sharpness = -1;
+  float quant_mul_base = 0.0f;
+  float sharp_lut[8] = {};
+  bool has_epf = false;
+};
+
 // One entropy-coded Modular channel-data stream (jxl-modular/src/image.rs:456-593).
 struct ModularStreamJob {
   size_t bit_pos = 0;        // absolute bit offset into the codestream where channel data begins
@@ -38,6 +58,12 @@ struct ModularStreamJob {
   uint32_t stream_index = 0;  // MA property 1
   std::vector<ModularChannelTarget> channels;
   size_t end_bit = 0;         // out: absolute bit offset after the stream
+  // HfMetadata stream without Modular transforms: its LF group's varblock placement, which a backend may run right
+  // after the stream (the list and the sharpness rectangle are final then). It reports that in `placed`, and the
+  // outcome in `layout_ok`; the planner runs the placements no backend ran through build_block_info().
+  VarblockPlacement placement;
+  bool placed = false;     // out
+  bool layout_ok = true;   // out
 };
 
 // One HF coefficient stream (one pass of one 256x256 group), jxl-vardct/src/hf_coeff.rs:21-252.
@@ -45,10 +71,6 @@ struct HfGroupJob {
   size_t bit_pos = 0, bit_limit = 0;
   uint32_t group_idx = 0, pass_idx = 0;
   size_t end_bit = 0;  // out
-};
-
-struct LfGroupRect {  // geometry of one LF group in 8x8-block units
-  uint32_t bx0 = 0, by0 = 0, bw = 0, bh = 0;
 };
 
 // Frame-level state of a VarDCT frame. Planes are allocated by the planner.
@@ -82,6 +104,20 @@ struct VarDctState {
   int coeff[3] = {-1, -1, -1};  // i32 coefficients -> f32 samples in place, (bw*8) x (bh*8)
 };
 
+inline VarblockPlacement varblock_placement(const VarDctState& st, const BlockInfoJob& group) {
+  const EpfParams& epf = st.fh->restoration_filter.epf;
+  VarblockPlacement p;
+  p.group = group;
+  p.blk_type = st.blk_type;
+  p.blk_mul = st.blk_mul;
+  p.epf_sigma = st.epf_sigma;
+  p.sharpness = st.sharpness;
+  p.quant_mul_base = epf.quant_mul * 65536.0f / float(st.lfg->global_scale);
+  for (int i = 0; i < 8; ++i) p.sharp_lut[i] = epf.sharp_lut[i];
+  p.has_epf = epf.iters > 0;
+  return p;
+}
+
 // The part of an LF-group rectangle channel c covers (shift_size of an even-sized rectangle).
 inline LfGroupRect shifted_rect(const LfGroupRect& r, uint32_t hshift, uint32_t vshift) {
   return LfGroupRect{r.bx0 >> hshift, r.by0 >> vshift, (r.bw + (1u << hshift) - 1) >> hshift, (r.bh + (1u << vshift) - 1) >> vshift};
@@ -90,12 +126,6 @@ inline LfGroupRect shifted_rect(const LfGroupRect& r, uint32_t hshift, uint32_t 
 struct LfDequantJob {  // copy_lf_dequant (jxl-render/src/vardct/mod.rs:387-412)
   LfGroupRect rect;
   float scale[3];  // X, Y, B
-};
-
-struct BlockInfoJob {  // HfMetadata post-processing (jxl-vardct/src/hf_metadata.rs:99-230)
-  LfGroupRect rect;
-  int raw_plane = -1;  // nb_blocks x 2
-  uint32_t nb_blocks = 0;
 };
 
 struct ColorParams {  // XYB -> (linear) sRGB, jxl-color/src/{xyb.rs,ciexyz.rs:81,tf/srgb.rs}
@@ -150,6 +180,8 @@ class Backend {
   virtual void int_to_float(const View& v, const BitDepth& depth) = 0;
   virtual void modular_xyb_to_float(const View yxb[3], const float m_lf_unscaled[3]) = 0;
   // VarDCT
+  // Varblock placement as a pass of its own, for the LF groups whose HfMetadata stream did not place them (see
+  // ModularStreamJob::placement).
   virtual void build_block_info(VarDctState& st, const std::vector<BlockInfoJob>& jobs) = 0;
   virtual void decode_hf(VarDctState& st, std::vector<HfGroupJob>& jobs) = 0;
   virtual void lf_dequant(VarDctState& st, const std::vector<LfDequantJob>& jobs) = 0;

@@ -660,13 +660,21 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
       chans.push_back({View{st_.sharpness, rc.bx0, rc.by0, rc.bw, rc.bh}, 0, 0});
       pend.push_back(prepare_stream(r, lf_limit[g], chans, 1 + 2 * num_lf_groups + g, &jobs));
       bjobs.push_back({rc, raw, nb_blocks});
+      // without Modular transforms the stream's own output is final: the backend may place right after the stream
+      if (pend.back().direct) jobs[pend.back().job_index].placement = varblock_placement(st_, bjobs.back());
     }
     be_.decode_modular(jobs);
     for (uint32_t g = 0; g < num_lf_groups; ++g) {
       finish_stream(pend[g]);
       lf_pos[g] = jobs[pend[g].job_index].end_bit;
     }
-    be_.build_block_info(st_, bjobs);
+    std::vector<BlockInfoJob> rest;  // LF groups the backend did not place with their stream
+    for (uint32_t g = 0; g < num_lf_groups; ++g) {
+      const ModularStreamJob& j = jobs[pend[g].job_index];
+      if (j.placed) JXLB_CHECK(j.layout_ok, kErrBitstream, "invalid HfMetadata block layout");
+      else rest.push_back(bjobs[g]);
+    }
+    if (!rest.empty()) be_.build_block_info(st_, rest);
     for (auto& b : bjobs) drop_plane(b.raw_plane);
   }
   be_.phase_mark("hf_metadata");

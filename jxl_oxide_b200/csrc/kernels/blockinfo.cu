@@ -1,153 +1,23 @@
-// HfMetadata post-processing (jxl-vardct/src/hf_metadata.rs:99-230) on the device.
-//
-// The placement scan is inherently serial (each varblock goes to the first unoccupied 8x8 cell in
-// raster order), so it is split in two:
-//   1. one warp per LF group: the (dct_select, hf_mul) list is staged through shared memory by
-//      all lanes, lane 0 runs the scan against a shared-memory occupancy bitmap (256 x 256 cells =
-//      8 KiB) and emits one record per varblock;
-//   2. a fully parallel kernel expands every record into the frame-global grids
-//      (blk_type / blk_mul / epf_sigma).
-#include "kernels.h"
+// Varblock placement as a launch of its own, for the HfMetadata streams that carry Modular transforms: their
+// (dct_select, hf_mul) lists are only final after the inverse transforms, so the stream's warp cannot place them. Every
+// other HfMetadata stream places its varblocks inside the stream kernel (modular_stream.cu); both run placement.cuh.
+#include "placement.cuh"
 
 namespace jxlb {
 
 namespace {
 
-__device__ __constant__ const uint8_t kBlkSize[27][2] = {
-    {1, 1}, {1, 1}, {1, 1}, {1, 1}, {2, 2}, {4, 4}, {1, 2}, {2, 1}, {1, 4}, {4, 1}, {2, 4}, {4, 2}, {1, 1}, {1, 1},
-    {1, 1}, {1, 1}, {1, 1}, {1, 1}, {8, 8}, {4, 8}, {8, 4}, {16, 16}, {8, 16}, {16, 8}, {32, 32}, {16, 32}, {32, 16}};
-
-struct BlockRec {
-  uint16_t x, y;  // cell position inside the frame grid
-  uint32_t type_mul;  // dct_select | hf_mul << 8 (hf_mul validated to fit)
-};
-
-constexpr uint32_t kStageRecords = 2048;
-
-__global__ void __launch_bounds__(32) place_blocks_kernel(DevFrame f, const DevBlockInfoJob* __restrict__ jobs,
-                                                           BlockRec* __restrict__ recs, uint32_t* __restrict__ rec_count,
-                                                           uint32_t rec_stride, int* __restrict__ status) {
-  __shared__ uint32_t occ[256][8];
-  __shared__ int32_t s_sel[kStageRecords], s_mul[kStageRecords];
-  const int j = blockIdx.x;
-  const uint32_t lane = threadIdx.x;
-  const DevBlockInfoJob job = jobs[j];
-  const DevLfGroupRect rc = job.rect;
-  for (uint32_t i = lane; i < 256 * 8; i += 32) (&occ[0][0])[i] = 0;
-  BlockRec* out = recs + size_t(j) * rec_stride;
-  const uint32_t words = (rc.bw + 31) / 32;
-  const uint32_t last_valid = (rc.bw & 31) ? ((1u << (rc.bw & 31)) - 1) : 0xffffffffu;
-  // scan state (meaningful in lane 0; broadcast after every staged chunk)
-  uint32_t data_idx = 0, y = 0, wi = 0;
-  int err = kDevOk;
-  bool full = rc.bw == 0 || rc.bh == 0;
-  while (!full && err == kDevOk) {
-    // all lanes stage the next chunk of (dct_select, hf_mul) records
-    const uint32_t staged_base = data_idx;
-    const uint32_t staged_n = min(kStageRecords, job.nb_blocks > data_idx ? job.nb_blocks - data_idx : 0u);
-    __syncwarp();
-    for (uint32_t i = lane; i < staged_n; i += 32) {
-      s_sel[i] = job.raw[staged_base + i];
-      s_mul[i] = job.raw[job.raw_stride + staged_base + i];
-    }
-    __syncwarp();
-    if (lane == 0) {  // the serial placement scan over this chunk
-      for (;;) {
-        // next unoccupied cell in raster order
-        uint32_t free_bits = 0;
-        while (y < rc.bh) {
-          free_bits = ~occ[y][wi] & (wi + 1 == words ? last_valid : 0xffffffffu);
-          if (free_bits) break;
-          if (++wi == words) {
-            wi = 0;
-            ++y;
-          }
-        }
-        if (y >= rc.bh) {
-          full = true;
-          break;
-        }
-        if (data_idx >= job.nb_blocks) {
-          err = kDevInvalid;  // cells left but no varblock to put there
-          break;
-        }
-        if (data_idx >= staged_base + staged_n) break;  // chunk consumed: stage more
-        const uint32_t x = wi * 32 + uint32_t(__ffs(int(free_bits)) - 1);
-        const int32_t sel = s_sel[data_idx - staged_base];
-        const int32_t hf_mul = s_mul[data_idx - staged_base] + 1;
-        if (sel < 0 || sel >= 27 || hf_mul <= 0 || hf_mul >= (1 << 24)) {
-          err = kDevInvalid;
-          break;
-        }
-        const uint32_t dw = kBlkSize[sel][0], dh = kBlkSize[sel][1];
-        if ((x % 32) + dw > 32 || (y % 32) + dh > 32 || x + dw > rc.bw || y + dh > rc.bh) {
-          err = kDevInvalid;
-          break;
-        }
-        const uint32_t mask = (dw >= 32 ? 0xffffffffu : ((1u << dw) - 1)) << (x & 31);
-        uint32_t clash = 0;
-        for (uint32_t dy = 0; dy < dh; ++dy) {
-          clash |= occ[y + dy][wi] & mask;
-          occ[y + dy][wi] |= mask;
-        }
-        if (clash) {  // varblocks overlap
-          err = kDevInvalid;
-          break;
-        }
-        out[data_idx] = {uint16_t(rc.bx0 + x), uint16_t(rc.by0 + y), uint32_t(sel) | (uint32_t(hf_mul) << 8)};
-        ++data_idx;
-      }
-    }
-    data_idx = __shfl_sync(0xffffffffu, data_idx, 0);
-    err = __shfl_sync(0xffffffffu, err, 0);
-    full = __shfl_sync(0xffffffffu, int(full), 0) != 0;
-  }
-  if (lane == 0) {
-    rec_count[j] = data_idx;
-    status[j] = err;
-  }
-}
-
-__global__ void expand_blocks_kernel(DevFrame f, const BlockRec* __restrict__ recs, const uint32_t* __restrict__ rec_count,
-                                     uint32_t rec_stride, float quant_mul_base, const float* __restrict__ sharp_lut,
-                                     int has_epf, int* __restrict__ status) {
-  const int j = blockIdx.y;
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= rec_count[j]) return;
-  const BlockRec r = recs[size_t(j) * rec_stride + i];
-  const uint32_t sel = r.type_mul & 0xff;
-  const int32_t hf_mul = int32_t(r.type_mul >> 8);
-  const uint32_t dw = kBlkSize[sel][0], dh = kBlkSize[sel][1];
-  const float sigma_q = __fdiv_rn(quant_mul_base, float(hf_mul));
-  for (uint32_t dy = 0; dy < dh; ++dy)
-    for (uint32_t dx = 0; dx < dw; ++dx) {
-      const size_t gi = size_t(r.y + dy) * f.bw + r.x + dx;
-      f.blk_type[gi] = (dx == 0 && dy == 0) ? int32_t(sel) : -int32_t(1 + dx + 32 * dy);
-      f.blk_mul[gi] = hf_mul;
-      if (has_epf) {
-        const int32_t s = f.sharpness[gi];
-        if (s < 0 || s >= 8) {
-          status[j] = kDevInvalid;
-          continue;
-        }
-        f.epf_sigma[gi] = __fmul_rn(sigma_q, sharp_lut[s]);
-      }
-    }
+__global__ void __launch_bounds__(32) place_varblocks_kernel(const DevPlacement* __restrict__ jobs, int* __restrict__ status) {
+  __shared__ PlaceShared s;
+  const int err = place_varblocks(PlaceWarp{threadIdx.x}, s, jobs[blockIdx.x]);
+  if (threadIdx.x == 0) status[blockIdx.x] = err;
 }
 
 }  // namespace
 
-void launch_build_block_info(DevFrame f, const DevBlockInfoJob* jobs, int num_jobs, float quant_mul_base,
-                             const float* sharp_lut8, int has_epf, int* status, void* scratch, cudaStream_t stream) {
+void launch_place_varblocks(const DevPlacement* jobs, int num_jobs, int* status, cudaStream_t stream) {
   if (num_jobs <= 0) return;
-  const uint32_t rec_stride = 65536;
-  BlockRec* recs = static_cast<BlockRec*>(scratch);
-  uint32_t* counts = reinterpret_cast<uint32_t*>(recs + size_t(num_jobs) * rec_stride);
-  place_blocks_kernel<<<num_jobs, 32, 0, stream>>>(f, jobs, recs, counts, rec_stride, status);
-  dim3 grid(rec_stride / 128, num_jobs);
-  expand_blocks_kernel<<<grid, 128, 0, stream>>>(f, recs, counts, rec_stride, quant_mul_base, sharp_lut8, has_epf, status);
+  place_varblocks_kernel<<<num_jobs, 32, 0, stream>>>(jobs, status);
 }
-
-size_t build_block_info_scratch_bytes(int num_jobs) { return size_t(num_jobs) * 65536 * sizeof(BlockRec) + size_t(num_jobs) * 4 + 64; }
 
 }  // namespace jxlb

@@ -13,6 +13,7 @@ enum DevStatus : int {
   kDevOverrun = 2,     // read past the end of the section
   kDevInvalid = 3,     // semantic validation failed (e.g. non_zeros too large)
   kDevUnsupported = 4, // valid syntax outside the implemented set
+  kDevBadLayout = 5,   // HfMetadata: the varblocks do not tile their LF group (placement.cuh)
 };
 
 struct DevEntropyCode {

@@ -29,6 +29,25 @@ struct DevChannelPlan {
   uint32_t lut_len, lut_offset;  // u16 leaf-node indices at job.luts[lut_offset ...]
 };
 
+// Varblock placement of one LF group (HfMetadata post-processing, jxl-vardct/src/hf_metadata.rs:99-230; see
+// placement.cuh): the (dct_select, hf_mul - 1) list in, the group's rectangle of the frame's block grids out.
+struct DevPlacement {
+  const int32_t* raw;  // nb_blocks x 2 (stride raw_stride); null: no placement
+  uint32_t raw_stride, nb_blocks;
+  uint32_t bw, bh;     // the LF group in 8x8 blocks
+  uint32_t grid_stride;  // of the four grids below, which point at the group's top-left cell
+  int32_t* blk_type;
+  int32_t* blk_mul;
+  float* epf_sigma;
+  const int32_t* sharpness;
+  float quant_mul_base;
+  float sharp_lut[8];
+  uint32_t has_epf;
+};
+// Shared memory one placement warp needs (placement.cuh: PlaceShared); a Modular launch with HfMetadata jobs reserves at
+// least this much per CTA.
+constexpr size_t kPlaceSharedBytes = 2112;
+
 struct DevModularJob {
   uint64_t bit_pos, bit_limit;
   const MaNode* tree;
@@ -43,6 +62,7 @@ struct DevModularJob {
   uint32_t use_wp;
   int32_t* wp_scratch;   // 5 * max_width ints when use_wp
   uint32_t* lz_window;   // when code.lz77_enabled
+  DevPlacement place;    // HfMetadata streams: the LF group's varblock placement, run by the stream's warp after the decode
 };
 
 struct DevView {
@@ -105,11 +125,6 @@ void launch_fill_u32(uint32_t* p, size_t n, uint32_t value, cudaStream_t stream)
 struct DevLfGroupRect {
   uint32_t bx0, by0, bw, bh;
 };
-struct DevBlockInfoJob {
-  DevLfGroupRect rect;
-  const int32_t* raw;  // nb_blocks x 2 (stride raw_stride)
-  uint32_t raw_stride, nb_blocks;
-};
 struct DevFrame {  // frame-global grids (device pointers), all with stride == their width
   uint32_t width, height, bw, bh;      // pixels / 8x8 blocks
   uint32_t cw, ch;                     // coefficient plane size (bw*8, bh*8)
@@ -128,10 +143,10 @@ struct DevFrame {  // frame-global grids (device pointers), all with stride == t
   uint32_t group_blocks;  // group_dim / 8
   uint8_t hshift[3], vshift[3], subsampled;
 };
-void launch_build_block_info(DevFrame f, const DevBlockInfoJob* jobs, int num_jobs, float quant_mul_base,
-                             const float* sharp_lut8 /*device*/, int has_epf, int* status, void* scratch,
-                             cudaStream_t stream);
-size_t build_block_info_scratch_bytes(int num_jobs);
+// The placement of HfMetadata streams with Modular transforms, whose lists are only final after the inverse transforms
+// (the other HfMetadata streams place their varblocks in the stream kernel): one warp per job; status kDevBadLayout or
+// kDevOk per job.
+void launch_place_varblocks(const DevPlacement* jobs, int num_jobs, int* status, cudaStream_t stream);
 
 struct DevHfParams {
   DevEntropyCode code;

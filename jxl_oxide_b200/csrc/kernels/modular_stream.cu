@@ -1,5 +1,6 @@
 // Modular stream decode: one warp per entropy-coded Modular stream (LfCoeff, ModularLfGroup,
-// HfMetadata, GlobalModular, pass-group modular data).
+// HfMetadata, GlobalModular, pass-group modular data). After an HfMetadata stream the same warp places the LF group's
+// varblocks (placement.cuh), so the placement rides whatever launch or batch the stream rides.
 //
 // A stream is strictly serial (one ANS state; each sample's context depends on already decoded
 // neighbours), so the kernel is built around the shortest dependent-instruction chain per sample:
@@ -17,6 +18,7 @@
 // Integer semantics are those of crates/jxl-modular/src/{image.rs:456-593,1169-1260, predictor.rs,
 // ma.rs} (bit-exact, wrapping i32).
 #include "modular_lanes.cuh"
+#include "placement.cuh"
 
 namespace jxlb {
 
@@ -113,9 +115,16 @@ __device__ __forceinline__ void modular_stream_body(uint8_t* smem, const uint8_t
     fs.rows_b = reinterpret_cast<int32_t*>(smem + L.fast_rows);
   }
   decode_stream_channels(DeviceWarp{lane}, job, cv, tree, luts, chans, chplans, wp_rows, s_div, fs, s);
+  int err = __shfl_sync(0xffffffffu, s.err, 0);
+  if (job.place.raw && err == kDevOk) {
+    // HfMetadata: the warp places the LF group's varblocks in the shared memory the tables were staged in (the launch
+    // reserves at least sizeof(PlaceShared)); the raw list and the sharpness rectangle are what lane 0 just wrote
+    __syncwarp();
+    err = place_varblocks(PlaceWarp{lane}, *reinterpret_cast<PlaceShared*>(smem), job.place);
+  }
   if (lane != 0) return;
   end_bits[job_idx] = s.br.pos();
-  status[job_idx] = s.err;
+  status[job_idx] = err;
   if (trace) {
     unsigned long long now;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));

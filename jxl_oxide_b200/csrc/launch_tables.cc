@@ -266,11 +266,38 @@ ModularLaunch build_modular_launch(const std::vector<ModularStreamJob>& jobs,
       L.needs[i].whole_tree = true;
     }
     L.smem_bytes = std::max(L.smem_bytes, modular_job_smem_bytes(d, max_w));
+    if (j.placement.group.nb_blocks) {
+      d.place = make_dev_placement(j.placement, view_to_dev);
+      L.smem_bytes = std::max(L.smem_bytes, kPlaceSharedBytes);
+    }
     L.all_staged = L.all_staged && modular_job_all_staged(d, max_w);
     if (d.use_wp && max_w) L.needs[i].wp_scratch_bytes = size_t(max_w) * 5 * 4;
     if (d.code.lz77_enabled) L.needs[i].lz_window_bytes = size_t(std::min<uint64_t>(1u << 20, std::max<uint64_t>(samples, 1))) * 4;
   }
   return L;
+}
+
+DevPlacement make_dev_placement(const VarblockPlacement& p, const std::function<DevView(const View&)>& view_to_dev) {
+  const BlockInfoJob& g = p.group;
+  DevPlacement d;
+  std::memset(&d, 0, sizeof(d));
+  const DevView raw = view_to_dev(View{g.raw_plane, 0, 0, g.nb_blocks, 2});
+  d.raw = static_cast<const int32_t*>(raw.ptr);
+  d.raw_stride = raw.stride;
+  d.nb_blocks = g.nb_blocks;
+  d.bw = g.rect.bw;
+  d.bh = g.rect.bh;
+  auto grid = [&](int plane) { return view_to_dev(View{plane, g.rect.bx0, g.rect.by0, g.rect.bw, g.rect.bh}); };
+  const DevView type = grid(p.blk_type);
+  d.grid_stride = type.stride;
+  d.blk_type = static_cast<int32_t*>(type.ptr);
+  d.blk_mul = static_cast<int32_t*>(grid(p.blk_mul).ptr);
+  d.epf_sigma = static_cast<float*>(grid(p.epf_sigma).ptr);
+  d.sharpness = static_cast<const int32_t*>(grid(p.sharpness).ptr);
+  d.quant_mul_base = p.quant_mul_base;
+  for (int i = 0; i < 8; ++i) d.sharp_lut[i] = p.sharp_lut[i];
+  d.has_epf = p.has_epf ? 1 : 0;
+  return d;
 }
 
 std::vector<uint32_t> natural_order_table(uint32_t offset[13]) {

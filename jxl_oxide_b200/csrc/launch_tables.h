@@ -23,7 +23,8 @@ void pack_wp(const WpHeader& w, uint32_t out[11]);  // p1 p2 p3a p3b p3c p3d p3e
 // Channel subtrees with more nodes than this are not copied per job: the job walks the frame's whole tree instead.
 constexpr size_t kMaxChannelTreeNodes = 60000;
 
-// One Modular launch. The jobs' global scratch (wp_scratch, lz_window) is left null for the caller to fill.
+// One Modular launch. The jobs' global scratch (wp_scratch, lz_window) is left null for the caller to fill. A job with a
+// varblock placement carries it (DevModularJob::place), and the launch reserves kPlaceSharedBytes per CTA at least.
 struct ModularLaunch {
   struct JobNeeds {
     size_t wp_scratch_bytes = 0, lz_window_bytes = 0;
@@ -41,6 +42,9 @@ struct ModularLaunch {
 ModularLaunch build_modular_launch(const std::vector<ModularStreamJob>& jobs,
                                    const std::function<DevView(const View&)>& view_to_dev, TableSink& sink,
                                    size_t max_channel_tree_nodes = kMaxChannelTreeNodes);
+
+// The device form of a varblock placement (kernels/placement.cuh).
+DevPlacement make_dev_placement(const VarblockPlacement& p, const std::function<DevView(const View&)>& view_to_dev);
 
 // The 13 natural coefficient orders back to back; offset[id] is where order `id` starts.
 std::vector<uint32_t> natural_order_table(uint32_t offset[13]);

@@ -10,6 +10,7 @@
 // slab the full-resolution planes are carved from, so a frame costs no allocator call. HBM use grows with both counts:
 // heavy_frames x slab, and per worker its LF arena and the memory pool of its decoder (which keeps what it held). Frames flow without barriers, so the contexts de-phase by themselves and
 // the GPU-filling stages of some frames overlap the latency-bound stages of others.
+#include <chrono>
 #include <condition_variable>
 #include <cstdio>
 #include <cstdlib>
@@ -451,16 +452,28 @@ struct jxlb_pipeline {
     // A heavy slot = slab + stream. The planner's begin_heavy_stage() takes the slot for its memory; the stream is handed
     // to the decoder only when it first needs one (a Modular frame decodes all its streams through the batch service
     // and wants the stream for the inverse transforms only).
-    dec->be->on_heavy_stage = [&](size_t hint) {
-      if (held >= 0) return;  // a later frame of the same image: it shares the slot (overflow goes to the pool)
+    // With profiling on, the decoder's phase profile gets host:slot_wait (acquire to grant) and host:slot_hold (grant to
+    // release) per frame: the hold is what bounds the frames per second at `heavy_frames` slots.
+    std::chrono::steady_clock::time_point granted;
+    auto profiled = [&] { return dec->be->profile || dec->be->host_phases; };
+    auto add_ms = [&](const char* name, std::chrono::steady_clock::time_point since, std::chrono::steady_clock::time_point now) {
+      auto& acc = dec->be->profile_acc[name];
+      acc.first += 1;
+      acc.second += std::chrono::duration<double, std::milli>(now - since).count();
+    };
+    auto take_slot = [&](size_t hint) {
+      const auto t0 = std::chrono::steady_clock::now();
       held = acquire_slab(hint);
+      granted = std::chrono::steady_clock::now();
+      if (profiled()) add_ms("host:slot_wait", t0, granted);
       dec->be->set_arena(slabs[size_t(held)].base, slabs[size_t(held)].bytes);
     };
+    dec->be->on_heavy_stage = [&](size_t hint) {
+      if (held >= 0) return;  // a later frame of the same image: it shares the slot (overflow goes to the pool)
+      take_slot(hint);
+    };
     dec->be->on_need_stream = [&] {
-      if (held < 0) {
-        held = acquire_slab(0);
-        dec->be->set_arena(slabs[size_t(held)].base, slabs[size_t(held)].bytes);
-      }
+      if (held < 0) take_slot(0);
       dec->be->set_stream(slabs[size_t(held)].stream);
     };
     dec->be->lf_service = batcher.get();
@@ -547,6 +560,7 @@ struct jxlb_pipeline {
         }
         release_slab(held);
         held = -1;
+        if (profiled()) add_ms("host:slot_hold", granted, std::chrono::steady_clock::now());
       }
       {
         std::lock_guard<std::mutex> lk(mu);

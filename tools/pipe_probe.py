@@ -68,6 +68,13 @@ def main():
                 if n:
                     acc[p] = round(ms / n, 1)
             line += "\n    wall ms per frame by host phase: %s  (sum %.0f)" % (acc, sum(acc.values()))
+            # heavy slot: acquire -> grant, grant -> release (ms per frame), and streams taken before begin_heavy_stage()
+            slot = {}
+            for p in ("slot_wait", "slot_hold"):
+                n = sum(d.profile("host:" + p)[0] for d in decs)
+                slot[p] = round(sum(d.profile("host:" + p)[1] for d in decs) / n, 1) if n else None
+            slot["slot_before_heavy"] = sum(d.profile("host:slot_before_heavy")[0] for d in decs)
+            line += "\n    heavy slot: %s" % slot
         if trace:  # per Modular launch: host launch -> device start, device run, device end -> host return
             q, run_ms, wake = [], [], []
             for d in decs:
