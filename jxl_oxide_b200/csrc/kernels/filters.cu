@@ -1,73 +1,22 @@
-// Restoration filters and colour on the device: Gaborish 3x3, edge-preserving filter (steps
-// 0/1/2), XYB -> linear sRGB (-> sRGB). Float op order follows the reference's generic path:
-// crates/jxl-render/src/filter/{gabor.rs,epf.rs}, filter/impls/generic/{gabor.rs,epf.rs},
-// crates/jxl-color/src/{xyb.rs:35-60, ciexyz.rs:81-87, tf/srgb.rs:13-48}. Compiled with
-// -fmad=false; fused multiply-add only where the reference uses mul_add.
+// Restoration filters and colour as stand-alone stages: Gaborish 3x3, edge-preserving filter (steps 0/1/2), XYB -> RGB
+// (the per-pixel formulas: pixel_math.cuh), and the render features (upsampling, patches, splines, noise, JPEG chroma
+// upsampling, YCbCr, packing). Float op order follows the reference's generic path. Compiled with -fmad=false; fused
+// multiply-add only where the reference uses mul_add.
 #include "kernels.h"
+#include "pixel_math.cuh"
 
 namespace jxlb {
 
 namespace {
 
-__device__ __forceinline__ float fadd(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ float fsub(float a, float b) { return __fsub_rn(a, b); }
-__device__ __forceinline__ float fmul(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ float fdiv(float a, float b) { return __fdiv_rn(a, b); }
-
-// impls/generic/gabor.rs: the formulas differ between interior rows, top/bottom rows, first/last
-// columns and the degenerate 1-row / 1-column cases; each is reproduced literally.
+// impls/generic/gabor.rs, one thread per pixel
 __global__ void gaborish_kernel(DevView in, DevView out, float w0, float w1) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
   const int width = int(in.w), height = int(in.h);
   if (x >= width) return;
   const float* base = static_cast<const float*>(in.ptr);
-  const float gw = fdiv(1.0f, fadd(fadd(1.0f, fmul(w0, 4.0f)), fmul(w1, 4.0f)));
-  auto at = [&](int xx, int yy) { return base[size_t(yy) * in.stride + xx]; };
-  float res;
-  if (height == 1) {
-    if (width == 1) {
-      res = at(0, 0);
-    } else {
-      const float merged_w0 = fadd(fadd(1.0f, 2.0f), w0);
-      const float merged_w1 = fadd(w0, fmul(2.0f, w1));
-      if (x == 0) res = fmul(fadd(fmul(at(0, 0), fadd(merged_w0, merged_w1)), fmul(at(1, 0), merged_w1)), gw);
-      else if (x == width - 1)
-        res = fmul(fadd(fmul(at(width - 1, 0), fadd(merged_w0, merged_w1)), fmul(at(width - 2, 0), merged_w1)), gw);
-      else res = fmul(fadd(fmul(at(x, 0), merged_w0), fmul(fadd(at(x - 1, 0), at(x + 1, 0)), merged_w1)), gw);
-    }
-  } else if (y == 0 || y == height - 1) {
-    const int ya = (y == 0) ? 1 : height - 2;  // the one adjacent row
-    if (width == 1) {
-      float u = at(0, ya), c = at(0, y);
-      res = fmul(fadd(fmul(c, fadd(fadd(1.0f, fmul(3.0f, w0)), fmul(2.0f, w1))), fmul(u, fadd(w0, fmul(2.0f, w1)))), gw);
-    } else if (x == 0 || x == width - 1) {
-      const int xo = (x == 0) ? 1 : width - 2;
-      float a1 = at(x, ya), a0 = at(xo, ya), c1 = at(x, y), c0 = at(xo, y);
-      res = fmul(fadd(fadd(fmul(c1, fadd(fadd(1.0f, fmul(2.0f, w0)), w1)), fmul(fadd(a1, c0), fadd(w0, w1))), fmul(a0, w1)), gw);
-    } else {
-      float a0 = at(x - 1, ya), a1 = at(x, ya), a2 = at(x + 1, ya);
-      float c0 = at(x - 1, y), c1 = at(x, y), c2 = at(x + 1, y);
-      res = fmul(fadd(fadd(c1, fmul(fadd(fadd(fadd(a1, c0), c1), c2), w0)), fmul(fadd(fadd(fadd(a0, a2), c0), c2), w1)), gw);
-    }
-  } else {
-    if (width == 1) {
-      float t = at(0, y - 1), c = at(0, y), b = at(0, y + 1);
-      float sum_side = fadd(fadd(t, fmul(2.0f, c)), b);
-      float sum_diag = fmul(2.0f, fadd(t, b));
-      res = fmul(fadd(fadd(c, fmul(sum_side, w0)), fmul(sum_diag, w1)), gw);
-    } else if (x == 0 || x == width - 1) {
-      const int xo = (x == 0) ? 1 : width - 2;
-      float t1 = at(x, y - 1), c1 = at(x, y), b1 = at(x, y + 1);
-      float t0 = at(xo, y - 1), c0 = at(xo, y), b0 = at(xo, y + 1);
-      float sum_side = fadd(fadd(fadd(t1, c0), c1), b1);
-      float sum_diag = fadd(fadd(fadd(t0, t1), b0), b1);
-      res = fmul(fadd(fadd(c1, fmul(sum_side, w0)), fmul(sum_diag, w1)), gw);
-    } else {
-      float sum_side = fadd(fadd(fadd(at(x, y - 1), at(x - 1, y)), at(x + 1, y)), at(x, y + 1));
-      float sum_diag = fadd(fadd(fadd(at(x - 1, y - 1), at(x + 1, y - 1)), at(x - 1, y + 1)), at(x + 1, y + 1));
-      res = fmul(fadd(fadd(at(x, y), fmul(sum_side, w0)), fmul(sum_diag, w1)), gw);
-    }
-  }
+  auto at = [&](int dx, int dy) { return base[size_t(y + dy) * in.stride + x + dx]; };
+  const float res = gaborish_px(at, x, y, width, height, w0, w1, gaborish_norm(w0, w1));
   static_cast<float*>(out.ptr)[size_t(y) * out.stride + x] = res;
 }
 
@@ -78,12 +27,6 @@ __device__ __forceinline__ int mirror(int offset, int len) {  // util.rs:376-386
     else return offset;
   }
 }
-
-__device__ __constant__ const int8_t kKernel1[4][2] = {{0, -1}, {0, 1}, {-1, 0}, {1, 0}};
-__device__ __constant__ const int8_t kKernel2[12][2] = {{0, -2}, {-1, -1}, {0, -1}, {1, -1}, {-2, 0}, {-1, 0},
-                                                        {1, 0},  {2, 0},   {-1, 1}, {0, 1},  {1, 1},  {0, 2}};
-__device__ __constant__ const int8_t kDist0[5][2] = {{0, -1}, {1, 0}, {0, 0}, {-1, 0}, {0, 1}};
-__device__ __constant__ const int8_t kDist1[5][2] = {{0, -1}, {0, 0}, {0, 1}, {-1, 0}, {1, 0}};
 
 struct View3 {
   DevView v[3];
@@ -104,37 +47,28 @@ __global__ void epf_kernel(View3 in, View3 out, const float* __restrict__ sigma,
 #pragma unroll
     for (int c = 0; c < 3; ++c) o[c] = ch[c][size_t(y) * stride[c] + x];
   } else {
-    const float step_multiplier = STEP == 0 ? p.pass0_sigma_scale : (STEP == 2 ? p.pass2_sigma_scale : 1.0f);
-    const bool is_y_border = ((y + 1) & 6) == 0;
-    float sm;
-    if (is_y_border) sm = fmul(step_multiplier, p.border_sad_mul);
-    else sm = ((x & 7) == 0 || (x & 7) == 7) ? fmul(step_multiplier, p.border_sad_mul) : step_multiplier;
-    const float neg_inv_sigma = fmul(fdiv(fmul(6.6f, fsub(0.70710678118654752440f, 1.0f)), sigma_val), sm);
+    const float neg_inv_sigma = fmul(epf_inv_sigma(sigma_val), epf_step_mul(p, STEP, epf_row_border(y) || epf_col_border(x)));
     float sum_weights = 1.0f;
     float sum_channels[3];
 #pragma unroll
     for (int c = 0; c < 3; ++c) sum_channels[c] = ch[c][size_t(y) * stride[c] + x];
-    constexpr int NK = STEP == 0 ? 12 : 4;
-    constexpr int ND = STEP == 2 ? 1 : 5;
 #pragma unroll
-    for (int k = 0; k < NK; ++k) {
-      const int kx = x + (STEP == 0 ? kKernel2[k][0] : kKernel1[k][0]);
-      const int ky = y + (STEP == 0 ? kKernel2[k][1] : kKernel1[k][1]);
+    for (int k = 0; k < epf_neighbours(STEP); ++k) {
+      const int kx = x + epf_nb_x(STEP, k), ky = y + epf_nb_y(STEP, k);
       float dist = 0.0f;
 #pragma unroll
       for (int c = 0; c < 3; ++c) {
         float acc = 0.0f;
 #pragma unroll
-        for (int i = 0; i < ND; ++i) {
-          const int ox = STEP == 2 ? 0 : (STEP == 0 ? kDist0[i][0] : kDist1[i][0]);
-          const int oy = STEP == 2 ? 0 : (STEP == 0 ? kDist0[i][1] : kDist1[i][1]);
+        for (int i = 0; i < epf_plus_size(STEP); ++i) {
+          const int ox = epf_plus_x(STEP, i), oy = epf_plus_y(STEP, i);
           const int ay = mirror(ky + oy, height), ax = mirror(kx + ox, width);
           const int by = mirror(y + oy, height), bx = mirror(x + ox, width);
-          acc = fadd(acc, fabsf(fsub(ch[c][size_t(ay) * stride[c] + ax], ch[c][size_t(by) * stride[c] + bx])));
+          acc = fadd(acc, absdiff(ch[c][size_t(ay) * stride[c] + ax], ch[c][size_t(by) * stride[c] + bx]));
         }
         dist = fadd(dist, fmul(p.channel_scale[c], acc));
       }
-      const float weight = fmaxf(fadd(1.0f, fmul(dist, neg_inv_sigma)), 0.0f);
+      const float weight = epf_weight(dist, neg_inv_sigma);
       sum_weights = fadd(sum_weights, weight);
       const int my = mirror(ky, height), mx = mirror(kx, width);
 #pragma unroll
@@ -145,56 +79,6 @@ __global__ void epf_kernel(View3 in, View3 out, const float* __restrict__ sigma,
   }
 #pragma unroll
   for (int c = 0; c < 3; ++c) static_cast<float*>(out.v[c].ptr)[size_t(y) * out.v[c].stride + x] = o[c];
-}
-
-__device__ __constant__ const uint8_t kPowUpper[16] = {0x00, 0x0a, 0x19, 0x26, 0x32, 0x41, 0x4d, 0x5c,
-                                                       0x68, 0x75, 0x83, 0x8f, 0xa0, 0xaa, 0xb9, 0xc6};
-__device__ __constant__ const uint8_t kPowLower[16] = {0x00, 0xb7, 0x04, 0x0d, 0xcb, 0xe7, 0x41, 0x68,
-                                                       0x51, 0xd1, 0xeb, 0xf2, 0x00, 0xb7, 0x04, 0x0d};
-
-__device__ __forceinline__ float linear_to_srgb(float s) {  // tf/srgb.rs:28-47 (scalar path)
-  uint32_t bits = __float_as_uint(s);
-  uint32_t vb = bits & 0x7fffffffu;
-  float v_adj = __uint_as_float((vb | 0x3e800000u) & 0x3effffffu);
-  float pow = 0.059914046f;
-  pow = fsub(fmul(pow, v_adj), 0.10889456f);
-  pow = fadd(fmul(pow, v_adj), 0.107963754f);
-  pow = fadd(fmul(pow, v_adj), 0.018092343f);
-  uint32_t idx = ((vb >> 23) - 118) & 0xf;
-  float mul = __uint_as_float(0x40000000u | (uint32_t(kPowUpper[idx]) << 18) | (uint32_t(kPowLower[idx]) << 10));
-  float av = __uint_as_float(vb);
-  float small = fmul(av, 12.92f);
-  float acc = fsub(fmul(pow, mul), 0.055f);
-  float res = av <= 0.0031308f ? small : acc;
-  return copysignf(res, s);
-}
-
-
-// BT.709 OETF exactly as the reference's generic path evaluates it (jxl-color/src/tf/bt709.rs:61-68 with
-// fastmath/powf.rs:7-22, 147-156 and rational_poly.rs:2-6): rational-polynomial log2 / pow2, un-fused
-// except for the final mul_add.
-__device__ __forceinline__ float linear_to_bt709(float a) {
-  if (a <= 0.018f) return fmul(4.5f, a);
-  const int32_t x_bits = __float_as_int(a);
-  const int32_t exp_shifted = (x_bits - 0x3f2aaaab) >> 23;
-  const float mantissa = __int_as_float(x_bits - (exp_shifted << 23));
-  const float exp_val = float(exp_shifted);
-  const float x = fsub(mantissa, 1.0f);
-  const float yp = fadd(fmul(fadd(fmul(7.4245873327820566e-1f, x), 1.4287160470083755f), x), -1.8503833400518310e-6f);
-  const float yq = fadd(fmul(fadd(fmul(1.7409343003366853e-1f, x), 1.0096718572241148f), x), 9.9032814277590719e-1f);
-  const float l2 = fadd(fdiv(yp, yq), exp_val);
-  const float e = fmul(l2, 0.45f);
-  const float x_floor = floorf(e);
-  const float ex = __int_as_float(int32_t(uint32_t(int32_t(x_floor) + 127) << 23));
-  const float frac = fsub(e, x_floor);
-  float num = fadd(frac, 1.01749063e1f);
-  num = fadd(fmul(num, frac), 4.88687798e1f);
-  num = fadd(fmul(num, frac), 9.85506591e1f);
-  num = fmul(num, ex);
-  float den = fadd(fmul(2.10242958e-1f, frac), -2.22328856e-2f);
-  den = fadd(fmul(den, frac), -1.94414990e1f);
-  den = fadd(fmul(den, frac), 9.85506633e1f);
-  return __fmaf_rn(fdiv(num, den), 1.099f, -0.099f);
 }
 
 // apply_jpeg_upsampling_single (jxl-render/src/filter/ycbcr.rs:6-78): the horizontal pass, then the vertical pass over
@@ -236,74 +120,9 @@ __global__ void ycbcr_to_rgb_kernel(DevView vcb, DevView vy, DevView vcr, DevYcb
   float* py = static_cast<float*>(vy.ptr) + size_t(y) * vy.stride + x;
   float* pcr = static_cast<float*>(vcr.ptr) + size_t(y) * vcr.stride + x;
   const float cb = *pcb, yy = fadd(*py, p.y_offset), cr = *pcr;
-  *pcb = __fmaf_rn(cr, p.cr_to_r, yy);
-  *py = __fmaf_rn(cb, p.cb_to_g, __fmaf_rn(cr, p.cr_to_g, yy));
-  *pcr = __fmaf_rn(cb, p.cb_to_b, yy);
-}
-
-// linear_to_pq_generic (jxl-color/src/tf/pq.rs:126-142): fourth root, then a 4/4 rational polynomial (Horner, un-fused)
-__device__ __forceinline__ float pq_tf(float s, float y_mult) {
-  const float a = fabsf(s);
-  const float a_1_4 = __fsqrt_rn(__fsqrt_rn(fmul(a, y_mult)));
-  float yp, yq;
-  if (a < 1e-4f) {
-    yp = fadd(fmul(fadd(fmul(fadd(fmul(fadd(fmul(-2.864824e5f, a_1_4), 6.889862e4f), a_1_4), 1.352821e2f), a_1_4), 3.881234e-1f), a_1_4), 9.863406e-6f);
-    yq = fadd(fmul(fadd(fmul(fadd(fmul(fadd(fmul(-2.072546e5f, a_1_4), -4.389884e4f), a_1_4), 1.608477e4f), a_1_4), 1.477719e3f), a_1_4), 3.371868e1f);
-  } else {
-    yp = fadd(fmul(fadd(fmul(fadd(fmul(fadd(fmul(4.838434e1f, a_1_4), 1.492516e2f), a_1_4), 5.522776e1f), a_1_4), -1.095778f), a_1_4), 1.351392e-2f);
-    yq = fadd(fmul(fadd(fmul(fadd(fmul(fadd(fmul(2.590418e1f, a_1_4), 1.120607e2f), a_1_4), 9.26371e1f), a_1_4), 2.016708e1f), a_1_4), 1.012416f);
-  }
-  return copysignf(fdiv(yp, yq), s);
-}
-
-// apply_gamma's scalar tail (jxl-color/src/tf.rs:62-69): v <= 1e-7 ? 0 : fast_powf_generic(v, gamma)
-__device__ __forceinline__ float gamma_tf(float a, float gamma) {
-  if (a <= 1e-7f) return 0.0f;
-  const int32_t x_bits = __float_as_int(a);
-  const int32_t exp_shifted = (x_bits - 0x3f2aaaab) >> 23;
-  const float mantissa = __int_as_float(x_bits - (exp_shifted << 23));
-  const float x = fsub(mantissa, 1.0f);
-  const float yp = fadd(fmul(fadd(fmul(7.4245873327820566e-1f, x), 1.4287160470083755f), x), -1.8503833400518310e-6f);
-  const float yq = fadd(fmul(fadd(fmul(1.7409343003366853e-1f, x), 1.0096718572241148f), x), 9.9032814277590719e-1f);
-  const float e = fmul(fadd(fdiv(yp, yq), float(exp_shifted)), gamma);
-  const float x_floor = floorf(e);
-  const float ex = __int_as_float(int32_t(uint32_t(__float2int_rz(x_floor) + 127) << 23));  // saturating, NaN -> 0
-  const float frac = fsub(e, x_floor);
-  float num = fadd(frac, 1.01749063e1f);
-  num = fadd(fmul(num, frac), 4.88687798e1f);
-  num = fadd(fmul(num, frac), 9.85506591e1f);
-  num = fmul(num, ex);
-  float den = fadd(fmul(2.10242958e-1f, frac), -2.22328856e-2f);
-  den = fadd(fmul(den, frac), -1.94414990e1f);
-  den = fadd(fmul(den, frac), 9.85506633e1f);
-  return fdiv(num, den);
-}
-
-// map_gamut_generic (jxl-color/src/gamut.rs:4-46) followed by the merged target matrix (convert.rs:397-466)
-__device__ __forceinline__ void second_colour_stage(const DevColorParams& p, float& o0, float& o1, float& o2) {
-  float o[3] = {o0, o1, o2};
-  const float yl = fadd(fadd(fmul(o[0], p.luminances[0]), fmul(o[1], p.luminances[1])), fmul(o[2], p.luminances[2]));
-  float gray_saturation = 0.0f, gray_luminance = 0.0f;
-#pragma unroll
-  for (int i = 0; i < 3; ++i) {
-    const float v_sub_y = fsub(o[i], yl);
-    const float inv = fdiv(1.0f, v_sub_y == 0.0f ? 1.0f : v_sub_y);
-    const float v_over = fmul(o[i], inv);
-    if (!(v_sub_y >= 0.0f)) gray_saturation = fmaxf(gray_saturation, v_over);
-    gray_luminance = fmaxf(v_sub_y <= 0.0f ? gray_saturation : fsub(v_over, inv), gray_luminance);
-  }
-  float gray_mix = fadd(fmul(0.3f, fsub(gray_saturation, gray_luminance)), gray_luminance);
-  gray_mix = gray_mix < 0.0f ? 0.0f : (gray_mix > 1.0f ? 1.0f : gray_mix);
-  const float max_colour = fmaxf(o[2], fmaxf(o[1], fmaxf(o[0], 1.0f)));
-#pragma unroll
-  for (int i = 0; i < 3; ++i) o[i] = fdiv(fadd(fmul(gray_mix, fsub(yl, o[i])), o[i]), max_colour);
-  const float* m = p.matrix2;
-  const float t0 = fadd(fadd(fmul(m[0], o[0]), fmul(m[1], o[1])), fmul(m[2], o[2]));
-  const float t1 = fadd(fadd(fmul(m[3], o[0]), fmul(m[4], o[1])), fmul(m[5], o[2]));
-  const float t2 = fadd(fadd(fmul(m[6], o[0]), fmul(m[7], o[1])), fmul(m[8], o[2]));
-  o0 = p.to_luma ? t1 : t0;
-  o1 = t1;
-  o2 = t2;
+  *pcb = ffma(cr, p.cr_to_r, yy);
+  *py = ffma(cb, p.cb_to_g, ffma(cr, p.cr_to_g, yy));
+  *pcr = ffma(cb, p.cb_to_b, yy);
 }
 
 __global__ void xyb_to_rgb_kernel(DevView vx, DevView vy, DevView vb, DevColorParams p) {
@@ -312,39 +131,22 @@ __global__ void xyb_to_rgb_kernel(DevView vx, DevView vy, DevView vb, DevColorPa
   float* px = static_cast<float*>(vx.ptr) + size_t(y) * vx.stride + x;
   float* py = static_cast<float*>(vy.ptr) + size_t(y) * vy.stride + x;
   float* pb = static_cast<float*>(vb.ptr) + size_t(y) * vb.stride + x;
-  float xx = *px, yy = *py, bb = *pb;
-  float g_l = fsub(fadd(yy, xx), p.cbrt_opsin_bias[0]);
-  float g_m = fsub(fsub(yy, xx), p.cbrt_opsin_bias[1]);
-  float g_s = fsub(bb, p.cbrt_opsin_bias[2]);
-  float a = fmul(__fmaf_rn(fmul(g_l, g_l), g_l, p.opsin_bias[0]), p.itscale);
-  float b = fmul(__fmaf_rn(fmul(g_m, g_m), g_m, p.opsin_bias[1]), p.itscale);
-  float c = fmul(__fmaf_rn(fmul(g_s, g_s), g_s, p.opsin_bias[2]), p.itscale);
-  const float* m = p.matrix;
-  float o0 = fadd(fadd(fmul(m[0], a), fmul(m[1], b)), fmul(m[2], c));
-  float o1 = fadd(fadd(fmul(m[3], a), fmul(m[4], b)), fmul(m[5], c));
-  float o2 = fadd(fadd(fmul(m[6], a), fmul(m[7], b)), fmul(m[8], c));
-  if (p.second_stage) second_colour_stage(p, o0, o1, o2);
+  float o[3] = {*px, *py, *pb};
+  xyb_to_linear(o, p);
+  if (p.second_stage) second_colour_stage(o, p);
   if (p.pq_intensity_target > 0.0f) {
     const float y_mult = fdiv(p.pq_intensity_target, 10000.0f);
-    o0 = pq_tf(o0, y_mult);
-    o1 = pq_tf(o1, y_mult);
-    o2 = pq_tf(o2, y_mult);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o[c] = pq_tf(o[c], y_mult);
   } else if (p.gamma > 0.0f) {
-    o0 = gamma_tf(o0, p.gamma);
-    o1 = gamma_tf(o1, p.gamma);
-    o2 = gamma_tf(o2, p.gamma);
-  } else if (p.apply_srgb_tf) {
-    o0 = linear_to_srgb(o0);
-    o1 = linear_to_srgb(o1);
-    o2 = linear_to_srgb(o2);
-  } else if (p.apply_bt709_tf) {
-    o0 = linear_to_bt709(o0);
-    o1 = linear_to_bt709(o1);
-    o2 = linear_to_bt709(o2);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o[c] = gamma_tf(o[c], p.gamma);
+  } else {
+    encode_tf(o, colour_tf(p), kSrgbPow);
   }
-  *px = o0;
-  *py = o1;
-  *pb = o2;
+  *px = o[0];
+  *py = o[1];
+  *pb = o[2];
 }
 
 // upsample_inner<K, NW> (features/upsampling.rs:45-132): one thread per output sample; the 5x5
@@ -524,7 +326,7 @@ __global__ void __launch_bounds__(256) splat_splines_kernel(DevView v0, DevView 
         const DevSplineArc& q = hit[i];
         if (x < q.xbegin || x >= q.xend || y < q.ybegin || y >= q.yend) continue;
         const float dx = fsub(float(x), q.x), dy = fsub(float(y), q.y);
-        const float distance = __fsqrt_rn(fadd(fmul(dx, dx), fmul(dy, dy)));
+        const float distance = fsqrt(fadd(fmul(dx, dx), fmul(dy, dy)));
         const float factor = fsub(spline_erf(fmul(fadd(fmul(0.5f, distance), 0.35355338f), q.inv_sigma)),
                                   spline_erf(fmul(fsub(fmul(0.5f, distance), 0.35355338f), q.inv_sigma)));
 #pragma unroll

@@ -14,11 +14,9 @@
 // shared memory; half-stage 2 reads two values per direction pair and forms weights and weighted sums in the
 // reference's neighbour order. Same values, same rounding, half the arithmetic and a third of the shared-memory reads.
 //
-// Per-pixel arithmetic and its order are those of the stand-alone kernels in filters.cu, i.e. the
-// reference's generic path (crates/jxl-render/src/filter/impls/generic/{gabor.rs,epf.rs},
-// crates/jxl-color/src/xyb.rs). Border semantics: Gaborish uses its own edge formulas on the image
-// border (gabor.rs:119-167); EPF mirrors coordinates (util.rs:376-386) -- after each stage the part
-// of the halo that lies outside the image is filled by mirroring, so the stencils index plainly.
+// The per-pixel formulas are those of every filter kernel (pixel_math.cuh, the reference's generic path). Border semantics:
+// Gaborish uses its own edge formulas on the image border (gabor.rs:119-167); EPF mirrors coordinates (util.rs:376-386) --
+// after each stage the part of the halo that lies outside the image is filled by mirroring, so the stencils index plainly.
 #include "filter_strip.cuh"
 #include "kernels.h"
 
@@ -31,11 +29,6 @@
 namespace jxlb {
 
 namespace {
-
-__device__ __forceinline__ float fadd(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ float fsub(float a, float b) { return __fsub_rn(a, b); }
-__device__ __forceinline__ float fmul(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ float fdiv(float a, float b) { return __fdiv_rn(a, b); }
 
 constexpr int kT = 32;  // output tile
 // Shared-memory planes are kS x kS cells with a margin of (kS - kT) / 2 around the tile: 48 (margin 8 >= stencil radius 7) when
@@ -51,65 +44,6 @@ __device__ __forceinline__ int mirror1(int v, int len) {  // single reflection (
   return v < 0 ? -v - 1 : (v >= len ? 2 * len - v - 1 : v);
 }
 
-// Gaborish at one in-image pixel; `a` points at the pixel in a shared plane (gabor.rs:3-167).
-template <int kS>
-__device__ __forceinline__ float gab_px(const float* a, int x, int y, int width, int height, float w0, float w1, float gw) {
-  auto at = [&](int dx, int dy) { return a[dy * kS + dx]; };
-  if (height == 1) {
-    if (width == 1) return at(0, 0);
-    const float merged_w0 = fadd(fadd(1.0f, 2.0f), w0);
-    const float merged_w1 = fadd(w0, fmul(2.0f, w1));
-    if (x == 0) return fmul(fadd(fmul(at(0, 0), fadd(merged_w0, merged_w1)), fmul(at(1, 0), merged_w1)), gw);
-    if (x == width - 1) return fmul(fadd(fmul(at(0, 0), fadd(merged_w0, merged_w1)), fmul(at(-1, 0), merged_w1)), gw);
-    return fmul(fadd(fmul(at(0, 0), merged_w0), fmul(fadd(at(-1, 0), at(1, 0)), merged_w1)), gw);
-  }
-  if (y == 0 || y == height - 1) {
-    const int ya = (y == 0) ? 1 : -1;  // the one adjacent row
-    if (width == 1) {
-      const float u = at(0, ya), c = at(0, 0);
-      return fmul(fadd(fmul(c, fadd(fadd(1.0f, fmul(3.0f, w0)), fmul(2.0f, w1))), fmul(u, fadd(w0, fmul(2.0f, w1)))), gw);
-    }
-    if (x == 0 || x == width - 1) {
-      const int xo = (x == 0) ? 1 : -1;
-      const float a1 = at(0, ya), a0 = at(xo, ya), c1 = at(0, 0), c0 = at(xo, 0);
-      return fmul(fadd(fadd(fmul(c1, fadd(fadd(1.0f, fmul(2.0f, w0)), w1)), fmul(fadd(a1, c0), fadd(w0, w1))), fmul(a0, w1)), gw);
-    }
-    const float a0 = at(-1, ya), a1 = at(0, ya), a2 = at(1, ya);
-    const float c0 = at(-1, 0), c1 = at(0, 0), c2 = at(1, 0);
-    return fmul(fadd(fadd(c1, fmul(fadd(fadd(fadd(a1, c0), c1), c2), w0)), fmul(fadd(fadd(fadd(a0, a2), c0), c2), w1)), gw);
-  }
-  if (width == 1) {
-    const float t = at(0, -1), c = at(0, 0), b = at(0, 1);
-    const float sum_side = fadd(fadd(t, fmul(2.0f, c)), b);
-    const float sum_diag = fmul(2.0f, fadd(t, b));
-    return fmul(fadd(fadd(c, fmul(sum_side, w0)), fmul(sum_diag, w1)), gw);
-  }
-  if (x == 0 || x == width - 1) {
-    const int xo = (x == 0) ? 1 : -1;
-    const float t1 = at(0, -1), c1 = at(0, 0), b1 = at(0, 1);
-    const float t0 = at(xo, -1), c0 = at(xo, 0), b0 = at(xo, 1);
-    const float sum_side = fadd(fadd(fadd(t1, c0), c1), b1);
-    const float sum_diag = fadd(fadd(fadd(t0, t1), b0), b1);
-    return fmul(fadd(fadd(c1, fmul(sum_side, w0)), fmul(sum_diag, w1)), gw);
-  }
-  const float sum_side = fadd(fadd(fadd(at(0, -1), at(-1, 0)), at(1, 0)), at(0, 1));
-  const float sum_diag = fadd(fadd(fadd(at(-1, -1), at(1, -1)), at(-1, 1)), at(1, 1));
-  return fmul(fadd(fadd(at(0, 0), fmul(sum_side, w0)), fmul(sum_diag, w1)), gw);
-}
-
-// Neighbour offsets in the reference's order (epf.rs): 4 for steps 1 / 2, 12 for step 0. constexpr functions, so that every
-// offset below folds into an immediate address.
-__device__ __forceinline__ constexpr int fk_x(int step, int k) {
-  constexpr int k1[4] = {0, 0, -1, 1};
-  constexpr int k2[12] = {0, -1, 0, 1, -2, -1, 1, 2, -1, 0, 1, 0};
-  return step == 0 ? k2[k] : k1[k];
-}
-__device__ __forceinline__ constexpr int fk_y(int step, int k) {
-  constexpr int k1[4] = {-1, 1, 0, 0};
-  constexpr int k2[12] = {-2, -1, -1, -1, 0, 0, 0, 0, 1, 1, 1, 2};
-  return step == 0 ? k2[k] : k1[k];
-}
-
 // "Positive" directions of each step; the other half of the neighbour list is their negation.
 //   step 0: (0,2) (1,1) (0,1) (-1,1) (2,0) (1,0)        steps 1, 2: (0,1) (1,0)
 __device__ __forceinline__ constexpr int dplus_x(int step, int m) {
@@ -117,13 +51,6 @@ __device__ __forceinline__ constexpr int dplus_x(int step, int m) {
 }
 __device__ __forceinline__ constexpr int dplus_y(int step, int m) {
   return step == 0 ? (m == 0 ? 2 : m == 1 ? 1 : m == 2 ? 1 : m == 3 ? 1 : 0) : (m == 0 ? 1 : 0);
-}
-// offsets of the 5-sample plus in the reference's summation order (epf.rs: step 0 and step 1 differ), step 2: centre only
-__device__ __forceinline__ constexpr int plus_x(int step, int i) {
-  return step == 2 ? 0 : step == 0 ? (i == 1 ? 1 : i == 3 ? -1 : 0) : (i == 3 ? -1 : i == 4 ? 1 : 0);
-}
-__device__ __forceinline__ constexpr int plus_y(int step, int i) {
-  return step == 2 ? 0 : step == 0 ? (i == 0 ? -1 : i == 4 ? 1 : 0) : (i == 0 ? -1 : i == 2 ? 1 : 0);
 }
 
 // Half-stage 1: the distance maps of one EPF step at cell q. `a` points at q in channel 0 of the input buffer, `d` at q in
@@ -133,7 +60,7 @@ template <int STEP, int kS>
 __device__ __forceinline__ void epf_dist(const float* __restrict__ a, float* __restrict__ d, const DevEpfParams& p) {
   constexpr int kPlane = kS * kS;
   constexpr int NM = STEP == 0 ? 6 : 2;
-  constexpr int ND = STEP == 2 ? 1 : 5;
+  constexpr int ND = epf_plus_size(STEP);
   float dist[NM];  // all maps first, stores last: a store between them would make the compiler reload every sample
 #pragma unroll
   for (int m = 0; m < NM; ++m) {
@@ -146,8 +73,8 @@ __device__ __forceinline__ void epf_dist(const float* __restrict__ a, float* __r
       float acc = 0.0f;
 #pragma unroll
       for (int i = 0; i < ND; ++i) {
-        const int ox = plus_x(STEP, i), oy = plus_y(STEP, i);
-        const float t = fabsf(fsub(a[c * kPlane + (dy + oy) * kS + dx + ox], a[c * kPlane + oy * kS + ox]));
+        const int ox = epf_plus_x(STEP, i), oy = epf_plus_y(STEP, i);
+        const float t = absdiff(a[c * kPlane + (dy + oy) * kS + dx + ox], a[c * kPlane + oy * kS + ox]);
         acc = i == 0 ? t : fadd(acc, t);
       }
       const float term = fmul(p.channel_scale[c], acc);
@@ -159,7 +86,7 @@ __device__ __forceinline__ void epf_dist(const float* __restrict__ a, float* __r
 }
 
 // Half-stage 2: weights and weighted sums at pixel p in the reference's neighbour order; `a` points at p in channel 0 of
-// the input buffer, `d` at p in distance map 0.
+// the input buffer, `d` at p in distance map 0, `inv_sigma` is epf_inv_sigma of p's 8x8 block.
 template <int STEP, int kS>
 __device__ __forceinline__ void epf_apply(const float* a, const float* d, int x, int y, float sigma_val, float inv_sigma,
                                           const DevEpfParams& p, float o[3]) {
@@ -169,21 +96,15 @@ __device__ __forceinline__ void epf_apply(const float* a, const float* d, int x,
     for (int c = 0; c < 3; ++c) o[c] = a[c * kPlane];
     return;
   }
-  const float step_multiplier = STEP == 0 ? p.pass0_sigma_scale : (STEP == 2 ? p.pass2_sigma_scale : 1.0f);
-  const bool is_y_border = ((y + 1) & 6) == 0;
-  float sm;
-  if (is_y_border) sm = fmul(step_multiplier, p.border_sad_mul);
-  else sm = ((x & 7) == 0 || (x & 7) == 7) ? fmul(step_multiplier, p.border_sad_mul) : step_multiplier;
-  const float neg_inv_sigma = fmul(inv_sigma, sm);  // inv_sigma = 6.6 * (1/sqrt(2) - 1) / sigma, one division per 8x8 block
+  const float neg_inv_sigma = fmul(inv_sigma, epf_step_mul(p, STEP, epf_row_border(y) || epf_col_border(x)));
   float sum_weights = 1.0f;
   float sum_channels[3];
 #pragma unroll
   for (int c = 0; c < 3; ++c) sum_channels[c] = a[c * kPlane];
-  constexpr int NK = STEP == 0 ? 12 : 4;
   constexpr int NM = STEP == 0 ? 6 : 2;
 #pragma unroll
-  for (int k = 0; k < NK; ++k) {
-    const int kx = fk_x(STEP, k), ky = fk_y(STEP, k);
+  for (int k = 0; k < epf_neighbours(STEP); ++k) {
+    const int kx = epf_nb_x(STEP, k), ky = epf_nb_y(STEP, k);
     // which map holds this neighbour's distance, and at which cell
     float dist = 0.0f;
 #pragma unroll
@@ -192,86 +113,13 @@ __device__ __forceinline__ void epf_apply(const float* a, const float* d, int x,
       if (dx == kx && dy == ky) dist = d[m * kPlane];                      // positive direction: dist_d(p)
       if (dx == -kx && dy == -ky) dist = d[m * kPlane + ky * kS + kx];     // its negation: dist_d(p - d) = dist_d(p + k)
     }
-    const float weight = fmaxf(fadd(1.0f, fmul(dist, neg_inv_sigma)), 0.0f);
+    const float weight = epf_weight(dist, neg_inv_sigma);
     sum_weights = fadd(sum_weights, weight);
 #pragma unroll
     for (int c = 0; c < 3; ++c) sum_channels[c] = fadd(sum_channels[c], fmul(weight, a[c * kPlane + ky * kS + kx]));
   }
 #pragma unroll
   for (int c = 0; c < 3; ++c) o[c] = fdiv(sum_channels[c], sum_weights);
-}
-
-__device__ __constant__ const uint8_t kFPowUpper[16] = {0x00, 0x0a, 0x19, 0x26, 0x32, 0x41, 0x4d, 0x5c,
-                                                        0x68, 0x75, 0x83, 0x8f, 0xa0, 0xaa, 0xb9, 0xc6};
-__device__ __constant__ const uint8_t kFPowLower[16] = {0x00, 0xb7, 0x04, 0x0d, 0xcb, 0xe7, 0x41, 0x68,
-                                                        0x51, 0xd1, 0xeb, 0xf2, 0x00, 0xb7, 0x04, 0x0d};
-
-__device__ __forceinline__ float linear_to_srgb_f(float s) {  // tf/srgb.rs:28-47 (scalar path)
-  const uint32_t bits = __float_as_uint(s);
-  const uint32_t vb = bits & 0x7fffffffu;
-  const float v_adj = __uint_as_float((vb | 0x3e800000u) & 0x3effffffu);
-  float pow = 0.059914046f;
-  pow = fsub(fmul(pow, v_adj), 0.10889456f);
-  pow = fadd(fmul(pow, v_adj), 0.107963754f);
-  pow = fadd(fmul(pow, v_adj), 0.018092343f);
-  const uint32_t idx = ((vb >> 23) - 118) & 0xf;
-  const float mul = __uint_as_float(0x40000000u | (uint32_t(kFPowUpper[idx]) << 18) | (uint32_t(kFPowLower[idx]) << 10));
-  const float av = __uint_as_float(vb);
-  const float small = fmul(av, 12.92f);
-  const float acc = fsub(fmul(pow, mul), 0.055f);
-  const float res = av <= 0.0031308f ? small : acc;
-  return copysignf(res, s);
-}
-
-
-// BT.709 OETF exactly as the reference's generic path evaluates it (jxl-color/src/tf/bt709.rs:61-68 with
-// fastmath/powf.rs:7-22, 147-156 and rational_poly.rs:2-6): rational-polynomial log2 / pow2, un-fused
-// except for the final mul_add.
-__device__ __forceinline__ float linear_to_bt709_f(float a) {
-  if (a <= 0.018f) return fmul(4.5f, a);
-  const int32_t x_bits = __float_as_int(a);
-  const int32_t exp_shifted = (x_bits - 0x3f2aaaab) >> 23;
-  const float mantissa = __int_as_float(x_bits - (exp_shifted << 23));
-  const float exp_val = float(exp_shifted);
-  const float x = fsub(mantissa, 1.0f);
-  const float yp = fadd(fmul(fadd(fmul(7.4245873327820566e-1f, x), 1.4287160470083755f), x), -1.8503833400518310e-6f);
-  const float yq = fadd(fmul(fadd(fmul(1.7409343003366853e-1f, x), 1.0096718572241148f), x), 9.9032814277590719e-1f);
-  const float l2 = fadd(fdiv(yp, yq), exp_val);
-  const float e = fmul(l2, 0.45f);
-  const float x_floor = floorf(e);
-  const float ex = __int_as_float(int32_t(uint32_t(int32_t(x_floor) + 127) << 23));
-  const float frac = fsub(e, x_floor);
-  float num = fadd(frac, 1.01749063e1f);
-  num = fadd(fmul(num, frac), 4.88687798e1f);
-  num = fadd(fmul(num, frac), 9.85506591e1f);
-  num = fmul(num, ex);
-  float den = fadd(fmul(2.10242958e-1f, frac), -2.22328856e-2f);
-  den = fadd(fmul(den, frac), -1.94414990e1f);
-  den = fadd(fmul(den, frac), 9.85506633e1f);
-  return __fmaf_rn(fdiv(num, den), 1.099f, -0.099f);
-}
-
-__device__ __forceinline__ void xyb_px(float o[3], const DevColorParams& p) {  // xyb.rs:35-60, ciexyz.rs:81-87
-  const float xx = o[0], yy = o[1], bb = o[2];
-  const float g_l = fsub(fadd(yy, xx), p.cbrt_opsin_bias[0]);
-  const float g_m = fsub(fsub(yy, xx), p.cbrt_opsin_bias[1]);
-  const float g_s = fsub(bb, p.cbrt_opsin_bias[2]);
-  const float a = fmul(__fmaf_rn(fmul(g_l, g_l), g_l, p.opsin_bias[0]), p.itscale);
-  const float b = fmul(__fmaf_rn(fmul(g_m, g_m), g_m, p.opsin_bias[1]), p.itscale);
-  const float c = fmul(__fmaf_rn(fmul(g_s, g_s), g_s, p.opsin_bias[2]), p.itscale);
-  const float* m = p.matrix;
-  o[0] = fadd(fadd(fmul(m[0], a), fmul(m[1], b)), fmul(m[2], c));
-  o[1] = fadd(fadd(fmul(m[3], a), fmul(m[4], b)), fmul(m[5], c));
-  o[2] = fadd(fadd(fmul(m[6], a), fmul(m[7], b)), fmul(m[8], c));
-  if (p.apply_srgb_tf) {
-    o[0] = linear_to_srgb_f(o[0]);
-    o[1] = linear_to_srgb_f(o[1]);
-    o[2] = linear_to_srgb_f(o[2]);
-  } else if (p.apply_bt709_tf) {
-    o[0] = linear_to_bt709_f(o[0]);
-    o[1] = linear_to_bt709_f(o[1]);
-    o[2] = linear_to_bt709_f(o[2]);
-  }
 }
 
 // Visits every cell of `r` once with all 256 threads busy: the cells are numbered row by row and thread t takes cells
@@ -317,12 +165,40 @@ __device__ __forceinline__ void border_tile_of(const FusedViews& v, int i, int& 
   fstrip::border_tile_index(v.nbx, v.nby, v.bx_last, v.by_last, i, tx, ty);
 }
 
-// TMA descriptors of the three input planes (2-D, f32, box kS x kS, out-of-bounds cells read as zero).
+// TMA descriptors of the three input planes (encode_plane_maps).
 struct FusedMaps {
   CUtensorMap map[3];
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return uint32_t(__cvta_generic_to_shared(p)); }
+
+// Window load by TMA: the elected thread arms the mbarrier `mbar` with the byte count and issues three bulk tensor copies,
+// one box per plane with its corner at image pixel (gx0, gy0), into dst[c * kPlane]; the copies of the three planes are in
+// flight together, and no thread spends registers or address arithmetic on them. Cells outside the image arrive as zeros.
+template <int kPlane>
+__device__ __forceinline__ void window_load_issue(uint32_t mbar, float* dst, const FusedMaps& maps, int gx0, int gy0) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(mbar));
+  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mbar), "r"(uint32_t(3 * kPlane * sizeof(float))) : "memory");
+#pragma unroll
+  for (int c = 0; c < 3; ++c)
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
+            smem_u32(dst + c * kPlane)),
+        "l"(reinterpret_cast<uint64_t>(&maps.map[c])), "r"(gx0), "r"(gy0), "r"(mbar)
+        : "memory");
+}
+
+// Every thread waits on the barrier's phase; the barrier must be initialised (a __syncthreads after the issue) before.
+__device__ __forceinline__ void window_load_wait(uint32_t mbar) {
+  uint32_t done = 0;
+  for (uint32_t spin = 0; !done && spin < (1u << 24); ++spin)
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(done)
+        : "r"(mbar), "r"(0u)
+        : "memory");
+}
 
 // Cells of `need` that lie outside the image take the value of their mirrored in-image cell.
 template <int kS>
@@ -377,36 +253,17 @@ __global__ void __launch_bounds__(256) fused_filter_kernel(FusedViews v, DevFuse
       float sg = p.epf.sigma_for_modular;
       if (p.sigma) sg = (bx < ((width + 7) >> 3) && by < ((height + 7) >> 3)) ? __ldg(p.sigma + size_t(by) * p.sigma_stride + bx) : 1.0f;
       s_sigma[t] = sg;
-      s_inv_sigma[t] = fdiv(fmul(6.6f, fsub(0.70710678118654752440f, 1.0f)), sg);
+      s_inv_sigma[t] = epf_inv_sigma(sg);
     }
   }
 
   if (v.use_tma) {
-    // Tile + halo by TMA: one elected thread arms an mbarrier with the byte count and issues three bulk tensor copies
-    // (the whole kS x kS window of each plane; cells outside the image arrive as zeros and are never read before
-    // mirror_fill overwrites them), everybody waits on the barrier's phase. No per-thread address arithmetic, no
-    // register staging, and the copies of the three planes are in flight together.
+    // tile + halo: the whole kS x kS window of each plane (cells outside the image are never read before mirror_fill
+    // overwrites them)
     const uint32_t mbar = smem_u32(&s_mbar);
-    if (threadIdx.x == 0 && threadIdx.y == 0) {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(mbar));
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-      asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mbar), "r"(uint32_t(3 * kPlane * sizeof(float))) : "memory");
-#pragma unroll
-      for (int c = 0; c < 3; ++c)
-        asm volatile(
-            "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
-                smem_u32(cur + c * kPlane)),
-            "l"(reinterpret_cast<uint64_t>(&maps.map[c])), "r"(gx0), "r"(gy0), "r"(mbar)
-            : "memory");
-    }
+    if (threadIdx.x == 0 && threadIdx.y == 0) window_load_issue<kPlane>(mbar, cur, maps, gx0, gy0);
     __syncthreads();  // the barrier is initialised before anybody polls it
-    uint32_t done = 0;
-    for (uint32_t spin = 0; !done && spin < (1u << 24); ++spin)
-      asm volatile(
-          "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-          : "=r"(done)
-          : "r"(mbar), "r"(0u)
-          : "memory");
+    window_load_wait(mbar);
   } else {  // load the input region (planes whose pitch TMA cannot address)
     const Rect r = clip(rect(halo));
     for_region(r, [&](int lx, int ly) {
@@ -421,23 +278,24 @@ __global__ void __launch_bounds__(256) fused_filter_kernel(FusedViews v, DevFuse
     const Rect r = clip(rect(halo));
     float gw[3];
 #pragma unroll
-    for (int c = 0; c < 3; ++c) gw[c] = fdiv(1.0f, fadd(fadd(1.0f, fmul(p.gab_w[c][0], 4.0f)), fmul(p.gab_w[c][1], 4.0f)));
+    for (int c = 0; c < 3; ++c) gw[c] = gaborish_norm(p.gab_w[c][0], p.gab_w[c][1]);
     if (!border_tile) {  // no pixel of the window lies on the image border: the 3x3 formula without the edge cases
       for_region(r, [&](int lx, int ly) {
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
           const float* a = cur + c * kPlane + ly * kS + lx;
-          const float sum_side = fadd(fadd(fadd(a[-kS], a[-1]), a[1]), a[kS]);
-          const float sum_diag = fadd(fadd(fadd(a[-kS - 1], a[-kS + 1]), a[kS - 1]), a[kS + 1]);
-          alt[c * kPlane + ly * kS + lx] = fmul(fadd(fadd(a[0], fmul(sum_side, p.gab_w[c][0])), fmul(sum_diag, p.gab_w[c][1])), gw[c]);
+          alt[c * kPlane + ly * kS + lx] = gaborish_3x3(a[-kS - 1], a[-kS], a[-kS + 1], a[-1], a[0], a[1], a[kS - 1], a[kS], a[kS + 1],
+                                                        p.gab_w[c][0], p.gab_w[c][1], gw[c]);
         }
       });
     } else {
       for_region(r, [&](int lx, int ly) {
 #pragma unroll
-        for (int c = 0; c < 3; ++c)
-          alt[c * kPlane + ly * kS + lx] =
-              gab_px<kS>(cur + c * kPlane + ly * kS + lx, gx0 + lx, gy0 + ly, width, height, p.gab_w[c][0], p.gab_w[c][1], gw[c]);
+        for (int c = 0; c < 3; ++c) {
+          const float* a = cur + c * kPlane + ly * kS + lx;
+          alt[c * kPlane + ly * kS + lx] = gaborish_px([a](int dx, int dy) { return a[dy * kS + dx]; }, gx0 + lx, gy0 + ly, width,
+                                                       height, p.gab_w[c][0], p.gab_w[c][1], gw[c]);
+        }
       });
     }
     float* t = cur;
@@ -469,7 +327,7 @@ __global__ void __launch_bounds__(256) fused_filter_kernel(FusedViews v, DevFuse
         float o[3];
         epf_apply<STEP, kS>(cur + ly * kS + lx, dmap + ly * kS + lx, x, y, s_sigma[bi], s_inv_sigma[bi], p.epf, o);
         if (last) {
-          if (p.colour) xyb_px(o, p.col);
+          if (p.colour) xyb_to_rgb_px(o, p.col, colour_tf(p.col), kSrgbPow);
 #pragma unroll
           for (int c = 0; c < 3; ++c) v.out[c][size_t(y) * v.out_stride[c] + x] = o[c];
         } else {
@@ -499,7 +357,7 @@ __global__ void __launch_bounds__(256) fused_filter_kernel(FusedViews v, DevFuse
       float o[3];
 #pragma unroll
       for (int c = 0; c < 3; ++c) o[c] = cur[c * kPlane + ly * kS + lx];
-      if (p.colour) xyb_px(o, p.col);
+      if (p.colour) xyb_to_rgb_px(o, p.col, colour_tf(p.col), kSrgbPow);
       const int x = gx0 + lx, y = gy0 + ly;
 #pragma unroll
       for (int c = 0; c < 3; ++c) v.out[c][size_t(y) * v.out_stride[c] + x] = o[c];
@@ -519,27 +377,10 @@ strip_filter_kernel(FusedViews v, DevFusedFilterParams p, const __grid_constant_
   const int tid = int(threadIdx.x);
   const StripGeom g = strip_geom(v.width, v.height, r.x0, r.y0, r.x1, r.y1, int(blockIdx.x), int(blockIdx.y));
   const uint32_t mbar = smem_u32(&s_mbar);
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(mbar));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mbar), "r"(uint32_t(3 * kPlane * sizeof(float))) : "memory");
-#pragma unroll
-    for (int c = 0; c < 3; ++c)
-      asm volatile(
-          "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
-              smem_u32(s_buf + c * kPlane)),
-          "l"(reinterpret_cast<uint64_t>(&maps.map[c])), "r"(g.gx0), "r"(g.gy0), "r"(mbar)
-          : "memory");
-  }
+  if (tid == 0) window_load_issue<kPlane>(mbar, s_buf, maps, g.gx0, g.gy0);
   phase_sigma(tid, s_buf, g, p);
   __syncthreads();  // the barrier is initialised before anybody polls it; sigma table complete
-  uint32_t done = 0;
-  for (uint32_t spin = 0; !done && spin < (1u << 24); ++spin)
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(mbar), "r"(0u)
-        : "memory");
+  window_load_wait(mbar);
   const float gw[3] = {gw0, gw1, gw2};
   phase_gab(tid, s_buf, p, gw);
   __syncthreads();
@@ -572,6 +413,26 @@ EncodeTiledFn tensor_map_encoder() {
   }();
   return fn;
 }
+
+// TMA descriptors of the three input planes for a box_w x box_h window (2-D, f32, out-of-bounds cells read as zero). False,
+// with `maps` zeroed, when the driver has no encoder or a plane's base or row pitch is not 16-byte aligned.
+bool encode_plane_maps(const FusedViews& v, int box_w, int box_h, FusedMaps& maps) {
+  std::memset(&maps, 0, sizeof(maps));
+  const EncodeTiledFn enc = tensor_map_encoder();
+  if (!enc) return false;
+  for (int c = 0; c < 3; ++c) {
+    if ((reinterpret_cast<uintptr_t>(v.in[c]) & 15) != 0 || (size_t(v.in_stride[c]) * 4) % 16 != 0) return false;
+    const cuuint64_t dims[2] = {cuuint64_t(v.width), cuuint64_t(v.height)};
+    const cuuint64_t strides[1] = {cuuint64_t(v.in_stride[c]) * 4};
+    const cuuint32_t box[2] = {cuuint32_t(box_w), cuuint32_t(box_h)};
+    const cuuint32_t estr[2] = {1, 1};
+    if (enc(&maps.map[c], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(v.in[c]), dims, strides, box, estr,
+            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+      return false;
+  }
+  return true;
+}
 }  // namespace
 
 void launch_filters_fused(const DevView in[3], const DevView out[3], DevFusedFilterParams p, cudaStream_t stream) {
@@ -589,23 +450,7 @@ void launch_filters_fused(const DevView in[3], const DevView out[3], DevFusedFil
   const int ks = window_size(nmaps);
   const size_t plane_bytes = size_t(ks) * ks * sizeof(float);
   FusedMaps maps;
-  std::memset(&maps, 0, sizeof(maps));
-  v.use_tma = 0;
-  if (EncodeTiledFn enc = tensor_map_encoder()) {
-    bool ok = true;
-    for (int c = 0; c < 3 && ok; ++c) {
-      ok = (reinterpret_cast<uintptr_t>(v.in[c]) & 15) == 0 && (size_t(v.in_stride[c]) * 4) % 16 == 0;
-      if (!ok) break;
-      const cuuint64_t dims[2] = {cuuint64_t(v.width), cuuint64_t(v.height)};
-      const cuuint64_t strides[1] = {cuuint64_t(v.in_stride[c]) * 4};
-      const cuuint32_t box[2] = {cuuint32_t(ks), cuuint32_t(ks)};
-      const cuuint32_t estr[2] = {1, 1};
-      ok = enc(&maps.map[c], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(v.in[c]), dims, strides, box, estr,
-               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-    }
-    v.use_tma = ok ? 1 : 0;
-  }
+  v.use_tma = encode_plane_maps(v, ks, ks, maps) ? 1 : 0;
   // C++ function-local statics are initialised once, thread-safely: no worker thread launches before the limits are set
   static const bool attr_set = [] {
     cudaFuncSetAttribute(fused_filter_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 6 * window_size(0) * window_size(0) * 4);
@@ -634,19 +479,7 @@ void launch_filters_fused(const DevView in[3], const DevView out[3], DevFusedFil
   const bool origins_aligned = (v.width & 3) == 0;
   if (v.use_tma && origins_aligned && p.gab_enabled && (p.epf_iters == 1 || p.epf_iters == 2) && r.x1 > r.x0 && r.y1 > r.y0) {
     FusedMaps smaps;
-    std::memset(&smaps, 0, sizeof(smaps));
-    bool ok = true;
-    EncodeTiledFn enc = tensor_map_encoder();
-    for (int c = 0; c < 3 && ok; ++c) {
-      const cuuint64_t dims[2] = {cuuint64_t(v.width), cuuint64_t(v.height)};
-      const cuuint64_t strides[1] = {cuuint64_t(v.in_stride[c]) * 4};
-      const cuuint32_t box[2] = {cuuint32_t(fstrip::kWX), cuuint32_t(fstrip::kWY)};
-      const cuuint32_t estr[2] = {1, 1};
-      ok = enc(&smaps.map[c], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(v.in[c]), dims, strides, box, estr,
-               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-    }
-    if (ok) {
+    if (encode_plane_maps(v, fstrip::kWX, fstrip::kWY, smaps)) {
       float gw[3];
       fstrip::strip_gab_norm(p, gw);
       dim3 sgrid((r.x1 - r.x0 + fstrip::kTX - 1) / fstrip::kTX, (r.y1 - r.y0 + fstrip::kTY - 1) / fstrip::kTY);

@@ -1,7 +1,8 @@
 """Host emulation of the column-strip restoration-filter kernel (kernels/filter_strip.cuh).
 
 The kernel's phase functions (Gaborish, EPF step-1 distance maps, step-1 weighted sums, step 2 + colour) are plain
-functions of (thread id, shared window); tests/emu/ compiles them for the host, runs every CTA thread by thread and
+functions of (thread id, shared window), and the per-pixel formulas they call (kernels/pixel_math.cuh) are those of every
+filter kernel; tests/emu/ compiles them for the host, runs every CTA thread by thread and
 phase by phase over the frame's interior and compares each pixel with the oracle's own Gaborish / EPF / XYB stages
 (bit patterns). The device launch (TMA window load, barriers, border tiles in the general kernel) is covered by
 tests/test_gpu_parity.py and tests/test_zz_gpu_pipeline.py on a GPU.

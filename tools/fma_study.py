@@ -1,8 +1,8 @@
 """What would north_star's 1-ULP budget buy in the restoration-filter chain? (experiment, not part of the build)
 
 The shipped kernels compute every a*b+c as the reference's generic path does (multiply, round, add, round) and match the
-oracle bit for bit. This script makes a COPY of the column-strip filter kernel's phase functions
-(jxl_oxide_b200/csrc/kernels/filter_strip.cuh) in which the multiply-adds of Gaborish, the EPF distances / weights /
+oracle bit for bit. This script makes a COPY of the column-strip filter kernel's phase functions and the per-pixel formulas they call
+(jxl_oxide_b200/csrc/kernels/{filter_strip,pixel_math}.cuh) in which the multiply-adds of Gaborish, the EPF distances / weights /
 weighted sums and the colour stage are contracted to one fused multiply-add each (divisions stay IEEE divisions), and reports
 
   1. the error that costs: the copy is compiled for the host (tests/emu harness: every CTA run thread by thread, phase by
@@ -28,45 +28,46 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 BUILD = os.path.join(ROOT, "tools", "_fma_build")
 
-HELPER_OLD = "JXLB_FS float fs_absdiff(float a, float b) { return fabsf(fs_sub(a, b)); }"
-HELPER_NEW = HELPER_OLD + "\nJXLB_FS float fs_mad(float a, float b, float c) { return fs_fma(a, b, c); }  // contracted (experiment copy)"
-REPLACEMENTS = [
-    ("o[i * kWX] = fs_mul(fs_add(fs_add(mc, fs_mul(sum_side, w0)), fs_mul(sum_diag, w1)), g);",
-     "o[i * kWX] = fs_mul(fs_mad(sum_diag, w1, fs_mad(sum_side, w0, mc)), g);"),
-    ("        d01[i] = fs_add(d01[i], t01);\n        d10[i] = fs_add(d10[i], t10);",
-     "        d01[i] = fs_fma(sc, p01, d01[i]);\n        d10[i] = fs_fma(sc, p10, d10[i]);"),
-    ("const float wu = fmaxf(fs_add(1.0f, fs_mul(du, nis)), 0.0f);", "const float wu = fmaxf(fs_mad(du, nis, 1.0f), 0.0f);"),
-    ("const float wd = fmaxf(fs_add(1.0f, fs_mul(dd, nis)), 0.0f);", "const float wd = fmaxf(fs_mad(dd, nis, 1.0f), 0.0f);"),
-    ("const float wl = fmaxf(fs_add(1.0f, fs_mul(dl, nis)), 0.0f);", "const float wl = fmaxf(fs_mad(dl, nis, 1.0f), 0.0f);"),
-    ("const float wr = fmaxf(fs_add(1.0f, fs_mul(dr, nis)), 0.0f);", "const float wr = fmaxf(fs_mad(dr, nis, 1.0f), 0.0f);"),
-    ("float sum = fs_add(ce[c], fs_mul(wu, up[c]));", "float sum = fs_mad(wu, up[c], ce[c]);"),
-    ("sum = fs_add(sum, fs_mul(wd, dn[c]));", "sum = fs_mad(wd, dn[c], sum);"),
-    ("sum = fs_add(sum, fs_mul(wl, le[c]));", "sum = fs_mad(wl, le[c], sum);"),
-    ("sum = fs_add(sum, fs_mul(wr, ri[c]));", "sum = fs_mad(wr, ri[c], sum);"),
-    ("pw = fs_sub(fs_mul(pw, v_adj), 0.10889456f);", "pw = fs_mad(pw, v_adj, -0.10889456f);"),
-    ("pw = fs_add(fs_mul(pw, v_adj), 0.107963754f);", "pw = fs_mad(pw, v_adj, 0.107963754f);"),
-    ("pw = fs_add(fs_mul(pw, v_adj), 0.018092343f);", "pw = fs_mad(pw, v_adj, 0.018092343f);"),
-    ("const float acc = fs_sub(fs_mul(pw, mul), 0.055f);", "const float acc = fs_mad(pw, mul, -0.055f);"),
-    ("o[0] = fs_add(fs_add(fs_mul(m[0], a), fs_mul(m[1], b)), fs_mul(m[2], c));", "o[0] = fs_mad(m[2], c, fs_mad(m[1], b, fs_mul(m[0], a)));"),
-    ("o[1] = fs_add(fs_add(fs_mul(m[3], a), fs_mul(m[4], b)), fs_mul(m[5], c));", "o[1] = fs_mad(m[5], c, fs_mad(m[4], b, fs_mul(m[3], a)));"),
-    ("o[2] = fs_add(fs_add(fs_mul(m[6], a), fs_mul(m[7], b)), fs_mul(m[8], c));", "o[2] = fs_mad(m[8], c, fs_mad(m[7], b, fs_mul(m[6], a)));"),
-]
-DIST2 = re.compile(r"fs_add\(fs_add\(fs_mul\(s0, (fs_absdiff\([^)]*\))\), fs_mul\(s1, (fs_absdiff\([^)]*\))\)\), fs_mul\(s2, (fs_absdiff\([^)]*\))\)\)")
+HELPER_OLD = "JXLB_PX float absdiff(float a, float b) { return fabsf(fsub(a, b)); }"
+HELPER_NEW = HELPER_OLD + "\nJXLB_PX float fmad(float a, float b, float c) { return ffma(a, b, c); }  // contracted (experiment copy)"
+# per header: (old, new) text substitutions, each of which must apply
+REPLACEMENTS = {
+    "pixel_math.cuh": [
+        (HELPER_OLD, HELPER_NEW),
+        ("return fmul(fadd(fadd(mc, fmul(sum_side, w0)), fmul(sum_diag, w1)), gw);", "return fmul(fmad(sum_diag, w1, fmad(sum_side, w0, mc)), gw);"),
+        ("return fmaxf(fadd(1.0f, fmul(dist, nis)), 0.0f);", "return fmaxf(fmad(dist, nis, 1.0f), 0.0f);"),
+        ("pw = fsub(fmul(pw, v_adj), 0.10889456f);", "pw = fmad(pw, v_adj, -0.10889456f);"),
+        ("pw = fadd(fmul(pw, v_adj), 0.107963754f);", "pw = fmad(pw, v_adj, 0.107963754f);"),
+        ("pw = fadd(fmul(pw, v_adj), 0.018092343f);", "pw = fmad(pw, v_adj, 0.018092343f);"),
+        ("const float acc = fsub(fmul(pw, mul), 0.055f);", "const float acc = fmad(pw, mul, -0.055f);"),
+        ("o[0] = fadd(fadd(fmul(m[0], a), fmul(m[1], b)), fmul(m[2], c));", "o[0] = fmad(m[2], c, fmad(m[1], b, fmul(m[0], a)));"),
+        ("o[1] = fadd(fadd(fmul(m[3], a), fmul(m[4], b)), fmul(m[5], c));", "o[1] = fmad(m[5], c, fmad(m[4], b, fmul(m[3], a)));"),
+        ("o[2] = fadd(fadd(fmul(m[6], a), fmul(m[7], b)), fmul(m[8], c));", "o[2] = fmad(m[8], c, fmad(m[7], b, fmul(m[6], a)));"),
+    ],
+    "filter_strip.cuh": [
+        ("        d01[i] = fadd(d01[i], t01);\n        d10[i] = fadd(d10[i], t10);",
+         "        d01[i] = ffma(sc, p01, d01[i]);\n        d10[i] = ffma(sc, p10, d10[i]);"),
+        ("float sum = fadd(ce[c], fmul(wu, up[c]));", "float sum = fmad(wu, up[c], ce[c]);"),
+        ("sum = fadd(sum, fmul(wd, dn[c]));", "sum = fmad(wd, dn[c], sum);"),
+        ("sum = fadd(sum, fmul(wl, le[c]));", "sum = fmad(wl, le[c], sum);"),
+        ("sum = fadd(sum, fmul(wr, ri[c]));", "sum = fmad(wr, ri[c], sum);"),
+    ],
+}
+DIST2 = re.compile(r"fadd\(fadd\(fmul\(s0, (absdiff\([^)]*\))\), fmul\(s1, (absdiff\([^)]*\))\)\), fmul\(s2, (absdiff\([^)]*\))\)\)")
 
 
-def contracted_header(text):
-    assert HELPER_OLD in text
-    text = text.replace(HELPER_OLD, HELPER_NEW, 1)
-    for old, new in REPLACEMENTS:
+def contracted_header(name, text):
+    for old, new in REPLACEMENTS[name]:
         assert old in text, old
         text = text.replace(old, new, 1)
-    text, n = DIST2.subn(r"fs_mad(s2, \3, fs_mad(s1, \2, fs_mul(s0, \1)))", text)
-    assert n == 4
+    if name == "filter_strip.cuh":
+        text, n = DIST2.subn(r"fmad(s2, \3, fmad(s1, \2, fmul(s0, \1)))", text)
+        assert n == 4
     return text
 
 
 def prepare():
-    """A private copy of csrc/, tests/emu/ and oracle/ whose filter_strip.cuh is the contracted one."""
+    """A private copy of csrc/, tests/emu/ and oracle/ whose filter_strip.cuh and pixel_math.cuh are the contracted ones."""
     shutil.rmtree(BUILD, ignore_errors=True)
     os.makedirs(BUILD)
     shutil.copytree(os.path.join(ROOT, "jxl_oxide_b200", "csrc"), os.path.join(BUILD, "jxl_oxide_b200", "csrc"))
@@ -74,11 +75,12 @@ def prepare():
     shutil.copytree(os.path.join(ROOT, "oracle"), os.path.join(BUILD, "oracle"), ignore=shutil.ignore_patterns("_build", "_ref"))
     os.makedirs(os.path.join(BUILD, "tests"))
     shutil.copytree(os.path.join(ROOT, "tests", "emu"), os.path.join(BUILD, "tests", "emu"), ignore=shutil.ignore_patterns("_build"))
-    hdr = os.path.join(BUILD, "jxl_oxide_b200", "csrc", "kernels", "filter_strip.cuh")
-    with open(hdr) as f:
-        text = f.read()
-    with open(hdr, "w") as f:
-        f.write(contracted_header(text))
+    for name in REPLACEMENTS:
+        hdr = os.path.join(BUILD, "jxl_oxide_b200", "csrc", "kernels", name)
+        with open(hdr) as f:
+            text = f.read()
+        with open(hdr, "w") as f:
+            f.write(contracted_header(name, text))
 
 
 def sass_size(obj, kernel_tag):
@@ -149,7 +151,7 @@ def main():
     lines = ["# FMA contraction in the strip filter kernel: what it costs and what it saves (tools/fma_study.py)", "",
              "The shipped kernel rounds every product before adding, like the reference's generic path, and matches the oracle bit for",
              "bit. This experiment contracts the multiply-adds of Gaborish, the EPF distances / weights / weighted sums and the colour",
-             "stage (matrix, sRGB polynomial) into fused multiply-adds in a COPY of `kernels/filter_strip.cuh` - divisions stay IEEE -",
+             "stage (matrix, sRGB polynomial) into fused multiply-adds in a COPY of the strip kernel's headers - divisions stay IEEE -",
              "runs the copy's phases on the host (the tests/emu harness; `std::fmaf` and the device's FFMA are the same correctly",
              "rounded operation) and compares the final samples with the oracle's. Interior of the frame only (64 samples in from",
              "every edge: the strip kernel's territory).", "",
