@@ -815,6 +815,7 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
     }
     View sigma_view;
     if (vardct) sigma_view = View{st_.epf_sigma, 0, 0, st_.bw, st_.bh};
+    if (vardct && rf.epf.iters > 0) be_.stage_marker("epf_sigma", &sigma_view, 1);
     ColorParams cp;
     // colour conversion follows upsampling (render.rs:136-149), so it is fused only without it
     const bool want_colour = !upsampled && !colour_done && !lfg_.has_noise && !lfg_.has_patches && !lfg_.has_splines &&

@@ -81,6 +81,60 @@ void jxlo_linear_to_pq(float* samples, size_t n, float intensity_target) {
   for (size_t i = 0; i < n; ++i) samples[i] = jxlo::linear_to_pq(samples[i], intensity_target);
 }
 
+// Known-answer hooks: the restoration filters on three caller planes of width x height f32 samples (tightly packed),
+// filtered in place, default parameters. jxlo_epf takes the per-8x8-block sigma grid ((w + 7) / 8 x (h + 7) / 8), or
+// NULL for the constant sigma of a Modular frame.
+void jxlo_gaborish(float* p0, float* p1, float* p2, uint32_t w, uint32_t h, const float weights[6]) {
+  jxlo::OracleBackend be(1);
+  float* p[3] = {p0, p1, p2};
+  jxlb::View v[3];
+  float wt[3][2];
+  for (int c = 0; c < 3; ++c) {
+    v[c] = jxlb::View{be.alloc_plane(w, h, false), 0, 0, w, h};
+    std::memcpy(be.plane(v[c].plane).f32(), p[c], size_t(w) * h * 4);
+    wt[c][0] = weights[2 * c], wt[c][1] = weights[2 * c + 1];
+  }
+  be.gaborish(v, wt);
+  for (int c = 0; c < 3; ++c) std::memcpy(p[c], be.plane(v[c].plane).f32(), size_t(w) * h * 4);
+}
+
+void jxlo_epf(float* p0, float* p1, float* p2, uint32_t w, uint32_t h, const float* sigma, float sigma_const, uint32_t iters) {
+  jxlo::OracleBackend be(1);
+  float* p[3] = {p0, p1, p2};
+  jxlb::View v[3], sv;
+  for (int c = 0; c < 3; ++c) {
+    v[c] = jxlb::View{be.alloc_plane(w, h, false), 0, 0, w, h};
+    std::memcpy(be.plane(v[c].plane).f32(), p[c], size_t(w) * h * 4);
+  }
+  const uint32_t bw = (w + 7) / 8, bh = (h + 7) / 8;
+  if (sigma) {
+    sv = jxlb::View{be.alloc_plane(bw, bh, false), 0, 0, bw, bh};
+    std::memcpy(be.plane(sv.plane).f32(), sigma, size_t(bw) * bh * 4);
+  }
+  jxlb::EpfParams prm;
+  prm.iters = iters;
+  prm.sigma_for_modular = sigma_const;
+  be.epf(v, sv, prm, sigma == nullptr);
+  for (int c = 0; c < 3; ++c) std::memcpy(p[c], be.plane(v[c].plane).f32(), size_t(w) * h * 4);
+}
+
+// features::upsample with the default weights: `in` (width x height, tightly packed) -> `out` (width * factor x
+// height * factor), factor 2, 4 or 8.
+void jxlo_upsample(const float* in, uint32_t w, uint32_t h, uint32_t factor, float* out) {
+  jxlo::OracleBackend be(1);
+  const jxlb::View v{be.alloc_plane(w, h, false), 0, 0, w, h};
+  std::memcpy(be.plane(v.plane).f32(), in, size_t(w) * h * 4);
+  const int id = be.upsample(v, factor == 2 ? 1 : (factor == 4 ? 2 : 3), jxlb::default_image_header());
+  std::memcpy(out, be.plane(id).f32(), size_t(w) * h * factor * factor * 4);
+}
+
+// The restoration filters a decoded frame's header asks for: Gaborish on / off and the EPF iteration count.
+void jxlo_frame_filters(void* hp, int frame, uint32_t* gab_enabled, uint32_t* epf_iters) {
+  const jxlb::RestorationFilter& rf = static_cast<Handle*>(hp)->res.frames.at(frame).header.restoration_filter;
+  *gab_enabled = rf.gab_enabled ? 1 : 0;
+  *epf_iters = rf.epf.iters;
+}
+
 size_t jxlo_image_original_icc(void* hp, uint8_t* dst, size_t cap) {
   const std::vector<uint8_t>& icc = static_cast<Handle*>(hp)->res.image_header.icc_profile;
   if (dst && cap >= icc.size() && !icc.empty()) std::memcpy(dst, icc.data(), icc.size());

@@ -293,6 +293,11 @@ extern "C" int jxle_filter_geometry_check(int width, int height) {
   return 0;
 }
 
+// The kernels' sRGB transfer function (pixel_math.cuh) on n samples, so that a test can bound its distance from the exact curve
+extern "C" void jxle_linear_to_srgb(const float* in, float* out, size_t n) {
+  for (size_t i = 0; i < n; ++i) out[i] = jxlb::linear_to_srgb(in[i], jxlb::kSrgbPow);
+}
+
 namespace jxlo {
 
 bool EmuBackend::filters_colour_fused(const View v[3], const RestorationFilter& rf, const View& sigma, bool sigma_is_constant,

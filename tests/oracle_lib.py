@@ -55,6 +55,7 @@ def _load(path, make_dir):
     L.jxlo_frame_stream_channels.restype = ctypes.c_uint32
     L.jxlo_stage.argtypes = [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_int, ctypes.POINTER(ctypes.c_uint32),
                              ctypes.POINTER(ctypes.c_uint32), ctypes.c_void_p]
+    L.jxlo_frame_filters.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_uint32)]
     L.jxlo_free.argtypes = [ctypes.c_void_p]
     return L
 
@@ -96,6 +97,12 @@ class OracleImage:
         for c in range(nch):
             L.jxlo_frame_channel(self._h, idx, c, out[c].ctypes.data)
         return out, ncol, bool(vardct)
+
+    def frame_filters(self, idx=0):
+        """(Gaborish on, EPF iteration count) of the frame's header."""
+        gab, iters = ctypes.c_uint32(), ctypes.c_uint32()
+        self._L.jxlo_frame_filters(self._h, idx, ctypes.byref(gab), ctypes.byref(iters))
+        return bool(gab.value), int(iters.value)
 
     def original_icc(self):
         L = self._L

@@ -15,7 +15,7 @@ MODULAR = ["grayalpha", "squeeze_edge", "issue_311", "alpha_triangles", "bicycle
 MODULAR_BENCH = ["srgb.d0-e1.jxl", "minecraft.d0-e6.jxl"]
 VARDCT = ["opsin_inverse", "alpha_premultiplied", "minecraft_vardct_e7", "upsampling", "noise", "bike", "bench_oriented_brg", "grayscale_jpeg", "cafe", "grayscale", "issue_425", "patches"]
 VARDCT_BENCH = ["starrail.d1-e6.jxl", "nahida-motion.d1-e7.jxl"]
-STAGES_F32 = ["lf", "hf_dequant", "idct", "jpeg_upsampled", "pre_filter", "gaborish", "epf", "upsampled", "patches", "splines", "noise", "rgb"]
+STAGES_F32 = ["lf", "hf_dequant", "idct", "jpeg_upsampled", "pre_filter", "epf_sigma", "gaborish", "epf", "upsampled", "patches", "splines", "noise", "rgb"]
 
 
 def ulp_diff(a, b):

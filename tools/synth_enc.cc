@@ -13,7 +13,10 @@
 // exact alias tables, so encoder and decoder cannot disagree about symbol mapping.
 // For tests, --all-types puts every one of the 27 transform types into the frame (the largest ones also in the partial
 // groups at the right / bottom edges and next to LF-group boundaries), --only-type T tiles the frame with one type, and
-// --dump-blocks FILE writes the varblock layout; without these flags the output does not change.
+// --dump-blocks FILE writes the varblock layout; without these flags the output does not change. A VarDCT frame of one
+// group (at most 256 x 256, down to 1 x 1) is written with a single TOC entry. --no-gaborish turns Gaborish off;
+// --modular-filters SIGMA gives a --modular frame Gaborish and --epf-iters EPF iterations with constant sigma SIGMA.
+// --sharpness-cell N makes the sharpness map (and so the EPF sigma grid) change every N blocks instead of 16.
 //
 // Not part of the product; not a general-purpose encoder (it does not transform an input image).
 #include <algorithm>
@@ -60,7 +63,22 @@ struct BitWriter {
     bytes.insert(bytes.end(), o.bytes.begin(), o.bytes.end());
     total_bits += o.total_bits;
   }
+  void append_bits(const BitWriter& o) {  // any alignment on either side
+    for (uint8_t b : o.bytes) write(8, b);
+    if (o.nbits) write(o.nbits, o.acc);
+  }
 };
+
+// binary16 of a normal value (restoration-filter parameters)
+uint16_t to_f16(float f) {
+  int e;
+  const float m = std::frexp(std::fabs(f), &e);  // |f| = m * 2^e, m in [0.5, 1)
+  int E = e - 1 + 15;
+  uint32_t frac = uint32_t(std::lround((m * 2.0f - 1.0f) * 1024.0f));
+  if (frac == 1024) frac = 0, ++E;
+  if (f == 0.0f || E < 1 || E > 30) fprintf(stderr, "%g is not a normal binary16 value\n", f), exit(2);
+  return uint16_t((f < 0 ? 0x8000u : 0u) | uint32_t(E) << 10 | frac);
+}
 
 // U32 with explicit selector
 void write_u32(BitWriter& w, int sel, int bits, uint32_t v) {
@@ -578,7 +596,10 @@ struct Args {
   std::string colour;     // "" = all-default metadata (sRGB); p3 | rec2020-gamma | gray | dci | custom: an enum colour encoding
   bool lf_frame = false;  // put the LF image into a separate Modular LF frame (frame type 1, lf_level 1)
   uint32_t epf_iters = 2; // edge-preserving filter iterations (0..3); 2 = the all-default restoration filter
-  uint32_t hf_presets = 1; // HF presets (hf_pass.rs): group g uses preset g % N, each preset has its own (rotated) cluster map
+  bool gaborish = true;   // --no-gaborish: a VarDCT frame without Gaborish (or a Modular one with --modular-filters)
+  float modular_sigma = 0; // --modular-filters S: Gaborish + `epf_iters` EPF iterations on a Modular frame, sigma S (f16)
+  uint32_t sharpness_cell = 16;  // the sharpness map is constant over cells of this many 8x8 blocks (EPF sigma 0 in the first)
+  uint32_t hf_presets = 1;// HF presets (hf_pass.rs): group g uses preset g % N, each preset has its own (rotated) cluster map
   std::string dump_raw;    // --modular: also write the source image (3 planes, int32 little endian) for lossless checks
   bool modular = false;    // a Modular lossless frame (RGB 8 bit, RCT + default Squeeze, weighted predictor) instead of VarDCT
   bool all_types = false;  // every one of the 27 transform types in the frame (forced_layout), the rest drawn from all 27
@@ -929,8 +950,19 @@ int encode_modular(const Args& a) {
   cs.write(1, 1);      // is_last
   cs.write(2, 0);      // name: empty
   cs.write(1, 0);      // restoration filter: not all_default
-  cs.write(1, 0);      //   gab_enabled = 0
-  cs.write(2, 0);      //   epf iters = 0
+  if (a.modular_sigma > 0.0f) {  // filter.rs:18-166, Modular: no sharpness LUT, constant sigma sigma_for_modular
+    cs.write(1, a.gaborish ? 1 : 0);  // gab_enabled
+    if (a.gaborish) cs.write(1, 0);   // gab_custom
+    cs.write(2, a.epf_iters & 3);
+    if (a.epf_iters & 3) {
+      cs.write(1, 0);   //   epf_weight_custom
+      cs.write(1, 0);   //   epf_sigma_custom
+      cs.write(16, to_f16(a.modular_sigma));
+    }
+  } else {
+    cs.write(1, 0);    //   gab_enabled = 0
+    cs.write(2, 0);    //   epf iters = 0
+  }
   cs.write(2, 0);      //   extensions
   cs.write(2, 0);      // frame extensions
   cs.write(1, 0);      // TOC not permuted
@@ -969,6 +1001,9 @@ int main(int argc, char** argv) {
     else if (s == "--passes") a.passes = uint32_t(atoi(next().c_str()));
     else if (s == "--colour") a.colour = next();
     else if (s == "--epf-iters") a.epf_iters = uint32_t(atoi(next().c_str()));
+    else if (s == "--no-gaborish") a.gaborish = false;
+    else if (s == "--sharpness-cell") a.sharpness_cell = uint32_t(std::max(1, atoi(next().c_str())));
+    else if (s == "--modular-filters") a.modular_sigma = float(atof(next().c_str()));
     else if (s == "--hf-presets") a.hf_presets = std::max(1, atoi(next().c_str()));
     else if (s == "--modular") a.modular = true;
     else if (s == "--dump-raw") a.dump_raw = next();
@@ -989,7 +1024,12 @@ int main(int argc, char** argv) {
   const uint32_t lcols = (W + 2047) / 2048, lrows = (H + 2047) / 2048, num_lf = lcols * lrows;
   if (a.passes < 1 || a.passes > 3 || (a.passes > 1 && a.lf_frame)) fprintf(stderr, "--passes takes 1..3 (not with --lf-frame)\n"), exit(2);
   const uint32_t P = a.passes;
-  if (num_groups == 1) fprintf(stderr, "single-group frames are not produced by this tool\n"), exit(2);
+  // one group and one pass: a single TOC entry holds LfGlobal, the LF group, HfGlobal and the pass group back to back,
+  // without padding between them (toc.rs; host/frame_syntax.cc reads them from one bit position on)
+  const bool single = num_groups == 1 && P == 1;
+  auto end_section = [&](BitWriter& w) {
+    if (!single) w.pad();
+  };
 
   // ---- content ----
   // varblock layout: raster scan per LF group (the order HfMetadata stores blocks in)
@@ -1095,9 +1135,10 @@ int main(int argc, char** argv) {
     }
     hm[3].w = lw, hm[3].h = lh;
     hm[3].v.resize(size_t(lw) * lh);
-    {  // piecewise-constant sharpness
+    {  // piecewise-constant sharpness over cells of sharpness_cell x sharpness_cell blocks
+      const uint32_t sc = a.sharpness_cell;
       for (uint32_t y = 0; y < lh; ++y)
-        for (uint32_t x = 0; x < lw; ++x) hm[3].v[size_t(y) * lw + x] = int32_t(((x / 16) * 7 + (y / 16) * 3 + lg) % 8);
+        for (uint32_t x = 0; x < lw; ++x) hm[3].v[size_t(y) * lw + x] = int32_t(((x / sc) * 7 + (y / sc) * 3 + lg) % 8);
     }
     modular_tokens(tree, hm, int32_t(1 + 2 * num_lf + lg), &hfmeta_tokens[lg]);
     if (!a.lf_frame) lf_tokens_all.insert(lf_tokens_all.end(), lfcoeff_tokens[lg].begin(), lfcoeff_tokens[lg].end());
@@ -1235,7 +1276,7 @@ int main(int argc, char** argv) {
     std::vector<uint8_t> map(size_t(tree.num_leaves()));
     for (size_t i = 0; i < map.size(); ++i) map[i] = uint8_t(i);
     lf_enc.write_header(w, lf_tokens_all, uint32_t(map.size()), map);
-    w.pad();
+    end_section(w);
   }
   for (uint32_t lg = 0; lg < num_lf; ++lg) {
     BitWriter& w = sections[1 + lg];
@@ -1249,7 +1290,7 @@ int main(int argc, char** argv) {
     w.write(int(ceil_log2_nonzero(lw * lh)), nb_blocks[lg] - 1);
     write_modular_header(w);
     lf_enc.write_tokens(w, hfmeta_tokens[lg]);
-    w.pad();
+    end_section(w);
   }
   {  // HfGlobal
     BitWriter& w = sections[1 + num_lf];
@@ -1259,14 +1300,14 @@ int main(int argc, char** argv) {
       write_u32(w, 2, 0, 0);  // used_orders = 0
       hf_enc[pass].write_header(w, hf_all[pass], 495 * nbc * NP, hf_map);
     }
-    w.pad();
+    end_section(w);
   }
   for (uint32_t pass = 0; pass < P; ++pass)
     for (uint32_t g = 0; g < num_groups; ++g) {
       BitWriter& w = sections[2 + num_lf + size_t(pass) * num_groups + g];
       w.write(int(ceil_log2_nonzero(NP)), g % NP);  // hfp: 0 bits with a single preset
       hf_enc[pass].write_tokens(w, hf_tokens[size_t(pass) * num_groups + g]);
-      w.pad();
+      end_section(w);
     }
 
   // ---- codestream ----
@@ -1418,7 +1459,7 @@ int main(int argc, char** argv) {
     cs.write(2, 0);         // name: empty
     cs.write(1, 1);         // restoration filter all_default
     write_u64_small(0);     // frame extensions
-  } else if (P > 1 || a.epf_iters != 2) {
+  } else if (P > 1 || a.epf_iters != 2 || !a.gaborish) {
     cs.write(1, 0);         // all_default
     cs.write(2, 0);         // Regular
     cs.write(1, 0);         // VarDCT
@@ -1435,12 +1476,12 @@ int main(int argc, char** argv) {
     cs.write(2, 0);         // blend mode Replace
     cs.write(1, 1);         // is_last
     cs.write(2, 0);         // name: empty
-    if (a.epf_iters == 2) {
+    if (a.epf_iters == 2 && a.gaborish) {
       cs.write(1, 1);       // restoration filter all_default
-    } else {                // filter.rs: Gaborish on with default weights, `epf_iters` EPF iterations, default parameters
+    } else {                // filter.rs: Gaborish with default weights or off, `epf_iters` EPF iterations, default parameters
       cs.write(1, 0);
-      cs.write(1, 1);       //   gab_enabled
-      cs.write(1, 0);       //   gab_custom
+      cs.write(1, a.gaborish ? 1 : 0);  //   gab_enabled
+      if (a.gaborish) cs.write(1, 0);   //   gab_custom
       cs.write(2, a.epf_iters & 3);
       if (a.epf_iters & 3) {
         cs.write(1, 0);     //   epf_sharp_custom
@@ -1455,6 +1496,12 @@ int main(int argc, char** argv) {
   }
   cs.write(1, 0);  // TOC not permuted
   cs.pad();
+  if (single) {
+    BitWriter one;
+    for (const BitWriter& s : sections) one.append_bits(s);
+    one.pad();
+    sections.assign(1, one);
+  }
   for (const BitWriter& s : sections) {
     uint32_t sz = uint32_t(s.bytes.size());
     if (sz < 1024) write_u32(cs, 0, 10, sz);
