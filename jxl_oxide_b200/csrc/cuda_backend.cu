@@ -881,10 +881,11 @@ void CudaBackend::hf_dequant_cfl(VarDctState& st) {
   p.base_correlation_x = st.lfg->base_correlation_x;
   p.base_correlation_b = st.lfg->base_correlation_b;
   p.colour_factor = float(st.lfg->colour_factor);
-  // Production path: dequantisation + chroma from luma run inside the inverse transforms' load stage (hf_transform), which
-  // saves one HBM round trip of the three coefficient planes. The separate kernel remains for stage snapshots (tests
-  // compare the "hf_dequant" planes) and for chroma-subsampled frames (per-channel grids, no chroma from luma).
-  if (!capture && !st.subsampled && fuse_dequant) {
+  // Dequantisation + chroma from luma run inside the inverse transforms' load stage (hf_transform), which saves one HBM
+  // round trip of the three coefficient planes. The separate kernel runs for stage snapshots (tests compare the
+  // "hf_dequant" planes) and for chroma-subsampled frames (per-channel grids, no chroma from luma); the same transform
+  // kernels then take the planes as they are. Both forms compute through one definition of each formula (vardct.cu).
+  if (!capture && !st.subsampled) {
     pending_dequant_ = p;
     have_pending_dequant_ = true;
     return;

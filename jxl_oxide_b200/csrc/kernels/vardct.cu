@@ -55,6 +55,11 @@ __global__ void lf_dequant_kernel(DevFrame f, const DevLfDequantJob* jobs) {
   }
 }
 
+// whether channel c of a chroma-subsampled frame has its own, shifted block grid
+__device__ __forceinline__ bool channel_shifted(const DevFrame& f, uint32_t c) {
+  return f.subsampled && (f.hshift[c] | f.vshift[c]);
+}
+
 // for_each_varblocks (vardct/mod.rs:693-730): where channel c keeps the varblock starting at (bx, by); false when a
 // subsampled channel skips it. The second look-up is group-local, like the reference's.
 __device__ __forceinline__ bool channel_block(const DevFrame& f, uint32_t c, uint32_t bx, uint32_t by, uint32_t& dbx, uint32_t& dby) {
@@ -72,9 +77,47 @@ __device__ __forceinline__ bool channel_block(const DevFrame& f, uint32_t c, uin
   return true;
 }
 
+// dequant_hf_varblock_grouped + chroma_from_luma_hf_grouped (vardct/mod.rs:442-542, 570-603), one formula each, shared
+// by the separate dequantisation kernels below and the load stage of the inverse transforms.
+struct DeqBlock {
+  float mul[3];         // 65536 / (global_scale * hf_mul) * qm_scale[c]
+  const float* mat[3];  // the block's weight matrices (normal or transposed), row stride = block width
+};
+__device__ __forceinline__ DeqBlock deq_block(const DevFrame& f, const DevDequantParams& p, int32_t t, uint32_t bx, uint32_t by) {
+  DeqBlock d;
+  const uint32_t set = kDevTransformInfo[t][2], tr = kDevTransformInfo[t][4];
+  const float hf_mul = float(f.blk_mul[size_t(by) * f.bw + bx]);
+  const float base = __fdiv_rn(65536.0f, __fmul_rn(p.global_scale, hf_mul));
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    d.mul[c] = __fmul_rn(base, p.qm_scale[c]);
+    d.mat[c] = p.matrices + p.matrix_offset[(set * 3 + c) * 2 + tr];
+  }
+  return d;
+}
+__device__ __forceinline__ float deq_one(uint32_t raw, float m, float mul, float qb, float qbn) {
+  // Most coefficients are zero: 0 * quant_bias is a signed zero that the positive matrix weight (validated by the
+  // parser) and multiplier leave as it is, so the zero case needs one multiplication, and the division below stays off
+  // the common path.
+  if (raw == 0) return __fmul_rn(0.0f, qb);
+  float q = float(int32_t(raw));
+  if (fabsf(q) <= 1.0f) q = __fmul_rn(q, qb);
+  else q = __fsub_rn(q, __fdiv_rn(qbn, q));
+  q = __fmul_rn(q, m);
+  return __fmul_rn(q, mul);
+}
+// chroma-from-luma factors of the 64x64 tile that holds coefficient position (x, y) (frame coordinates)
+__device__ __forceinline__ void cfl_factors(const DevFrame& f, const DevDequantParams& p, uint32_t x, uint32_t y, float& kx, float& kb) {
+  const size_t ti = size_t(y >> 6) * f.w64 + (x >> 6);
+  kx = __fadd_rn(p.base_correlation_x, __fdiv_rn(float(f.x_from_y[ti]), p.colour_factor));
+  kb = __fadd_rn(p.base_correlation_b, __fdiv_rn(float(f.b_from_y[ti]), p.colour_factor));
+}
+
 // dequant_hf_varblock_grouped for one channel of a chroma-subsampled frame (no chroma from luma, vardct/mod.rs:353):
-// one thread per coefficient of the channel's own (shifted) grid. Subsampled channels hold 8x8 varblocks only.
-__global__ void hf_dequant_channel_kernel(DevFrame f, DevDequantParams p, int c) {
+// one thread per coefficient of the channel's own (shifted) grid. Subsampled channels hold 8x8 varblocks only. The
+// channel is a template parameter so that DeqBlock's per-channel arrays are indexed statically (not in local memory).
+template <int c>
+__global__ void hf_dequant_channel_kernel(DevFrame f, DevDequantParams p) {
   const uint32_t hs = f.hshift[c], vs = f.vshift[c];
   const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
   if (x >= (f.cw >> hs) || y >= (f.ch >> vs)) return;
@@ -102,17 +145,10 @@ __global__ void hf_dequant_channel_kernel(DevFrame f, DevDequantParams p, int c)
     ix = x - bx * 8, iy = y - by * 8;
   }
   const uint32_t w = uint32_t(kDevTransformInfo[t][0]) * 8;
-  const uint32_t set = kDevTransformInfo[t][2], tr = kDevTransformInfo[t][4];
-  const float hf_mul = float(f.blk_mul[size_t(by) * f.bw + bx]);
+  const DeqBlock db = deq_block(f, p, t, bx, by);
   const size_t i = size_t(y) * f.cw + x;
-  const float mul = __fmul_rn(__fdiv_rn(65536.0f, __fmul_rn(p.global_scale, hf_mul)), p.qm_scale[c]);
-  const float m = __ldg(p.matrices + p.matrix_offset[(set * 3 + c) * 2 + tr] + iy * w + ix);
-  float q = float(int32_t(f.coeff[c][i]));
-  if (fabsf(q) <= 1.0f) q = __fmul_rn(q, p.quant_bias[c]);
-  else q = __fsub_rn(q, __fdiv_rn(p.quant_bias_numerator, q));
-  q = __fmul_rn(q, m);
-  q = __fmul_rn(q, mul);
-  f.coeff[c][i] = __float_as_uint(q);
+  const float m = __ldg(db.mat[c] + iy * w + ix);
+  f.coeff[c][i] = __float_as_uint(deq_one(f.coeff[c][i], m, db.mul[c], p.quant_bias[c], p.quant_bias_numerator));
 }
 
 __global__ void lf_cfl_kernel(DevFrame f, float kx, float kb) {
@@ -173,25 +209,15 @@ __global__ void hf_dequant_cfl_kernel(DevFrame f, DevDequantParams p) {
     t = f.blk_type[size_t(oy) * f.bw + ox];
   }
   const uint32_t w = uint32_t(kDevTransformInfo[t][0]) * 8;
-  const uint32_t set = kDevTransformInfo[t][2], tr = kDevTransformInfo[t][4];
   const uint32_t ix = x - ox * 8, iy = y - oy * 8;
-  const float hf_mul = float(f.blk_mul[size_t(oy) * f.bw + ox]);
+  const DeqBlock db = deq_block(f, p, t, ox, oy);
   const size_t i = size_t(y) * f.cw + x;
   float v[3];
 #pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    float mul = __fmul_rn(__fdiv_rn(65536.0f, __fmul_rn(p.global_scale, hf_mul)), p.qm_scale[c]);
-    float m = __ldg(p.matrices + p.matrix_offset[(set * 3 + c) * 2 + tr] + iy * w + ix);
-    float q = float(int32_t(f.coeff[c][i]));
-    if (fabsf(q) <= 1.0f) q = __fmul_rn(q, p.quant_bias[c]);
-    else q = __fsub_rn(q, __fdiv_rn(p.quant_bias_numerator, q));
-    q = __fmul_rn(q, m);
-    q = __fmul_rn(q, mul);
-    v[c] = q;
-  }
-  size_t ti = size_t(y >> 6) * f.w64 + (x >> 6);
-  float kx = __fadd_rn(p.base_correlation_x, __fdiv_rn(float(f.x_from_y[ti]), p.colour_factor));
-  float kb = __fadd_rn(p.base_correlation_b, __fdiv_rn(float(f.b_from_y[ti]), p.colour_factor));
+  for (int c = 0; c < 3; ++c)
+    v[c] = deq_one(f.coeff[c][i], __ldg(db.mat[c] + iy * w + ix), db.mul[c], p.quant_bias[c], p.quant_bias_numerator);
+  float kx, kb;
+  cfl_factors(f, p, x, y, kx, kb);
   v[0] = __fadd_rn(v[0], __fmul_rn(kx, v[1]));
   v[2] = __fadd_rn(v[2], __fmul_rn(kb, v[1]));
 #pragma unroll
@@ -320,216 +346,23 @@ __device__ void dct1d(float* io, float* scratch, int n, bool forward) {
   }
 }
 
-struct Grid {
-  float* p;
-  int stride, w, h;
-  __device__ __forceinline__ float& at(int x, int y) { return p[y * stride + x]; }
-};
-
-// dct_2d (generic/dct.rs:5-141), executed by a single thread on a small grid. `tmp` must hold
-// 3 * max(w, h) floats.
-__device__ void dct_2d_serial(Grid io, bool forward, float* tmp) {
-  const int width = io.w, height = io.h;
-  if (width * height <= 1) return;
-  const float mul = forward ? 0.5f : 1.0f;
-  if (width == 2 && height == 1) {
-    float v0 = io.at(0, 0), v1 = io.at(1, 0);
-    io.at(0, 0) = __fmul_rn(__fadd_rn(v0, v1), mul);
-    io.at(1, 0) = __fmul_rn(__fsub_rn(v0, v1), mul);
-    return;
-  }
-  if (width == 1 && height == 2) {
-    float v0 = io.at(0, 0), v1 = io.at(0, 1);
-    io.at(0, 0) = __fmul_rn(__fadd_rn(v0, v1), mul);
-    io.at(0, 1) = __fmul_rn(__fsub_rn(v0, v1), mul);
-    return;
-  }
-  if (width == 2 && height == 2) {
-    float v00 = io.at(0, 0), v01 = io.at(1, 0), v10 = io.at(0, 1), v11 = io.at(1, 1);
-    io.at(0, 0) = __fmul_rn(__fmul_rn(__fadd_rn(__fadd_rn(__fadd_rn(v00, v01), v10), v11), mul), mul);
-    io.at(1, 0) = __fmul_rn(__fmul_rn(__fsub_rn(__fadd_rn(__fsub_rn(v00, v01), v10), v11), mul), mul);
-    io.at(0, 1) = __fmul_rn(__fmul_rn(__fsub_rn(__fsub_rn(__fadd_rn(v00, v01), v10), v11), mul), mul);
-    io.at(1, 1) = __fmul_rn(__fmul_rn(__fadd_rn(__fsub_rn(__fsub_rn(v00, v01), v10), v11), mul), mul);
-    return;
-  }
-  float* line = tmp;
-  float* scratch = tmp + (width > height ? width : height);
-  if (height == 1) {
-    for (int x = 0; x < width; ++x) line[x] = io.at(x, 0);
-    dct1d(line, scratch, width, forward);
-    for (int x = 0; x < width; ++x) io.at(x, 0) = line[x];
-    return;
-  }
-  if (width == 1) {
-    for (int y = 0; y < height; ++y) line[y] = io.at(0, y);
-    dct1d(line, scratch, height, forward);
-    for (int y = 0; y < height; ++y) io.at(0, y) = line[y];
-    return;
-  }
-  if (height == 2) {
-    for (int x = 0; x < width; ++x) {
-      float t0 = io.at(x, 0), t1 = io.at(x, 1);
-      io.at(x, 0) = __fmul_rn(__fadd_rn(t0, t1), mul);
-      io.at(x, 1) = __fmul_rn(__fsub_rn(t0, t1), mul);
-    }
-    for (int r = 0; r < 2; ++r) {
-      for (int x = 0; x < width; ++x) line[x] = io.at(x, r);
-      dct1d(line, scratch, width, forward);
-      for (int x = 0; x < width; ++x) io.at(x, r) = line[x];
-    }
-    return;
-  }
-  if (width == 2) {
-    for (int y = 0; y < height; ++y) {
-      float v0 = io.at(0, y), v1 = io.at(1, y);
-      io.at(0, y) = __fmul_rn(__fadd_rn(v0, v1), mul);
-      io.at(1, y) = __fmul_rn(__fsub_rn(v0, v1), mul);
-    }
-    for (int c = 0; c < 2; ++c) {
-      for (int y = 0; y < height; ++y) line[y] = io.at(c, y);
-      dct1d(line, scratch, height, forward);
-      for (int y = 0; y < height; ++y) io.at(c, y) = line[y];
-    }
-    return;
-  }
-  for (int y = 0; y < height; ++y) {
-    for (int x = 0; x < width; ++x) line[x] = io.at(x, y);
-    dct1d(line, scratch, width, forward);
-    for (int x = 0; x < width; ++x) io.at(x, y) = line[x];
-  }
-  for (int x = 0; x < width; ++x) {
-    for (int y = 0; y < height; ++y) line[y] = io.at(x, y);
-    dct1d(line, scratch, height, forward);
-    for (int y = 0; y < height; ++y) io.at(x, y) = line[y];
-  }
-}
-
-// generic/transform.rs -------------------------------------------------------------------------
-__device__ void aux_idct2(Grid b, int size, float* s /* size*size */) {
-  const int n = size / 2;
-  for (int y = 0; y < n; ++y)
-    for (int x = 0; x < n; ++x) {
-      float c00 = b.at(x, y), c01 = b.at(x + n, y), c10 = b.at(x, y + n), c11 = b.at(x + n, y + n);
-      s[(2 * y) * size + 2 * x] = __fadd_rn(__fadd_rn(__fadd_rn(c00, c01), c10), c11);
-      s[(2 * y) * size + 2 * x + 1] = __fsub_rn(__fsub_rn(__fadd_rn(c00, c01), c10), c11);
-      s[(2 * y + 1) * size + 2 * x] = __fsub_rn(__fadd_rn(__fsub_rn(c00, c01), c10), c11);
-      s[(2 * y + 1) * size + 2 * x + 1] = __fadd_rn(__fsub_rn(__fsub_rn(c00, c01), c10), c11);
-    }
-  for (int y = 0; y < size; ++y)
-    for (int x = 0; x < size; ++x) b.at(x, y) = s[y * size + x];
-}
-
-// All 8x8 "special" transforms, executed by one thread on an 8x8 grid in shared memory.
-__device__ void transform_special(Grid c, int type, float* scratch /* 64 + 48 floats */) {
-  float* tmp = scratch + 64;
-  if (type == 2) {  // Dct2
-    aux_idct2(c, 2, scratch);
-    aux_idct2(c, 4, scratch);
-    aux_idct2(c, 8, scratch);
-  } else if (type == 3) {  // Dct4
-    aux_idct2(c, 2, scratch);
-    for (int y = 0; y < 2; ++y)
-      for (int x = 0; x < 2; ++x) {
-        Grid s{scratch + (y * 2 + x) * 16, 4, 4, 4};
-        for (int iy = 0; iy < 4; ++iy)
-          for (int ix = 0; ix < 4; ++ix) s.at(iy, ix) = c.at(x + ix * 2, y + iy * 2);
-      }
-    for (int k = 0; k < 4; ++k) dct_2d_serial(Grid{scratch + k * 16, 4, 4, 4}, false, tmp);
-    for (int y = 0; y < 2; ++y)
-      for (int x = 0; x < 2; ++x)
-        for (int iy = 0; iy < 4; ++iy)
-          for (int ix = 0; ix < 4; ++ix) c.at(x * 4 + ix, y * 4 + iy) = scratch[(y * 2 + x) * 16 + iy * 4 + ix];
-  } else if (type == 1) {  // Hornuss
-    aux_idct2(c, 2, scratch);
-    for (int y = 0; y < 2; ++y)
-      for (int x = 0; x < 2; ++x) {
-        float* s = scratch + (y * 2 + x) * 16;
-        for (int iy = 0; iy < 4; ++iy)
-          for (int ix = 0; ix < 4; ++ix) s[iy * 4 + ix] = c.at(x + ix * 2, y + iy * 2);
-        float residual_sum = 0.0f;
-        for (int i = 1; i < 16; ++i) residual_sum = __fadd_rn(residual_sum, s[i]);
-        float avg = __fsub_rn(s[0], __fdiv_rn(residual_sum, 16.0f));
-        s[0] = s[5];
-        s[5] = 0.0f;
-        for (int i = 0; i < 16; ++i) s[i] = __fadd_rn(s[i], avg);
-      }
-    for (int y = 0; y < 2; ++y)
-      for (int x = 0; x < 2; ++x)
-        for (int iy = 0; iy < 4; ++iy)
-          for (int ix = 0; ix < 4; ++ix) c.at(x * 4 + ix, y * 4 + iy) = scratch[(y * 2 + x) * 16 + iy * 4 + ix];
-  } else if (type == 12 || type == 13) {  // Dct4x8 / Dct8x4
-    float coeff0 = c.at(0, 0), coeff1 = c.at(0, 1);
-    c.at(0, 0) = __fadd_rn(coeff0, coeff1);
-    c.at(0, 1) = __fsub_rn(coeff0, coeff1);
-    for (int idx = 0; idx < 2; ++idx) {
-      Grid s{scratch + idx * 32, 8, 8, 4};
-      for (int iy = 0; iy < 4; ++iy)
-        for (int ix = 0; ix < 8; ++ix) s.at(ix, iy) = c.at(ix, iy * 2 + idx);
-      dct_2d_serial(s, false, tmp);
-    }
-    if (type == 13) {
-      for (int y = 0; y < 8; ++y)
-        for (int x = 0; x < 8; ++x) c.at(y, x) = scratch[y * 8 + x];
-    } else {
-      for (int y = 0; y < 8; ++y)
-        for (int x = 0; x < 8; ++x) c.at(x, y) = scratch[y * 8 + x];
-    }
-  } else {  // Afv0..3
-    const int n = type - 14;
-    const int flip_x = n % 2, flip_y = n / 2;
-    float* coeff_afv = scratch;        // 16
-    float* samples_afv = scratch + 16; // 16
-    float* s4x4 = scratch + 32;        // 16
-    float* s4x8 = scratch + 48;        // 32
-    float* tmp2 = scratch + 80;        // 24 (3 * 8)
-    coeff_afv[0] = __fmul_rn(__fadd_rn(__fadd_rn(c.at(0, 0), c.at(1, 0)), c.at(0, 1)), 4.0f);
-    for (int idx = 1; idx < 16; ++idx) coeff_afv[idx] = c.at(2 * (idx % 4), 2 * (idx / 4));
-    for (int j = 0; j < 16; ++j) samples_afv[j] = 0.0f;
-    for (int i = 0; i < 16; ++i)
-      for (int j = 0; j < 16; ++j) samples_afv[j] = __fmaf_rn(coeff_afv[i], kAfvBasis[i][j], samples_afv[j]);
-    for (int i = 0; i < 16; ++i) s4x4[i] = 0.0f;
-    for (int i = 0; i < 32; ++i) s4x8[i] = 0.0f;
-    s4x4[0] = __fadd_rn(__fsub_rn(c.at(0, 0), c.at(1, 0)), c.at(0, 1));
-    for (int iy = 0; iy < 4; ++iy)
-      for (int ix = 0; ix < 4; ++ix) {
-        if ((ix | iy) == 0) continue;
-        s4x4[ix * 4 + iy] = c.at(2 * ix + 1, 2 * iy);
-      }
-    dct_2d_serial(Grid{s4x4, 4, 4, 4}, false, tmp2);
-    s4x8[0] = __fsub_rn(c.at(0, 0), c.at(0, 1));
-    for (int iy = 0; iy < 4; ++iy)
-      for (int ix = 0; ix < 8; ++ix) {
-        if ((ix | iy) == 0) continue;
-        s4x8[iy * 8 + ix] = c.at(ix, 2 * iy + 1);
-      }
-    dct_2d_serial(Grid{s4x8, 8, 8, 4}, false, tmp2);
-    for (int iy = 0; iy < 4; ++iy) {
-      int afv_y = flip_y == 0 ? iy : 3 - iy;
-      for (int ix = 0; ix < 4; ++ix) {
-        int afv_x = flip_x == 0 ? ix : 3 - ix;
-        c.at(flip_x * 4 + ix, flip_y * 4 + iy) = samples_afv[afv_y * 4 + afv_x];
-      }
-    }
-    for (int iy = 0; iy < 4; ++iy)
-      for (int ix = 0; ix < 4; ++ix) c.at((1 - flip_x) * 4 + ix, flip_y * 4 + iy) = s4x4[iy * 4 + ix];
-    for (int iy = 0; iy < 4; ++iy)
-      for (int ix = 0; ix < 8; ++ix) c.at(ix, (1 - flip_y) * 4 + iy) = s4x8[iy * 8 + ix];
-  }
-}
-
-// transform_varblocks_inner (transform_common.rs:11-75): one CTA per (8x8 cell, channel); cells
-// that are not a varblock origin exit immediately. First, correctness-oriented version: rows then
-// columns straight on the coefficient plane (L1/L2 resident), one thread per line.
-//
-// Varblocks are independent, so the frame is first sorted into three work lists by size class and
-// each class gets a persistent (grid-stride) kernel shaped for it:
-//   small  (8x8 cells: DCT8 and the nine "special" 8x8 transforms): 8 threads per block, one row /
-//          column per thread in registers, 32 blocks per CTA;
-//   medium (16x8 ... 32x32): one warp per block, tile staged in shared memory (stride 33), one
-//          row / column per lane in registers;
-//   large  (64x64 ... 256x256): one 64-thread CTA per block, line buffers in shared memory.
-// Every variant performs exactly the reference's operations per line (rows first, then columns,
-// generic/dct.rs:93-140), so results are bit-identical to the single-threaded formulation.
+// transform_varblocks_inner (transform_common.rs:11-75). Varblocks are independent, so classify_varblocks_kernel first
+// sorts the frame into work lists by size class, and each class gets a persistent (grid-stride) kernel shaped for it:
+//   idct_small_kernel    8x8 cells (DCT8 and the nine "special" 8x8 transforms), one list per type: 8 threads per block,
+//                        one row / column per thread in registers, 32 blocks per CTA;
+//   idct_medium_kernel   16x8 ... 32x32, one list per shape: a warp per 32 x 32 tile of equally shaped blocks in shared
+//                        memory, one row / column per lane in registers, one instantiation per shape;
+//   idct_large64_kernel  64x64, 64x32, 32x64: a 128-thread CTA per block, one channel at a time staged in shared memory,
+//                        64-point lines split between two threads;
+//   idct_large_kernel    128 and 256 samples: a 64-thread CTA per block, lines walked in global memory.
+// With DEQ the coefficient planes still hold quantised integers, and the load stage dequantises them and applies chroma
+// from luma; without, the planes are already dequantised and the load stage takes them as they are. The small, medium
+// and 64-sample kernels take one work item per varblock and its channels in the order Y, X, B (Y's dequantised samples
+// feed the chroma channels). idct_large_kernel dequantises the three channels in place and then transforms them in
+// plane order; without DEQ it takes one work item per (varblock, channel): a frame often holds fewer of these blocks
+// than there are SMs, and with one item per block the transforms of a frame holding all 27 types took twice as long
+// (H100 80GB HBM3, 700 W). Every variant performs exactly the reference's operations per line (rows first, then
+// columns, generic/dct.rs:93-140), so results are bit-identical to the single-threaded formulation.
 
 // Medium class, by shape (width x height in 8x8 cells): 2x1 1x2 2x2 4x1 1x4 4x2 2x4 4x4. The medium kernel walks the shapes
 // one after the other so that the warps of an SM execute the same transform sizes at the same time (its unrolled
@@ -543,8 +376,8 @@ __host__ __device__ inline int medium_shape(int w8, int h8) {
 constexpr int kSmallTypes = 10;
 __host__ __device__ inline int small_type_index(int t) { return t < 4 ? t : t - 8; }  // types 0-3 and 12-17
 struct TransformLists {
-  uint32_t* counts;  // [0]: unused, [2], [3]: large64, large256; [4..11]: medium shapes; [12..21]: small types
-  uint32_t* items[4];
+  uint32_t* counts;  // [2], [3]: large64, large256; [4..11]: medium shapes; [12..21]: small types ([0], [1] unused)
+  uint32_t* large_items[2];  // large64, large256
   uint32_t* shape_items[kMediumShapes];
   uint32_t* small_items[kSmallTypes];
 };
@@ -570,7 +403,7 @@ __global__ void classify_varblocks_kernel(DevFrame f, TransformLists L) {
   if (int(lane) == leader) base = atomicAdd(L.counts + key, uint32_t(__popc(peers)));
   base = __shfl_sync(peers, base, leader);
   const uint32_t slot = base + uint32_t(__popc(peers & ((1u << lane) - 1)));
-  uint32_t* list = key >= 12 ? L.small_items[key - 12] : (key >= 4 ? L.shape_items[key - 4] : L.items[key]);
+  uint32_t* list = key >= 12 ? L.small_items[key - 12] : (key >= 4 ? L.shape_items[key - 4] : L.large_items[key - 2]);
   list[slot] = bx | (by << 16);
 }
 
@@ -605,8 +438,8 @@ struct RegIdct<4> {
 };
 
 // LLF of a multi-cell varblock: forward DCT of its bw x bh LF samples, rescaled
-// (transform_common.rs:33-58). `llf` holds bw*bh floats, `tmp` 3*max(bw,bh).
-// Shapes up to 4x4 cells, by one thread in registers: exactly the branches dct_2d_serial() takes for
+// (transform_common.rs:33-58). `llf` holds bw*bh floats.
+// Shapes up to 4x4 cells, by one thread in registers: exactly the branches the reference's dct_2d takes for
 // these sizes (generic/dct.rs:5-141), unrolled.
 __device__ __forceinline__ void llf_fwd4(float* a, int stride) {  // forward DCT-4 on a[0], a[stride], ...
   float v[4] = {a[0], a[stride], a[2 * stride], a[3 * stride]};
@@ -676,7 +509,7 @@ __device__ void compute_llf_small(const DevFrame& f, int c, uint32_t bx, uint32_
 }
 
 // The nine "special" 8x8 transforms (generic/transform.rs:50-240) by the 8 threads of a group:
-// the same per-element operation sequences as transform_special(), with the independent 1-D
+// the same per-element operation sequences as the reference's single-threaded code, with the independent 1-D
 // transforms / butterflies / dot products spread over the threads. `g`: the 8x8 block (row-major,
 // stride 8), `s`: 128 floats of scratch, both in shared memory; `r`: thread index in the group.
 __device__ __forceinline__ void idct4_strided(float* p, int stride) {
@@ -809,44 +642,6 @@ __device__ void transform_special_coop(float* g, int type, float* s, int r, uint
   }
 }
 
-// dequant_hf_varblock_grouped + chroma_from_luma_hf_grouped (vardct/mod.rs:442-542, 570-603) folded into the load
-// stage of the inverse transforms: per varblock, the three channels are dequantised together (chroma from luma needs
-// the dequantised Y coefficient at the same position), then transformed. Same operations in the same order as
-// hf_dequant_cfl_kernel, so the result is bit-identical to the two-pass form.
-struct DeqBlock {
-  float mul[3];         // 65536 / (global_scale * hf_mul) * qm_scale[c]
-  const float* mat[3];  // the block's weight matrices (normal or transposed), row stride = block width
-};
-__device__ __forceinline__ DeqBlock deq_block(const DevFrame& f, const DevDequantParams& p, int32_t t, uint32_t bx, uint32_t by) {
-  DeqBlock d;
-  const uint32_t set = kDevTransformInfo[t][2], tr = kDevTransformInfo[t][4];
-  const float hf_mul = float(f.blk_mul[size_t(by) * f.bw + bx]);
-  const float base = __fdiv_rn(65536.0f, __fmul_rn(p.global_scale, hf_mul));
-#pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    d.mul[c] = __fmul_rn(base, p.qm_scale[c]);
-    d.mat[c] = p.matrices + p.matrix_offset[(set * 3 + c) * 2 + tr];
-  }
-  return d;
-}
-__device__ __forceinline__ float deq_one(uint32_t raw, float m, float mul, float qb, float qbn) {
-  // Most coefficients are zero: 0 * quant_bias is a signed zero that the positive matrix weight (validated by the
-  // parser) and multiplier leave as it is, so the zero case needs one multiplication, and the division below stays off
-  // the common path.
-  if (raw == 0) return __fmul_rn(0.0f, qb);
-  float q = float(int32_t(raw));
-  if (fabsf(q) <= 1.0f) q = __fmul_rn(q, qb);
-  else q = __fsub_rn(q, __fdiv_rn(qbn, q));
-  q = __fmul_rn(q, m);
-  return __fmul_rn(q, mul);
-}
-// chroma-from-luma factors of the 64x64 tile that holds coefficient position (x, y) (frame coordinates)
-__device__ __forceinline__ void cfl_factors(const DevFrame& f, const DevDequantParams& p, uint32_t x, uint32_t y, float& kx, float& kb) {
-  const size_t ti = size_t(y >> 6) * f.w64 + (x >> 6);
-  kx = __fadd_rn(p.base_correlation_x, __fdiv_rn(float(f.x_from_y[ti]), p.colour_factor));
-  kb = __fadd_rn(p.base_correlation_b, __fdiv_rn(float(f.b_from_y[ti]), p.colour_factor));
-}
-
 // Measured: idct_small requesting the three channels' rows of a block together costs registers and a third of its warps;
 // idct_medium trips of 8 rows beat 4 and 16.
 constexpr int kMediumTrip = 8;      // idct_medium: tile rows whose loads are in flight together
@@ -858,15 +653,13 @@ __global__ void __launch_bounds__(kSmallGroups * 8, kSmallMinBlocks) idct_small_
   __shared__ float s_special[kSmallGroups][192];  // 8 x 8 copy + 128 scratch
   const uint32_t group = threadIdx.x >> 3, r = threadIdx.x & 7;
   const uint32_t gmask = 0xffu << (8 * ((threadIdx.x & 31) >> 3));
-  // DEQ: one work item per varblock (the three channels together: Y first, its dequantised row feeds the chroma
-  // channels); else one per (varblock, channel)
   float* tile = s_tile[group];
 #pragma unroll 1
   for (int list = 0; list < kSmallTypes; ++list) {
   const uint32_t* __restrict__ items = lists.small_items[list];
-  const uint32_t total = DEQ ? lists.counts[12 + list] : lists.counts[12 + list] * 3;
+  const uint32_t total = lists.counts[12 + list];
   for (uint32_t work = blockIdx.x * kSmallGroups + group; work < total; work += gridDim.x * kSmallGroups) {
-    const uint32_t item = items[DEQ ? work : work / 3];
+    const uint32_t item = items[work];
     const uint32_t sbx = item & 0xffff, sby = item >> 16;
     const int32_t t = f.blk_type[size_t(sby) * f.bw + sbx];
     DeqBlock db;
@@ -876,8 +669,8 @@ __global__ void __launch_bounds__(kSmallGroups * 8, kSmallMinBlocks) idct_small_
       cfl_factors(f, dq, sbx * 8, sby * 8, kx, kb);
     }
 #pragma unroll 1
-    for (int ci = 0; ci < (DEQ ? 3 : 1); ++ci) {
-      const uint32_t c = DEQ ? (ci == 0 ? 1u : (ci == 1 ? 0u : 2u)) : work % 3;
+    for (int ci = 0; ci < 3; ++ci) {
+      const uint32_t c = ci == 0 ? 1u : (ci == 1 ? 0u : 2u);
       uint32_t bx, by;  // where channel c keeps this block
       if (!channel_block(f, c, sbx, sby, bx, by)) continue;
       float* row = reinterpret_cast<float*>(f.coeff[c]) + (size_t(by) * 8 + r) * f.cw + size_t(bx) * 8;
@@ -938,142 +731,27 @@ __device__ __noinline__ void idct_line_smem(float* p, int stride) {
   for (int i = 0; i < N; ++i) p[i * stride] = v[i];
 }
 
-__device__ __forceinline__ void idct_line_dispatch(float* p, int stride, int n) {
-  if (n == 8) idct_line_smem<8>(p, stride);
-  else if (n == 16) idct_line_smem<16>(p, stride);
-  else idct_line_smem<32>(p, stride);
-}
-
-constexpr int kMediumWarps = 4;
-// One varblock of a warp's 32 x 32 tile (idct_medium_kernel).
-struct MediumSub {
-  uint32_t bx[3], by[3];  // where channel c keeps the block (8x8 cells); by == 0xffffffff: the channel skips it
-};
-// Varblocks of 16x8 ... 32x32 samples of frames whose coefficients are already dequantised, one warp per 32 x 32 TILE of
-// them: a tile holds (32 / w) x (32 / h) blocks of the shape being walked (8 of 16x8, 4 of 16x16, 1 of 32x32), so the row
-// pass (lane = tile row) and the column pass (lane = tile column) keep all 32 lanes busy whatever the shape; with one
-// block per warp a 16x8 block used 8 and 16 lanes of 32. Per block nothing changes: same loads, same operation order in
-// the line transforms. `dq` is unused: the launch passes the same arguments to every transform kernel.
-__global__ void __launch_bounds__(kMediumWarps * 32) idct_medium_kernel(DevFrame f, DevDequantParams dq, TransformLists lists) {
-  __shared__ float s_tile[kMediumWarps][32 * 33];
-  __shared__ float s_llf[kMediumWarps][8][16];
-  __shared__ MediumSub s_sub[kMediumWarps][8];
-  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  float* tile = s_tile[warp];
-  MediumSub* sub = s_sub[warp];
-#pragma unroll 1
-  for (int shape = 0; shape < kMediumShapes; ++shape) {
-    const uint32_t* __restrict__ items = lists.shape_items[shape];
-    const uint32_t total = lists.counts[4 + shape];
-    if (total == 0) continue;
-    // every entry of a shape's list has the same transform type
-    const uint32_t item0 = items[0];
-    const int32_t t = f.blk_type[size_t(item0 >> 16) * f.bw + (item0 & 0xffff)];
-    const int bw = kDevTransformInfo[t][0], bh = kDevTransformInfo[t][1];
-    const int w = bw * 8, h = bh * 8;
-    const int logw = 31 - __clz(w), logh = 31 - __clz(h);
-    const int lognx = 5 - logw, logny = 5 - logh, logp = lognx + logny;  // blocks across, down, per tile
-    const int ny = 1 << logny;
-    // this lane's tile column: block column sx, sample column x inside the block
-    const int sx = int(lane) >> logw, x = int(lane) & (w - 1);
-#pragma unroll 1
-    for (uint32_t group = blockIdx.x * kMediumWarps + warp; (group << logp) < total; group += gridDim.x * kMediumWarps) {
-      const uint32_t first = group << logp;
-      const int nb = int(min(uint32_t(1) << logp, total - first));
-      __syncwarp();
-      if (int(lane) < nb) {  // lane s describes block s of the tile
-        MediumSub m;
-        const uint32_t item = items[first + lane];
-        const uint32_t sbx = item & 0xffff, sby = item >> 16;
-#pragma unroll
-        for (uint32_t c = 0; c < 3; ++c) {
-          uint32_t bx, by;
-          const bool has = channel_block(f, c, sbx, sby, bx, by);
-          m.bx[c] = bx;
-          m.by[c] = has ? by : 0xffffffffu;
-        }
-        sub[lane] = m;
-      }
-      __syncwarp();
-#pragma unroll 1
-      for (int ci = 0; ci < 3; ++ci) {
-        const uint32_t c = uint32_t(ci);
-        // the (up to 4) blocks of this lane's tile column
-        float* col[4];
-#pragma unroll
-        for (int sy = 0; sy < 4; ++sy) {
-          const int s = (sy << lognx) + sx;
-          col[sy] = nullptr;
-          if (sy < ny && s < nb && sub[s].by[c] != 0xffffffffu)
-            col[sy] = reinterpret_cast<float*>(f.coeff[c]) + size_t(sub[s].by[c]) * 8 * f.cw + size_t(sub[s].bx[c]) * 8 + x;
-        }
-        // 32 tile rows, kMediumTrip per trip, all loads of a trip issued before the first use
-#pragma unroll 1
-        for (int y0 = 0; y0 < 32; y0 += kMediumTrip) {
-          float raw[kMediumTrip];
-#pragma unroll
-          for (int j = 0; j < kMediumTrip; ++j) {
-            const int Y = y0 + j, sy = Y >> logh, y = Y & (h - 1);
-            const float* src = sy == 0 ? col[0] : (sy == 1 ? col[1] : (sy == 2 ? col[2] : col[3]));
-            raw[j] = src ? src[size_t(y) * f.cw] : 0.0f;
-          }
-#pragma unroll
-          for (int j = 0; j < kMediumTrip; ++j) tile[(y0 + j) * 33 + int(lane)] = raw[j];
-        }
-        // lowest frequencies from the LF image: lane s for block s, then 16 lanes place the (at most) 16 values of the tile
-        if (int(lane) < nb && sub[lane].by[c] != 0xffffffffu) compute_llf_small(f, int(c), sub[lane].bx[c], sub[lane].by[c], bw, bh, s_llf[warp][lane]);
-        __syncwarp();
-        if (lane < 16) {
-          const int cells_log = (logw - 3) + (logh - 3);  // LLF values per block
-          const int s = int(lane) >> cells_log, local = int(lane) & ((1 << cells_log) - 1);
-          if (s < nb && sub[s].by[c] != 0xffffffffu) {
-            const int ly = local >> (logw - 3), lx = local & (bw - 1);
-            tile[(((s >> lognx) << logh) + ly) * 33 + ((s & ((1 << lognx) - 1)) << logw) + lx] = s_llf[warp][s][local];
-          }
-        }
-        __syncwarp();
-        {  // rows: lane = tile row, the row's blocks one after the other
-          const int sy = int(lane) >> logh;
-          for (int bxi = 0; bxi < (1 << lognx); ++bxi)
-            if ((sy << lognx) + bxi < nb) idct_line_dispatch(tile + lane * 33 + (bxi << logw), 1, w);
-        }
-        __syncwarp();
-        for (int sy = 0; sy < ny; ++sy)  // columns: lane = tile column
-          if ((sy << lognx) + sx < nb) idct_line_dispatch(tile + (sy << logh) * 33 + lane, 33, h);
-        __syncwarp();
-#pragma unroll 1
-        for (int y0 = 0; y0 < 32; y0 += 4) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int Y = y0 + j, sy = Y >> logh, y = Y & (h - 1);
-            float* dst = sy == 0 ? col[0] : (sy == 1 ? col[1] : (sy == 2 ? col[2] : col[3]));
-            if (dst) dst[size_t(y) * f.cw] = tile[Y * 33 + int(lane)];
-          }
-        }
-        __syncwarp();
-      }
-    }
-  }
-}
-
-// ---- medium varblocks, dequantising form, one instantiation per shape --------------------------------------------------
-// Same tiling as idct_medium_kernel (one warp per 32 x 32 tile of equally shaped blocks, lane = tile column in the load /
-// column / store passes, lane = tile row in the row pass) and the same per-sample operations in the same order, but the
-// shape is a template parameter: block-row / row loops are static, so the per-sample pointer selection, shifts and table
-// look-ups of the generic body (which spent several times more instructions on indexing than on arithmetic) fold into
-// immediates. The shapes are walked one after the other by all CTAs in step, so one instantiation's code is hot at a time,
-// and the line transforms are the shared idct_line_smem<N>.
+// ---- medium varblocks (16x8 ... 32x32), one instantiation per shape ----------------------------------------------------
+// One warp per 32 x 32 tile of equally shaped blocks: a tile holds (32 / w) x (32 / h) blocks (8 of 16x8, 4 of 16x16, 1 of
+// 32x32), so the row pass (lane = tile row) and the column pass (lane = tile column, as in the load and store passes) keep
+// all 32 lanes busy whatever the shape. The shape is a template parameter: block-row / row loops are static, so per-sample
+// pointer selection, shifts and table look-ups fold into immediates (a generic body with run-time shape spent several
+// times more instructions on indexing than on arithmetic). The shapes are walked one after the other by all CTAs in step,
+// so one instantiation's code is hot at a time, and the line transforms are the shared idct_line_smem<N>.
 // medium_walk unrolls the block rows and 8-row batches of a tile: as loops they take less than half the instructions, but
 // were measured slower.
+constexpr int kMediumWarps = 4;
 constexpr int kMediumOuterUnroll = 32;
 struct MediumBlk {
-  uint32_t bx, by;     // block position in 8x8 cells (dequantising frames are never subsampled: the same for all channels)
+  // block position in 8x8 cells, the same for every channel transformed: dequantising frames are never subsampled, and
+  // on subsampled frames the shifted channels, which hold 8x8 blocks only, are skipped
+  uint32_t bx, by;
   float mul[3];        // DeqBlock::mul
   float kx[4], kb[4];  // chroma-from-luma factors of the 2 x 2 64x64 tiles at (tx0, ty0)
   int xsplit, ysplit;  // first sample column / row of the block that lies in the right / lower 64x64 tile (>= w / h: none)
 };
 
-template <int LOGW, int LOGH>
+template <bool DEQ, int LOGW, int LOGH>
 __device__ __forceinline__ void medium_walk(const DevFrame& f, const DevDequantParams& dq, const uint32_t* __restrict__ items,
                                             uint32_t total, float* tile, float* ytile, float (*llf)[16], MediumBlk* sub,
                                             uint32_t first_group, uint32_t group_stride, uint32_t lane) {
@@ -1092,17 +770,19 @@ __device__ __forceinline__ void medium_walk(const DevFrame& f, const DevDequantP
       MediumBlk m;
       const uint32_t item = items[first + lane];
       m.bx = item & 0xffff, m.by = item >> 16;
-      const DeqBlock db = deq_block(f, dq, t, m.bx, m.by);
-      const uint32_t tx0 = (m.bx * 8) >> 6, ty0 = (m.by * 8) >> 6;
+      if (DEQ) {
+        const DeqBlock db = deq_block(f, dq, t, m.bx, m.by);
+        const uint32_t tx0 = (m.bx * 8) >> 6, ty0 = (m.by * 8) >> 6;
 #pragma unroll
-      for (int c = 0; c < 3; ++c) m.mul[c] = db.mul[c];
+        for (int c = 0; c < 3; ++c) m.mul[c] = db.mul[c];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const uint32_t tx = min(tx0 + uint32_t(i & 1), f.w64 - 1), ty = min(ty0 + uint32_t(i >> 1), (f.ch + 63) / 64 - 1);
-        cfl_factors(f, dq, tx << 6, ty << 6, m.kx[i], m.kb[i]);
+        for (int i = 0; i < 4; ++i) {
+          const uint32_t tx = min(tx0 + uint32_t(i & 1), f.w64 - 1), ty = min(ty0 + uint32_t(i >> 1), (f.ch + 63) / 64 - 1);
+          cfl_factors(f, dq, tx << 6, ty << 6, m.kx[i], m.kb[i]);
+        }
+        m.xsplit = int((tx0 + 1) * 64 - m.bx * 8);
+        m.ysplit = int((ty0 + 1) * 64 - m.by * 8);
       }
-      m.xsplit = int((tx0 + 1) * 64 - m.bx * 8);
-      m.ysplit = int((ty0 + 1) * 64 - m.by * 8);
       sub[lane] = m;
     }
     __syncwarp();
@@ -1111,6 +791,9 @@ __device__ __forceinline__ void medium_walk(const DevFrame& f, const DevDequantP
       const uint32_t c = ci == 0 ? 1u : (ci == 1 ? 0u : 2u);  // Y first: its dequantised samples feed the chroma channels
       // (requesting the chroma rows into L2 while Y is transformed was measured slower, with more DRAM reads: the tile's three
       // channels already overlap across the SM's warps)
+      // Without DEQ, a shifted channel of a subsampled frame is skipped: the HF decoders reject a frame in which a shifted
+      // channel holds a multi-cell varblock (hf_coeff.rs:143-155), so channel_block() is false for it on every block here.
+      if (!DEQ && channel_shifted(f, c)) continue;
       const float* __restrict__ matc = dq.matrices + dq.matrix_offset[(set * 3 + c) * 2 + tr] + x;
       const float qb = dq.quant_bias[c], qbn = dq.quant_bias_numerator;
       float* const plane = reinterpret_cast<float*>(f.coeff[c]);
@@ -1125,20 +808,23 @@ __device__ __forceinline__ void medium_walk(const DevFrame& f, const DevDequantP
         const float k_top = c == 0 ? m.kx[xt] : m.kb[xt], k_bottom = c == 0 ? m.kx[xt + 2] : m.kb[xt + 2];
         const int ysplit = m.ysplit;
 #pragma unroll kMediumOuterUnroll
-        for (int y0 = 0; y0 < H; y0 += 8) {
-          float raw[8], mt[8];
+        for (int y0 = 0; y0 < H; y0 += kMediumTrip) {
+          float raw[kMediumTrip], mt[kMediumTrip];
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
+          for (int j = 0; j < kMediumTrip; ++j) {
             raw[j] = have ? src[size_t(y0 + j) * f.cw] : 0.0f;
-            mt[j] = __ldg(matc + (y0 + j) * W);
+            if (DEQ) mt[j] = __ldg(matc + (y0 + j) * W);
           }
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
+          for (int j = 0; j < kMediumTrip; ++j) {
             const int y = y0 + j, Y = sy * H + y;
-            const float q = deq_one(__float_as_uint(raw[j]), mt[j], mulc, qb, qbn);
-            float v = q;
-            if (c == 1) ytile[Y * 33 + int(lane)] = q;
-            else v = __fadd_rn(q, __fmul_rn(y >= ysplit ? k_bottom : k_top, ytile[Y * 33 + int(lane)]));
+            float v = raw[j];
+            if (DEQ) {
+              const float q = deq_one(__float_as_uint(raw[j]), mt[j], mulc, qb, qbn);
+              v = q;
+              if (c == 1) ytile[Y * 33 + int(lane)] = q;
+              else v = __fadd_rn(q, __fmul_rn(y >= ysplit ? k_bottom : k_top, ytile[Y * 33 + int(lane)]));
+            }
             tile[Y * 33 + int(lane)] = v;
           }
         }
@@ -1181,10 +867,13 @@ __device__ __forceinline__ void medium_walk(const DevFrame& f, const DevDequantP
   }
 }
 
-constexpr int kMediumMinBlocks = 5;  // the fastest of 4 / 5 / 6 when measured; not re-measured on the H100
-__global__ void __launch_bounds__(kMediumWarps * 32, kMediumMinBlocks) idct_medium_deq_kernel(DevFrame f, DevDequantParams dq, TransformLists lists) {
+// With DEQ: the fastest of 4 / 5 / 6 when measured; not re-measured on the H100. Without, the register cap of 5 CTAs per
+// SM makes the kernel spill, so it asks for none.
+constexpr int kMediumMinBlocks = 5;
+template <bool DEQ>
+__global__ void __launch_bounds__(kMediumWarps * 32, DEQ ? kMediumMinBlocks : 1) idct_medium_kernel(DevFrame f, DevDequantParams dq, TransformLists lists) {
   __shared__ float s_tile[kMediumWarps][32 * 33];
-  __shared__ float s_ytile[kMediumWarps][32 * 33];  // dequantised Y coefficients (chroma from luma)
+  __shared__ float s_ytile[kMediumWarps][DEQ ? 32 * 33 : 1];  // dequantised Y coefficients (chroma from luma)
   __shared__ float s_llf[kMediumWarps][8][16];
   __shared__ MediumBlk s_sub[kMediumWarps][8];
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -1197,14 +886,14 @@ __global__ void __launch_bounds__(kMediumWarps * 32, kMediumMinBlocks) idct_medi
     float* tile = s_tile[warp];
     float* yt = s_ytile[warp];
     switch (shape) {  // medium_shape(): 0: 16x8, 1: 8x16, 2: 16x16, 3: 32x8, 4: 8x32, 5: 32x16, 6: 16x32, 7: 32x32 (w x h samples)
-      case 0: medium_walk<4, 3>(f, dq, items, total, tile, yt, s_llf[warp], s_sub[warp], g0, gs, lane); break;
-      case 1: medium_walk<3, 4>(f, dq, items, total, tile, yt, s_llf[warp], s_sub[warp], g0, gs, lane); break;
-      case 2: medium_walk<4, 4>(f, dq, items, total, tile, yt, s_llf[warp], s_sub[warp], g0, gs, lane); break;
-      case 3: medium_walk<5, 3>(f, dq, items, total, tile, yt, s_llf[warp], s_sub[warp], g0, gs, lane); break;
-      case 4: medium_walk<3, 5>(f, dq, items, total, tile, yt, s_llf[warp], s_sub[warp], g0, gs, lane); break;
-      case 5: medium_walk<5, 4>(f, dq, items, total, tile, yt, s_llf[warp], s_sub[warp], g0, gs, lane); break;
-      case 6: medium_walk<4, 5>(f, dq, items, total, tile, yt, s_llf[warp], s_sub[warp], g0, gs, lane); break;
-      default: medium_walk<5, 5>(f, dq, items, total, tile, yt, s_llf[warp], s_sub[warp], g0, gs, lane); break;
+      case 0: medium_walk<DEQ, 4, 3>(f, dq, items, total, tile, yt, s_llf[warp], s_sub[warp], g0, gs, lane); break;
+      case 1: medium_walk<DEQ, 3, 4>(f, dq, items, total, tile, yt, s_llf[warp], s_sub[warp], g0, gs, lane); break;
+      case 2: medium_walk<DEQ, 4, 4>(f, dq, items, total, tile, yt, s_llf[warp], s_sub[warp], g0, gs, lane); break;
+      case 3: medium_walk<DEQ, 5, 3>(f, dq, items, total, tile, yt, s_llf[warp], s_sub[warp], g0, gs, lane); break;
+      case 4: medium_walk<DEQ, 3, 5>(f, dq, items, total, tile, yt, s_llf[warp], s_sub[warp], g0, gs, lane); break;
+      case 5: medium_walk<DEQ, 5, 4>(f, dq, items, total, tile, yt, s_llf[warp], s_sub[warp], g0, gs, lane); break;
+      case 6: medium_walk<DEQ, 4, 5>(f, dq, items, total, tile, yt, s_llf[warp], s_sub[warp], g0, gs, lane); break;
+      default: medium_walk<DEQ, 5, 5>(f, dq, items, total, tile, yt, s_llf[warp], s_sub[warp], g0, gs, lane); break;
     }
   }
 }
@@ -1308,13 +997,13 @@ __global__ void __launch_bounds__(kLargeThreads) idct_large_kernel(DevFrame f, D
 }
 
 
-// ---- 64-sample varblocks (64x64, 64x32, 32x64), dequantising form: the block is staged in shared memory ---------------------
-// idct_large_kernel dequantises the three channels in place in global memory and then lets every thread walk a row, later a
-// column, of the block in global memory (one 4-byte request per sample, a warp's requests 64 rows apart). Here a CTA
-// keeps one channel of the block in a 64 x 65 shared tile: coefficients arrive with coalesced loads and are dequantised
-// on the way in (the dequantised Y copy stays in a second tile for chroma from luma), rows are transformed in place,
-// columns likewise (l64_idct_pass), and the samples leave with coalesced stores - one read and one write
-// of HBM per sample. Per sample the operations and their order are those of idct_large_kernel.
+// ---- 64-sample varblocks (64x64, 64x32, 32x64): the block is staged in shared memory -----------------------------------------
+// idct_large_kernel lets every thread walk a row, later a column, of the block in global memory (one 4-byte request per
+// sample, a warp's requests 64 rows apart). Here a CTA keeps one channel of the block in a 64 x 65 shared tile:
+// coefficients arrive with coalesced loads (with DEQ dequantised on the way in, the dequantised Y copy staying in a
+// second tile for chroma from luma), rows are transformed in place, columns likewise (l64_idct_pass), and the samples
+// leave with coalesced stores - one read and one write of HBM per sample. Per sample the operations and their order are
+// those of idct_large_kernel.
 // One 1-D inverse-DCT pass over the lines of the shared tile by 128 threads. A 64-point line is split between two threads
 // the way Dct1D<64>::run(inverse) splits it (generic/dct.rs:239-293): even-indexed and odd-indexed samples go through
 // independent 32-point transforms (register-resident RegIdct<32>, the same operation sequence as Dct1D<32>), the
@@ -1375,11 +1064,12 @@ __device__ __forceinline__ void l64_idct_pass(float* tile, int nlines, int len, 
 
 constexpr int kL64Threads = 128, kL64Pitch = 65, kL64Line = 2 * 8 + 1;  // line buffers: the forward DCT of the <= 8 x 8 LF samples only
 constexpr int kL64SmemFloats = 2 * 64 * kL64Pitch + 64 + 8 * kL64Line;
-__global__ void __launch_bounds__(kL64Threads, 3) idct_large64_deq_kernel(DevFrame f, DevDequantParams dq, const uint32_t* __restrict__ items,
-                                                                       const uint32_t* __restrict__ count_ptr) {
+template <bool DEQ>
+__global__ void __launch_bounds__(kL64Threads, 3) idct_large64_kernel(DevFrame f, DevDequantParams dq, const uint32_t* __restrict__ items,
+                                                                   const uint32_t* __restrict__ count_ptr) {
   extern __shared__ float s_l64[];
   float* tile = s_l64;                      // the channel being transformed
-  float* ytile = tile + 64 * kL64Pitch;     // dequantised Y
+  float* ytile = tile + 64 * kL64Pitch;     // dequantised Y (DEQ only)
   float* llf = ytile + 64 * kL64Pitch;      // <= 8 x 8 LF samples
   float* lines = llf + 64;                  // 8 per-thread line + scratch buffers for the LF samples' forward DCT
   __shared__ float s_k[2][25];
@@ -1392,16 +1082,21 @@ __global__ void __launch_bounds__(kL64Threads, 3) idct_large64_deq_kernel(DevFra
     const int bw = kDevTransformInfo[t][0], bh = kDevTransformInfo[t][1];
     const int w = bw * 8, h = bh * 8;
     const int logw = 31 - __clz(w);
-    const DeqBlock db = deq_block(f, dq, t, sbx, sby);
+    DeqBlock db;
+    if (DEQ) db = deq_block(f, dq, t, sbx, sby);
     const uint32_t tx0 = (sbx * 8) >> 6, ty0 = (sby * 8) >> 6;
-    if (tid < 25) {
-      const uint32_t tx = min(tx0 + uint32_t(tid) % 5, f.w64 - 1), ty = min(ty0 + uint32_t(tid) / 5, (f.ch + 63) / 64 - 1);
-      cfl_factors(f, dq, tx << 6, ty << 6, s_k[0][tid], s_k[1][tid]);
+    if (DEQ) {
+      if (tid < 25) {
+        const uint32_t tx = min(tx0 + uint32_t(tid) % 5, f.w64 - 1), ty = min(ty0 + uint32_t(tid) / 5, (f.ch + 63) / 64 - 1);
+        cfl_factors(f, dq, tx << 6, ty << 6, s_k[0][tid], s_k[1][tid]);
+      }
+      __syncthreads();
     }
-    __syncthreads();
 #pragma unroll 1
     for (int ci = 0; ci < 3; ++ci) {
       const uint32_t c = ci == 0 ? 1u : (ci == 1 ? 0u : 2u);
+      // as in idct_medium_kernel: on the frames that reach the transforms, shifted channels hold 8x8 blocks only
+      if (!DEQ && channel_shifted(f, c)) continue;
       float* const block = reinterpret_cast<float*>(f.coeff[c]) + size_t(sby) * 8 * f.cw + size_t(sbx) * 8;
       const float* __restrict__ matc = db.mat[c];
       const float mulc = db.mul[c], qb = dq.quant_bias[c], qbn = dq.quant_bias_numerator;
@@ -1412,18 +1107,21 @@ __global__ void __launch_bounds__(kL64Threads, 3) idct_large64_deq_kernel(DevFra
         for (int j = 0; j < 8; ++j) {
           const int idx = idx0 + j * kL64Threads, x = idx & (w - 1), y = idx >> logw;
           raw[j] = block[size_t(y) * f.cw + x];
-          mt[j] = __ldg(matc + idx);
+          if (DEQ) mt[j] = __ldg(matc + idx);
         }
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const int idx = idx0 + j * kL64Threads, x = idx & (w - 1), y = idx >> logw;
-          const float q = deq_one(__float_as_uint(raw[j]), mt[j], mulc, qb, qbn);
-          float v = q;
-          if (c == 1) {
-            ytile[y * kL64Pitch + x] = q;
-          } else {
-            const int ti = int(((sbx * 8 + uint32_t(x)) >> 6) - tx0) + 5 * int(((sby * 8 + uint32_t(y)) >> 6) - ty0);
-            v = __fadd_rn(q, __fmul_rn(s_k[c == 0 ? 0 : 1][ti], ytile[y * kL64Pitch + x]));
+          float v = raw[j];
+          if (DEQ) {
+            const float q = deq_one(__float_as_uint(raw[j]), mt[j], mulc, qb, qbn);
+            v = q;
+            if (c == 1) {
+              ytile[y * kL64Pitch + x] = q;
+            } else {
+              const int ti = int(((sbx * 8 + uint32_t(x)) >> 6) - tx0) + 5 * int(((sby * 8 + uint32_t(y)) >> 6) - ty0);
+              v = __fadd_rn(q, __fmul_rn(s_k[c == 0 ? 0 : 1][ti], ytile[y * kL64Pitch + x]));
+            }
           }
           tile[y * kL64Pitch + x] = v;
         }
@@ -1488,7 +1186,9 @@ void launch_hf_dequant_cfl(DevFrame f, DevDequantParams p, cudaStream_t stream) 
   dim3 block(64, 4);
   dim3 grid((f.cw + 63) / 64, (f.ch + 3) / 4);
   if (f.subsampled) {
-    for (int c = 0; c < 3; ++c) hf_dequant_channel_kernel<<<grid, block, 0, stream>>>(f, p, c);
+    hf_dequant_channel_kernel<0><<<grid, block, 0, stream>>>(f, p);
+    hf_dequant_channel_kernel<1><<<grid, block, 0, stream>>>(f, p);
+    hf_dequant_channel_kernel<2><<<grid, block, 0, stream>>>(f, p);
     return;
   }
   hf_dequant_cfl_kernel<<<grid, block, 0, stream>>>(f, p);
@@ -1496,25 +1196,21 @@ void launch_hf_dequant_cfl(DevFrame f, DevDequantParams p, cudaStream_t stream) 
 
 size_t hf_transform_scratch_bytes(uint32_t bw, uint32_t bh) {
   const size_t cells = size_t(bw) * bh;
-  // counters | small | (former medium list) | large | huge | the eight medium shapes (cells/2 x 2, /4 x 3, /8 x 2, /16)
-  // ... | the ten small types (cells each)
-  return 256 + (cells + cells / 2 + 2 * (cells / 32 + 1) + 64) * 4 + (cells * 9 / 4 + 64) * 4 + size_t(kSmallTypes) * (cells + 1) * 4;
+  // counters | large64 | large256 | the eight medium shapes (cells/2 x 2, /4 x 3, /8 x 2, /16) | the ten small types (cells each)
+  return 256 + 2 * (cells / 32 + 1) * 4 + (cells * 9 / 4 + 64) * 4 + size_t(kSmallTypes) * (cells + 1) * 4;
 }
 
 namespace {
 template <bool DEQ>
 void launch_idcts(DevFrame f, const DevDequantParams& dq, const TransformLists& L, size_t cells, int num_sms, cudaStream_t stream) {
-  const size_t per = DEQ ? 1 : 3;  // work items per varblock
-  const int small_grid = int(std::min<size_t>((cells * per + kSmallGroups - 1) / kSmallGroups, size_t(num_sms) * 8));
+  const int small_grid = int(std::min<size_t>((cells + kSmallGroups - 1) / kSmallGroups, size_t(num_sms) * 8));
   idct_small_kernel<DEQ><<<small_grid, kSmallGroups * 8, 0, stream>>>(f, dq, L);
-  const int medium_grid = int(std::min<size_t>((cells / 2 * per + kMediumWarps) / kMediumWarps, size_t(num_sms) * 8));
-  if (DEQ) idct_medium_deq_kernel<<<medium_grid, kMediumWarps * 32, 0, stream>>>(f, dq, L);
-  else idct_medium_kernel<<<medium_grid, kMediumWarps * 32, 0, stream>>>(f, dq, L);
-  const int large_grid = int(std::min<size_t>((cells / 32 + 1) * per, size_t(num_sms) * 4));
-  if (DEQ) idct_large64_deq_kernel<<<large_grid, kL64Threads, kL64SmemFloats * 4, stream>>>(f, dq, L.items[2], L.counts + 2);
-  else idct_large_kernel<DEQ><<<large_grid, kLargeThreads, (1024 + kLargeThreads * (2 * 64 + 1)) * 4, stream>>>(f, dq, L.items[2], L.counts + 2, 64);
-  const int huge_grid = int(std::min<size_t>((cells / 128 + 1) * per, size_t(num_sms)));
-  idct_large_kernel<DEQ><<<huge_grid, kLargeThreads, (1024 + kLargeThreads * (2 * 256 + 1)) * 4, stream>>>(f, dq, L.items[3], L.counts + 3, 256);
+  const int medium_grid = int(std::min<size_t>((cells / 2 + kMediumWarps) / kMediumWarps, size_t(num_sms) * 8));
+  idct_medium_kernel<DEQ><<<medium_grid, kMediumWarps * 32, 0, stream>>>(f, dq, L);
+  const int large_grid = int(std::min<size_t>(cells / 32 + 1, size_t(num_sms) * 4));
+  idct_large64_kernel<DEQ><<<large_grid, kL64Threads, kL64SmemFloats * 4, stream>>>(f, dq, L.large_items[0], L.counts + 2);
+  const int huge_grid = int(std::min<size_t>((cells / 128 + 1) * (DEQ ? 1 : 3), size_t(num_sms)));
+  idct_large_kernel<DEQ><<<huge_grid, kLargeThreads, (1024 + kLargeThreads * (2 * 256 + 1)) * 4, stream>>>(f, dq, L.large_items[1], L.counts + 3, 256);
 }
 }  // namespace
 
@@ -1524,14 +1220,11 @@ void launch_hf_transform(DevFrame f, void* scratch, const DevDequantParams* dq, 
   const size_t cells = size_t(f.bw) * f.bh;
   TransformLists L;
   L.counts = static_cast<uint32_t*>(scratch);
-  uint32_t* base = L.counts + 64;
-  L.items[0] = base;                                   // <= cells
-  L.items[1] = L.items[0] + cells;                     // <= cells / 2
-  L.items[2] = L.items[1] + cells / 2 + 1;             // <= cells / 32
-  L.items[3] = L.items[2] + cells / 32 + 1;            // <= cells / 128
+  L.large_items[0] = L.counts + 64;                     // <= cells / 32
+  L.large_items[1] = L.large_items[0] + cells / 32 + 1;  // <= cells / 128
   {  // a shape's list holds at most cells / (cells per block of that shape) entries
     static const int kShapeCells[kMediumShapes] = {2, 2, 4, 4, 4, 8, 8, 16};
-    uint32_t* q = L.items[3] + cells / 128 + 1;
+    uint32_t* q = L.large_items[1] + cells / 128 + 1;
     for (int sh = 0; sh < kMediumShapes; ++sh) {
       L.shape_items[sh] = q;
       q += cells / kShapeCells[sh] + 1;
@@ -1551,7 +1244,8 @@ void launch_hf_transform(DevFrame f, void* scratch, const DevDequantParams* dq, 
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
     cudaFuncSetAttribute(idct_large_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 140 * 1024);
     cudaFuncSetAttribute(idct_large_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 140 * 1024);
-    cudaFuncSetAttribute(idct_large64_deq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kL64SmemFloats * 4);
+    cudaFuncSetAttribute(idct_large64_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kL64SmemFloats * 4);
+    cudaFuncSetAttribute(idct_large64_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kL64SmemFloats * 4);
     return n;
   }();
   if (dq && !f.subsampled) {
