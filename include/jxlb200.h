@@ -128,8 +128,9 @@ int32_t jxlb_set_fuse_filters(jxlb_decoder* dec, int32_t on);
  * many streams share one CTA and its staged tables. 0 (default, = 16), 4 (= 8), 8, 16, 32: one warp per stream, all
  * presets' tables staged once per CTA - the shortest time for ONE frame; 64 / 128: one thread per stream (32 streams
  * per warp): slower for a frame alone, but 16 warps instead of 510, which is what a GPU full of frames wants
- * (jxlb_pipeline_create's default). Frames whose HF presets' cluster maps together exceed 32 KB always run one thread per
- * stream, 128 per CTA. Results are identical; the process-wide default comes from the environment variable JXLB_HF_LANES. */
+ * (jxlb_pipeline_create's default). Frames whose HF presets' cluster maps together exceed 32 KB, and passes whose HF code
+ * uses LZ77, always run one thread per stream, 128 per CTA. Results are identical; the process-wide default comes from the
+ * environment variable JXLB_HF_LANES. */
 int32_t jxlb_set_hf_streams_per_cta(jxlb_decoder* dec, int32_t streams);
 int32_t jxlb_stage_count(const jxlb_decoder* dec, const char* name);
 int32_t jxlb_stage_get(const jxlb_decoder* dec, const char* name, int32_t idx, uint32_t* width, uint32_t* height,

@@ -761,9 +761,10 @@ void CudaBackend::decode_hf(VarDctState& st, std::vector<HfGroupJob>& jobs) {
   if (jobs.empty()) return;
   const uint32_t pass = jobs[0].pass_idx;
   const HfPassSyntax& hp = st.hfg->passes[pass];
-  // The coefficient kernels read plain hybrid-uint tokens; an LZ77-enabled HF code (legal, hf_coeff.rs:181-222 goes
-  // through read_varint_with_multiplier_clustered, but no known encoder emits it) would decode silently wrong.
-  const bool hf_lz77 = hp.code.lz77_enabled;  // reported after the launch: a stream that is invalid anyway keeps its own error
+  // An LZ77 code runs the thread-per-stream kernel's LZ77 variant (hf_schedule), which has no chroma-subsampled form.
+  const bool hf_lz77 = hp.code.lz77_enabled;
+  JXLB_CHECK(!(hf_lz77 && st.subsampled), kErrUnsupported,
+             "LZ77 in the HF coefficient streams of a chroma-subsampled frame is not supported on the device");
   const DevHfParams p = build_hf_params(st, pass, *this, d_natural_orders_, natural_order_offset_);
   const HfSchedule sched = hf_schedule(p, hf_streams_per_cta);
   const std::vector<uint32_t> perm = hf_launch_order(jobs, sched.lanes);  // launch order -> `jobs`
@@ -784,10 +785,16 @@ void CudaBackend::decode_hf(VarDctState& st, std::vector<HfGroupJob>& jobs) {
     launch_hf_block_list(dev_frame(st), p, d_list, d_counts, S());
     end_k();
   }
+  uint32_t* d_lz = nullptr;  // one LZ77 window per stream, for this launch only
+  const size_t lz_len = hf_lz77 ? hf_lz77_window_entries(st.group_dim) : 0;
+  if (hf_lz77) {
+    d_lz = static_cast<uint32_t*>(dmalloc(jobs.size() * lz_len * 4));
+    temps_.push_back(d_lz);
+  }
   begin_k("decode_hf");
   if (sched.lanes)
     launch_decode_hf_lanes(active_cs_, dev_frame(st), p, d_list, d_counts, d_jobs, d_end, d_status, int(jobs.size()),
-                           pass == 0 ? 1 : 0, sched.per_cta, S());
+                           pass == 0 ? 1 : 0, sched.per_cta, S(), d_lz, uint32_t(lz_len));
   else
     launch_decode_hf(active_cs_, dev_frame(st), p, d_jobs, d_end, d_status, int(jobs.size()), pass == 0 ? 1 : 0,
                      sched.per_cta, S());
@@ -804,7 +811,6 @@ void CudaBackend::decode_hf(VarDctState& st, std::vector<HfGroupJob>& jobs) {
            std::string("HF group ") + std::to_string(job.group_idx) + ": " + dev_status_message(status[i]));
     job.end_bit = size_t(end[i]);
   }
-  JXLB_CHECK(!hf_lz77, kErrUnsupported, "LZ77 in the HF coefficient streams is not supported on the device");
 }
 
 void CudaBackend::lf_dequant(VarDctState& st, const std::vector<LfDequantJob>& jobs) {

@@ -264,13 +264,15 @@ __global__ void __launch_bounds__(256) hf_block_list_kernel(DevFrame f, DevHfPar
   if (tid == 0) counts[g] = base;
 }
 
-template <bool SUB, bool STAGED>
+// LZ77: stream `job_idx` keeps its values in lz_windows[job_idx * lz_window_len ...] (unused otherwise).
+template <bool SUB, bool STAGED, bool LZ77>
 __global__ void __launch_bounds__(128) decode_hf_lanes_kernel(const uint8_t* __restrict__ cs, DevFrame f, DevHfParams p,
                                                               const uint2* __restrict__ list,
                                                               const uint32_t* __restrict__ counts,
                                                               const DevHfJob* __restrict__ jobs,
                                                               uint64_t* __restrict__ end_bits, int* __restrict__ status,
-                                                              int num_jobs, int first_pass) {
+                                                              int num_jobs, int first_pass,
+                                                              uint32_t* lz_windows, uint32_t lz_window_len) {
   extern __shared__ __align__(16) uint8_t smem[];
   const uint32_t tid = threadIdx.x, nthreads = blockDim.x;
   const HfLaneSmem L = hf_lane_layout(p, nthreads);
@@ -330,8 +332,15 @@ __global__ void __launch_bounds__(128) decode_hf_lanes_kernel(const uint8_t* __r
   if (job_idx >= num_jobs) return;
   const DevHfJob job = jobs[job_idx];
   const uint32_t gb = p.group_dim_blocks;
-  hf_lane_stream<SUB, STAGED>(cs, f, p, T, list + size_t(job.group_idx) * gb * gb, __ldg(counts + job.group_idx), job,
-                              first_pass, end_bits + job_idx, status + job_idx);
+  if constexpr (LZ77) {
+    Lz77State lz;
+    lz77_init(lz, lz_windows + size_t(job_idx) * lz_window_len, lz_window_len);
+    hf_lane_stream<SUB, STAGED, true>(cs, f, p, T, list + size_t(job.group_idx) * gb * gb, __ldg(counts + job.group_idx),
+                                      job, first_pass, &lz, end_bits + job_idx, status + job_idx);
+  } else {
+    hf_lane_stream<SUB, STAGED, false>(cs, f, p, T, list + size_t(job.group_idx) * gb * gb, __ldg(counts + job.group_idx),
+                                       job, first_pass, nullptr, end_bits + job_idx, status + job_idx);
+  }
 }
 
 }  // namespace
@@ -349,29 +358,32 @@ void launch_hf_block_list(DevFrame f, DevHfParams p, uint2* list, uint32_t* coun
 
 void launch_decode_hf_lanes(const uint8_t* cs, DevFrame f, DevHfParams p, const uint2* list, const uint32_t* counts,
                             const DevHfJob* jobs, uint64_t* end_bits, int* status, int num_jobs, int first_pass,
-                            int streams_per_cta, cudaStream_t stream) {
+                            int streams_per_cta, cudaStream_t stream, uint32_t* lz_windows, uint32_t lz_window_len) {
   if (num_jobs <= 0) return;
   // C++ function-local statics are initialised once, thread-safely: no worker thread launches before the limits are set
   static const bool attr_set = [] {
-    cudaFuncSetAttribute(decode_hf_lanes_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(decode_hf_lanes_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(decode_hf_lanes_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(decode_hf_lanes_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(decode_hf_lanes_kernel<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(decode_hf_lanes_kernel<true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(decode_hf_lanes_kernel<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(decode_hf_lanes_kernel<true, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(decode_hf_lanes_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     return true;
   }();
   (void)attr_set;
   const int nthreads = streams_per_cta <= 64 ? 64 : 128;
   const HfLaneSmem L = hf_lane_layout(p, uint32_t(nthreads));
   const int ctas = (num_jobs + nthreads - 1) / nthreads;
-#define JXLB_HF_LANES(SUB_, STAGED_)                                                                                 \
-  decode_hf_lanes_kernel<SUB_, STAGED_><<<ctas, nthreads, L.total, stream>>>(cs, f, p, list, counts, jobs, end_bits, \
-                                                                             status, num_jobs, first_pass)
-  if (hf_lane_staged(p, L)) {
-    if (f.subsampled) JXLB_HF_LANES(true, true);
-    else JXLB_HF_LANES(false, true);
+#define JXLB_HF_LANES(SUB_, STAGED_, LZ77_)                                                                        \
+  decode_hf_lanes_kernel<SUB_, STAGED_, LZ77_><<<ctas, nthreads, L.total, stream>>>(                               \
+      cs, f, p, list, counts, jobs, end_bits, status, num_jobs, first_pass, lz_windows, lz_window_len)
+  if (p.code.lz77_enabled) {  // the caller rejects chroma-subsampled frames with an LZ77 code
+    JXLB_HF_LANES(false, false, true);
+  } else if (hf_lane_staged(p, L)) {
+    if (f.subsampled) JXLB_HF_LANES(true, true, false);
+    else JXLB_HF_LANES(false, true, false);
   } else {
-    if (f.subsampled) JXLB_HF_LANES(true, false);
-    else JXLB_HF_LANES(false, false);
+    if (f.subsampled) JXLB_HF_LANES(true, false, false);
+    else JXLB_HF_LANES(false, false, false);
   }
 #undef JXLB_HF_LANES
 }

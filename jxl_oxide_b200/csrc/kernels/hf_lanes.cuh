@@ -18,11 +18,17 @@
 #ifndef __CUDACC__
 #include <cstring>
 #include <vector>
+
+#include "../launch_tables.h"  // hf_lz77_window_entries
 #endif
 
 // Hook for the host emulation's SIMT model (tests/emu: which kind of symbol each loop trip decodes); nothing on the device.
 #ifndef JXLB_LANE_TRIP
 #define JXLB_LANE_TRIP(is_coefficient)
+#endif
+// Hook for the host emulation: values one LZ77 stream took from copies (tests/emu/hf_lz77_emu.cc counts them).
+#ifndef JXLB_LANE_LZ77_COPIED
+#define JXLB_LANE_LZ77_COPIED(n)
 #endif
 
 namespace jxlb {
@@ -202,9 +208,10 @@ __host__ __device__ inline HfLaneSmem hf_lane_layout(const DevHfParams& p, uint3
   L.total = off;
   return L;
 }
-// The staged variant of hf_lane_decode: an ANS code whose alias tables and cluster maps are both in shared memory.
+// The staged variant of hf_lane_decode: an ANS code without LZ77 whose alias tables and cluster maps are both in shared
+// memory. An LZ77 code always runs the general variant.
 __host__ __device__ inline bool hf_lane_staged(const DevHfParams& p, const HfLaneSmem& L) {
-  return !p.code.use_prefix && L.ans != 0xffffffffu && L.cmap != 0xffffffffu;
+  return !p.code.lz77_enabled && !p.code.use_prefix && L.ans != 0xffffffffu && L.cmap != 0xffffffffu;
 }
 
 // Tables one CTA shares, read through `Mem`. Always in shared memory: tinfo, order_offset, ctx, cfg, bctx, nz. The staged variant reads
@@ -308,11 +315,17 @@ __device__ __forceinline__ bool hf_block_record(const DevFrame& f, const DevHfPa
 
 // One stream. STAGED (hf_lane_staged): every table access goes through `Mem`, the bit reader is topped up once per
 // trip and the symbol path has no prefix-code or global-table branch; otherwise the general reader and tables.
+// LZ77 (general variant only): the code has LZ77 enabled, and every value -- non-zero count or coefficient -- goes
+// through lz77_read_value with distance multiplier 0 (hf_coeff.rs:181-222), keeping the stream's values in `*lz`'s
+// window (hf_lz77_window_entries of them). A copy still pending when the group ends is ignored, as in the reference.
+// Without LZ77, `lz` is unused (null).
 // `list` / `count`: this stream's group's varblock records.
-template <bool SUB, bool STAGED, class Mem>
+template <bool SUB, bool STAGED, bool LZ77, class Mem>
 __device__ __forceinline__ void hf_lane_stream(const uint8_t* __restrict__ cs, const DevFrame& f, const DevHfParams& p,
                                                const HfLaneView<Mem>& T, const uint2* __restrict__ list, uint32_t count,
-                                               const DevHfJob& job, int first_pass, uint64_t* end_bit, int* status) {
+                                               const DevHfJob& job, int first_pass, Lz77State* lz, uint64_t* end_bit,
+                                               int* status) {
+  static_assert(!(LZ77 && STAGED), "LZ77 codes run the general variant");
   using Addr = typename Mem::Addr;
   DevBitReader br;  // general variant
   HfBits hb;        // staged variant
@@ -438,7 +451,13 @@ __device__ __forceinline__ void hf_lane_stream(const uint8_t* __restrict__ cs, c
       hb.top_up();
       value = hf_read_value<Mem, true, false, true>(T.code, hb, ans_state, cl, last_word + 3, &past);
     } else {
-      value = cv_read_uint(br, Mem::u32(T.code.cfg + cl * 4), cv_read_symbol(T.cv, ans_state, br, cl));
+      // `if constexpr`: the variants without LZ77 keep the code they had before the LZ77 variant existed
+      if constexpr (LZ77) {
+        value = lz77_read_value(T.cv, p.code, *lz, ans_state, br, cl, 0, err);
+        if (err != kDevOk) break;
+      } else {
+        value = cv_read_uint(br, Mem::u32(T.code.cfg + cl * 4), cv_read_symbol(T.cv, ans_state, br, cl));
+      }
       past = br.next_word > stop_word;
     }
     if (past) {
@@ -532,10 +551,18 @@ struct HfLaneTables {
 
 // One stream on the host: `blk_ctx` holds hf_block_ctx_cell() of every cell of the frame (bw x bh); the stream's group
 // list is compacted from it in raster order, and the stream runs the variant the device launcher would pick for `p`.
+// An LZ77 code runs with a window of the device's size (hf_lz77_window_entries) and reports the number of values it
+// took from copies through JXLB_LANE_LZ77_COPIED; like CudaBackend::decode_hf, it is not supported in a chroma-subsampled
+// frame (status kDevUnsupported).
 template <bool SUB>
 inline void hf_lane_decode(const uint8_t* cs, const DevFrame& f, const DevHfParams& p, const HfLaneTables& T,
                            const uint32_t* blk_ctx, const DevHfJob& job, uint8_t* nz, uint32_t nz_stride, int first_pass,
                            uint64_t* end_bit, int* status) {
+  if (p.code.lz77_enabled && f.subsampled) {
+    *end_bit = job.bit_pos;
+    *status = kDevUnsupported;
+    return;
+  }
   const HfGroupRect r = hf_group_rect(f, p, job.group_idx);
   std::vector<uint2> list;
   for (uint32_t y = 0; y < r.height; ++y)
@@ -564,10 +591,16 @@ inline void hf_lane_decode(const uint8_t* cs, const DevFrame& f, const DevHfPara
   V.cv = T.cv;
   const uint2* recs = list.data();
   const uint32_t n = uint32_t(list.size());
-  if (hf_lane_staged(p, hf_lane_layout(p, nz_stride)))
-    hf_lane_stream<SUB, true>(cs, f, p, V, recs, n, job, first_pass, end_bit, status);
+  if (p.code.lz77_enabled) {
+    std::vector<uint32_t> window(hf_lz77_window_entries(p.group_dim_blocks * 8));
+    Lz77State lz;
+    lz77_init(lz, window.data(), window.size());
+    hf_lane_stream<SUB, false, true>(cs, f, p, V, recs, n, job, first_pass, &lz, end_bit, status);
+    JXLB_LANE_LZ77_COPIED(lz.copied);
+  } else if (hf_lane_staged(p, hf_lane_layout(p, nz_stride)))
+    hf_lane_stream<SUB, true, false>(cs, f, p, V, recs, n, job, first_pass, nullptr, end_bit, status);
   else
-    hf_lane_stream<SUB, false>(cs, f, p, V, recs, n, job, first_pass, end_bit, status);
+    hf_lane_stream<SUB, false, false>(cs, f, p, V, recs, n, job, first_pass, nullptr, end_bit, status);
 }
 #endif
 

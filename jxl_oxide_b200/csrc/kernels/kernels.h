@@ -177,11 +177,14 @@ void launch_decode_hf(const uint8_t* codestream, DevFrame f, DevHfParams p, cons
 // Same contract, one thread per stream (kernels/hf_lanes.cuh); `streams_per_cta` in {64, 128}.
 // `list` / `counts` come from launch_hf_block_list: per group (hf_block_list_count of them), its varblock origins in
 // raster order with their transform type and context offset, group_dim_blocks^2 records apart, and their number.
+// A code with LZ77 (not in chroma-subsampled frames) needs `lz_windows`: num_jobs windows of `lz_window_len` entries
+// (hf_lz77_window_entries in launch_tables.h), stream i's at lz_windows + i * lz_window_len.
 size_t hf_block_list_count(DevFrame f, DevHfParams p);
 void launch_hf_block_list(DevFrame f, DevHfParams p, uint2* list, uint32_t* counts, cudaStream_t stream);
 void launch_decode_hf_lanes(const uint8_t* codestream, DevFrame f, DevHfParams p, const uint2* list, const uint32_t* counts,
                             const DevHfJob* jobs, uint64_t* end_bits, int* status, int num_jobs, int first_pass,
-                            int streams_per_cta, cudaStream_t stream);
+                            int streams_per_cta, cudaStream_t stream, uint32_t* lz_windows = nullptr,
+                            uint32_t lz_window_len = 0);
 
 struct DevLfDequantJob {
   DevLfGroupRect rect;

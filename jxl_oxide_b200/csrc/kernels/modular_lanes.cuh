@@ -209,11 +209,9 @@ struct FastWp {
 
 constexpr int kMaxPrev = 16;
 
-struct StreamState {
+struct StreamState : Lz77State {  // the LZ77 state (stream_common.cuh) and the stream's reader
   WordBitReader br;
   uint32_t ans_state;
-  uint32_t* window;  // LZ77 state (lib.rs:346-352)
-  uint32_t lz_to_copy, lz_copy_pos, lz_decoded;
   int err;
 };
 
@@ -222,50 +220,16 @@ struct StreamState {
 template <bool FAST>
 __device__ __forceinline__ uint32_t read_token_value(const CodeView& cv, const DevEntropyCode& code, StreamState& s,
                                                      uint32_t cluster, bool lz77, uint32_t dist_multiplier) {
-  if (FAST) {
+  if constexpr (FAST) {
     const uint32_t token = cv_read_symbol_ans(cv, s.ans_state, s.br, cluster);
     return cv_read_uint(s.br, cv.configs[cluster], token);
-  }
-  if (!lz77) {
-    const uint32_t token = cv_read_symbol(cv, s.ans_state, s.br, cluster);
-    return cv_read_uint(s.br, cv.configs[cluster], token);
-  }
-  uint32_t token_value;
-  if (s.lz_to_copy > 0) {
-    token_value = s.window[s.lz_copy_pos & 0xfffff];
-    ++s.lz_copy_pos;
-    --s.lz_to_copy;
   } else {
-    const uint32_t token = cv_read_symbol(cv, s.ans_state, s.br, cluster);
-    if (token >= code.lz77_min_symbol) {
-      if (s.lz_decoded == 0) {
-        s.err = kDevBadStream;
-        return 0;
-      }
-      const uint32_t nc = cv_read_uint(s.br, code.lz_len_conf, token - code.lz77_min_symbol);
-      s.lz_to_copy = nc + code.lz77_min_length;
-      const uint32_t dtoken = cv_read_symbol(cv, s.ans_state, s.br, code.lz_dist_cluster);
-      uint32_t distance = cv_read_uint(s.br, cv.configs[code.lz_dist_cluster], dtoken);
-      if (dist_multiplier == 0) {
-      } else if (distance < 120) {
-        const int32_t dd = int32_t(kDevSpecialDistances[distance][0]) +
-                           int32_t(dist_multiplier) * int32_t(kDevSpecialDistances[distance][1]);
-        distance = uint32_t(max(dd - 1, 0));
-      } else {
-        distance -= 120;
-      }
-      distance = min(min((1u << 20) - 1, distance) + 1, s.lz_decoded);
-      s.lz_copy_pos = s.lz_decoded - distance;
-      token_value = s.window[s.lz_copy_pos & 0xfffff];
-      ++s.lz_copy_pos;
-      --s.lz_to_copy;
-    } else {
-      token_value = cv_read_uint(s.br, cv.configs[cluster], token);
+    if (!lz77) {
+      const uint32_t token = cv_read_symbol(cv, s.ans_state, s.br, cluster);
+      return cv_read_uint(s.br, cv.configs[cluster], token);
     }
+    return lz77_read_value(cv, code, s, s.ans_state, s.br, cluster, dist_multiplier, s.err);
   }
-  s.window[s.lz_decoded & 0xfffff] = token_value;
-  ++s.lz_decoded;
-  return token_value;
 }
 
 // Predictors other than Gradient / SelfCorrecting / Zero (predictor.rs:74-126)

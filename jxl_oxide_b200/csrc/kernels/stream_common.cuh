@@ -1,8 +1,13 @@
 // Helpers shared by the two entropy-stream kernels (modular_stream.cu, entropy.cu): wrapping
-// integer arithmetic, the shared-memory view of an entropy code and the symbol / hybrid-uint
-// readers (crates/jxl-coding/src/{lib.rs:572-605, ans.rs:276-330, prefix.rs:335-357}).
+// integer arithmetic, the shared-memory view of an entropy code, the symbol / hybrid-uint
+// readers (crates/jxl-coding/src/{lib.rs:572-605, ans.rs:276-330, prefix.rs:335-357}) and the
+// LZ77 step (lib.rs:476-569).
 #pragma once
 #include "common.cuh"
+#ifndef __CUDACC__
+#include <cstdio>
+#include <cstdlib>
+#endif
 
 namespace jxlb {
 namespace {
@@ -84,6 +89,96 @@ __device__ __forceinline__ uint32_t cv_read_uint(BR& br, uint32_t cfg, uint32_t 
   uint32_t t = (token >> lsb) & ((1u << msb) - 1);
   t |= 1u << msb;
   return uint32_t((((uint64_t(t) << n) | rest) << lsb) | low);
+}
+
+// LZ77 state of one stream (lib.rs:346-352): the window of decoded values, the copy in progress and how many values the
+// stream has produced. The window is indexed with `& 0xfffff` like the reference's 2^20-entry ring; a smaller window is
+// enough for a stream that produces fewer values than it has entries (the index never wraps then). Host builds (the
+// emulations in tests/emu/) check every index against `window_len` when the owner set it (lz77_init) and count the
+// values taken from copies.
+struct Lz77State {
+  uint32_t* window;
+  uint32_t lz_to_copy, lz_copy_pos, lz_decoded;
+#ifndef __CUDACC__
+  size_t window_len = ~size_t(0);
+  uint64_t copied = 0;
+#endif
+};
+__device__ __forceinline__ void lz77_init(Lz77State& lz, uint32_t* window, size_t window_len) {
+  lz.window = window;
+  lz.lz_to_copy = lz.lz_copy_pos = lz.lz_decoded = 0;
+#ifndef __CUDACC__
+  lz.window_len = window_len;
+  lz.copied = 0;
+#else
+  (void)window_len;
+#endif
+}
+__device__ __forceinline__ uint32_t lz77_slot(const Lz77State& lz, uint32_t pos) {
+  const uint32_t i = pos & 0xfffff;
+#ifndef __CUDACC__
+  if (i >= lz.window_len) {
+    std::fprintf(stderr, "LZ77 window index %u outside a window of %zu entries\n", i, lz.window_len);
+    std::abort();
+  }
+#endif
+  return i;
+}
+
+// One value of read_varint_with_multiplier_clustered (lib.rs:476-569) for a code with LZ77 enabled: the next value of a
+// copy in progress, or a symbol of `cluster` -- a literal, or a length token that starts a copy (its distance follows in
+// the code's distance cluster). Sets `err` to kDevBadStream and returns 0 for a copy before any value or a length that
+// overflows (InvalidLz77Symbol); the caller stops the stream then.
+template <typename BR>
+__device__ __forceinline__ uint32_t lz77_read_value(const CodeView& cv, const DevEntropyCode& code, Lz77State& lz,
+                                                    uint32_t& ans_state, BR& br, uint32_t cluster, uint32_t dist_multiplier,
+                                                    int& err) {
+  uint32_t value;
+  if (lz.lz_to_copy > 0) {
+    value = lz.window[lz77_slot(lz, lz.lz_copy_pos)];
+    ++lz.lz_copy_pos;
+    --lz.lz_to_copy;
+#ifndef __CUDACC__
+    ++lz.copied;
+#endif
+  } else {
+    const uint32_t token = cv_read_symbol(cv, ans_state, br, cluster);
+    if (token >= code.lz77_min_symbol) {
+      if (lz.lz_decoded == 0) {
+        err = kDevBadStream;
+        return 0;
+      }
+      const uint32_t nc = cv_read_uint(br, code.lz_len_conf, token - code.lz77_min_symbol);
+      if (nc > 0xffffffffu - code.lz77_min_length) {
+        err = kDevBadStream;
+        return 0;
+      }
+      lz.lz_to_copy = nc + code.lz77_min_length;
+      const uint32_t dtoken = cv_read_symbol(cv, ans_state, br, code.lz_dist_cluster);
+      uint32_t distance = cv_read_uint(br, cv.configs[code.lz_dist_cluster], dtoken);
+      if (dist_multiplier == 0) {
+      } else if (distance < 120) {
+        const int32_t dd = int32_t(kDevSpecialDistances[distance][0]) +
+                           int32_t(dist_multiplier) * int32_t(kDevSpecialDistances[distance][1]);
+        distance = uint32_t(max(dd - 1, 0));
+      } else {
+        distance -= 120;
+      }
+      distance = min(min((1u << 20) - 1, distance) + 1, lz.lz_decoded);
+      lz.lz_copy_pos = lz.lz_decoded - distance;
+      value = lz.window[lz77_slot(lz, lz.lz_copy_pos)];
+      ++lz.lz_copy_pos;
+      --lz.lz_to_copy;
+#ifndef __CUDACC__
+      ++lz.copied;
+#endif
+    } else {
+      value = cv_read_uint(br, cv.configs[cluster], token);
+    }
+  }
+  lz.window[lz77_slot(lz, lz.lz_decoded)] = value;
+  ++lz.lz_decoded;
+  return value;
 }
 
 // cooperative copy global -> shared by the 32 lanes of a warp (word granularity)

@@ -363,11 +363,15 @@ DevHfParams build_hf_params(const VarDctState& st, uint32_t pass, TableSink& sin
 
 HfSchedule hf_schedule(const DevHfParams& p, int streams_per_cta) {
   const bool cmaps_fit = 495u * p.num_block_clusters * p.num_hf_presets <= kLaneCmapSmemBytes;
-  if (!cmaps_fit || streams_per_cta > 64) return {true, 128};
+  if (p.code.lz77_enabled || !cmaps_fit || streams_per_cta > 64) return {true, 128};
   if (streams_per_cta == 64) return {true, 64};
   if (streams_per_cta >= 32) return {false, 32};
   if (streams_per_cta >= 16 || streams_per_cta == 0) return {false, 16};
   return {false, 8};
+}
+
+size_t hf_lz77_window_entries(uint32_t group_dim) {
+  return size_t(std::min<uint64_t>(uint64_t(1) << 20, 3 * uint64_t(group_dim) * group_dim));
 }
 
 std::vector<uint32_t> hf_launch_order(const std::vector<HfGroupJob>& jobs, bool longest_first) {

@@ -59,8 +59,14 @@ struct HfSchedule {
   int per_cta;
 };
 // `streams_per_cta` is the decoder's setting (jxlb_set_hf_streams_per_cta): 0 (one warp per stream, 16 per CTA), 4 (the
-// same as 8), 8, 16, 32, 64 or 128. Cluster maps larger than kLaneCmapSmemBytes always run one thread per stream, 128 per CTA.
+// same as 8), 8, 16, 32, 64 or 128. Cluster maps larger than kLaneCmapSmemBytes and codes with LZ77 always run one thread
+// per stream, 128 per CTA.
 HfSchedule hf_schedule(const DevHfParams& p, int streams_per_cta);
+// Entries of one HF stream's LZ77 window for groups of `group_dim` pixels: min(2^20, 3 * group_dim^2). A stream reads one
+// value per varblock channel (its non-zero count) plus at most 63 coefficients per 8x8 block of it, so at most
+// group_dim^2 values per channel; below 2^20 entries the window's `& 0xfffff` index never wraps, and at group_dim 1024
+// the window is the reference's 2^20-entry ring.
+size_t hf_lz77_window_entries(uint32_t group_dim);
 // Launch order of the HF streams as indices into `jobs`. longest_first (the thread-per-stream kernel): longest section
 // first, so that streams of similar length share a warp.
 std::vector<uint32_t> hf_launch_order(const std::vector<HfGroupJob>& jobs, bool longest_first);

@@ -17,6 +17,8 @@
 // group (at most 256 x 256, down to 1 x 1) is written with a single TOC entry. --no-gaborish turns Gaborish off;
 // --modular-filters SIGMA gives a --modular frame Gaborish and --epf-iters EPF iterations with constant sigma SIGMA.
 // --sharpness-cell N makes the sharpness map (and so the EPF sigma grid) change every N blocks instead of 16.
+// --hf-lz77 rle|match codes the HF passes with LZ77 (HfLz77 below); everything else is written as without it, and the
+// number of values the decoder takes from copies goes to stderr.
 //
 // Not part of the product; not a general-purpose encoder (it does not transform an input image).
 #include <algorithm>
@@ -90,10 +92,18 @@ struct Token {
   uint32_t ctx, value;
 };
 
+// A symbol as the entropy coder writes it: its context, its token and the extra bits of its hybrid-uint tail.
+struct Sym {
+  uint32_t ctx, tok, nbits, bits;
+};
+
+struct UintConfig {
+  uint32_t split_exp, msb, lsb;
+};
 // HybridUintConfig (4, 2, 0): the configuration libjxl uses for these streams
 const uint32_t kSplitExp = 4, kMsb = 2, kLsb = 0;
-void tokenize(uint32_t v, uint32_t* token, uint32_t* nbits, uint32_t* bits) {
-  const uint32_t split = 1u << kSplitExp;
+void tokenize_with(const UintConfig& c, uint32_t v, uint32_t* token, uint32_t* nbits, uint32_t* bits) {
+  const uint32_t split = 1u << c.split_exp;
   if (v < split) {
     *token = v;
     *nbits = 0;
@@ -102,10 +112,28 @@ void tokenize(uint32_t v, uint32_t* token, uint32_t* nbits, uint32_t* bits) {
   }
   uint32_t n = 31 - uint32_t(__builtin_clz(v));
   uint32_t m = v - (1u << n);
-  *token = split + ((n - kSplitExp) << (kMsb + kLsb)) + ((m >> (n - kMsb)) << kLsb) + (m & ((1u << kLsb) - 1));
-  *nbits = n - kMsb - kLsb;
-  *bits = (m >> kLsb) & ((1u << *nbits) - 1);
+  *token = split + ((n - c.split_exp) << (c.msb + c.lsb)) + ((m >> (n - c.msb)) << c.lsb) + (m & ((1u << c.lsb) - 1));
+  *nbits = n - c.msb - c.lsb;
+  *bits = (m >> c.lsb) & ((1u << *nbits) - 1);
 }
+void tokenize(uint32_t v, uint32_t* token, uint32_t* nbits, uint32_t* bits) {
+  tokenize_with({kSplitExp, kMsb, kLsb}, v, token, nbits, bits);
+}
+std::vector<Sym> to_syms(const std::vector<Token>& tokens) {
+  std::vector<Sym> s(tokens.size());
+  for (size_t i = 0; i < tokens.size(); ++i) {
+    s[i].ctx = tokens[i].ctx;
+    tokenize(tokens[i].value, &s[i].tok, &s[i].nbits, &s[i].bits);
+  }
+  return s;
+}
+
+// LZ77 parameters of an entropy code (lib.rs:321-343) with the U32 selectors they are written with.
+struct Lz77Header {
+  uint32_t min_symbol, min_length;
+  int symbol_sel, length_sel;  // min_symbol: 224, 512, 4096, 8 + u(15); min_length: 3, 4, 5 + u(2), 9 + u(8)
+  UintConfig len_cfg;
+};
 
 uint32_t add_log2_ceil(uint32_t x) { return ceil_log2_nonzero(x + 1); }
 
@@ -212,33 +240,48 @@ void write_ans_histogram(BitWriter& w, const std::vector<uint32_t>& counts) {
 }
 
 // Writes the entropy-code header for `tokens` (clustered by `cluster_of_ctx`) and then the ANS
-// stream itself (32-bit initial state first).
+// stream itself (32-bit initial state first). With `lz` set the code has LZ77 enabled: the symbols then hold
+// literals, length tokens (min_symbol and up) and distances, and the last context of the map is the distance context.
 struct EntropyEncoder {
   uint32_t num_ctx = 0, num_clusters = 0, log_alpha = 0;
   std::vector<uint8_t> cluster_of_ctx;
   std::vector<std::vector<uint32_t>> counts;     // per cluster, normalised
   std::vector<std::vector<std::vector<uint16_t>>> inv;  // cluster -> symbol -> offset -> idx
+  const Lz77Header* lz = nullptr;
 
   void write_header(BitWriter& w, const std::vector<Token>& tokens, uint32_t num_ctx_, const std::vector<uint8_t>& map) {
+    write_header_syms(w, to_syms(tokens), num_ctx_, map);
+  }
+  // `num_ctx_` counts the distance context of an LZ77 code.
+  void write_header_syms(BitWriter& w, const std::vector<Sym>& syms, uint32_t num_ctx_, const std::vector<uint8_t>& map) {
     num_ctx = num_ctx_;
     cluster_of_ctx = map;
     num_clusters = 0;
     for (uint8_t c : map) num_clusters = std::max<uint32_t>(num_clusters, c + 1u);
     std::vector<std::vector<uint64_t>> freq(num_clusters);
     uint32_t max_tok = 0;
-    for (const Token& t : tokens) {
-      uint32_t tok, nb, b;
-      tokenize(t.value, &tok, &nb, &b);
-      auto& f = freq[map[t.ctx]];
-      if (f.size() <= tok) f.resize(tok + 1, 0);
-      ++f[tok];
-      max_tok = std::max(max_tok, tok);
+    for (const Sym& s : syms) {
+      auto& f = freq[map[s.ctx]];
+      if (f.size() <= s.tok) f.resize(s.tok + 1, 0);
+      ++f[s.tok];
+      max_tok = std::max(max_tok, s.tok);
     }
     log_alpha = 5;
     while ((1u << log_alpha) <= max_tok) ++log_alpha;
     if (log_alpha > 8) fprintf(stderr, "token alphabet too large\n"), exit(1);
     BitWriter hw;
-    hw.write(1, 0);  // lz77 disabled
+    hw.write(1, lz ? 1 : 0);  // lz77
+    if (lz) {  // lib.rs:321-343
+      const uint32_t sym_bits[4] = {0, 0, 0, 15}, sym_base[4] = {224, 512, 4096, 8};
+      const uint32_t len_bits[4] = {0, 0, 2, 8}, len_base[4] = {3, 4, 5, 9};
+      write_u32(hw, lz->symbol_sel, int(sym_bits[lz->symbol_sel]), lz->min_symbol - sym_base[lz->symbol_sel]);
+      write_u32(hw, lz->length_sel, int(len_bits[lz->length_sel]), lz->min_length - len_base[lz->length_sel]);
+      hw.write(int(add_log2_ceil(8)), lz->len_cfg.split_exp);  // IntegerConfig with log_alphabet_size 8
+      if (lz->len_cfg.split_exp != 8) {
+        hw.write(int(add_log2_ceil(lz->len_cfg.split_exp)), lz->len_cfg.msb);
+        hw.write(int(add_log2_ceil(lz->len_cfg.split_exp - lz->len_cfg.msb)), lz->len_cfg.lsb);
+      }
+    }
     // cluster map (lib.rs:688-749)
     if (num_ctx > 1) {
       if (num_clusters <= 8) {
@@ -272,8 +315,12 @@ struct EntropyEncoder {
     hw.pad();
     // read it back with the decoder's parser to get the exact alias tables
     BitReader br(hw.bytes.data(), hw.bytes.size());
-    EntropyCode code = parse_entropy_code(br, num_ctx);
+    EntropyCode code = parse_entropy_code(br, num_ctx - (lz ? 1 : 0));
     if (code.num_clusters != num_clusters || code.log_alphabet_size != log_alpha) fprintf(stderr, "header readback mismatch\n"), exit(1);
+    if (lz && (!code.lz77_enabled || code.lz77_min_symbol != lz->min_symbol || code.lz77_min_length != lz->min_length ||
+               code.lz_len_conf.split_exponent != lz->len_cfg.split_exp || code.lz_len_conf.msb_in_token != lz->len_cfg.msb ||
+               code.lz_len_conf.lsb_in_token != lz->len_cfg.lsb || code.lz_dist_cluster() != map.back()))
+      fprintf(stderr, "LZ77 header readback mismatch\n"), exit(1);
     inv.assign(num_clusters, {});
     const uint32_t log_bucket = 12 - log_alpha;
     for (uint32_t c = 0; c < num_clusters; ++c) {
@@ -300,23 +347,23 @@ struct EntropyEncoder {
     }
   }
 
-  void write_tokens(BitWriter& w, const std::vector<Token>& tokens) const {
+  void write_tokens(BitWriter& w, const std::vector<Token>& tokens) const { write_syms(w, to_syms(tokens)); }
+  void write_syms(BitWriter& w, const std::vector<Sym>& syms) const {
     struct Out {
       uint16_t ans_bits;
       uint8_t has_ans;
       uint8_t nbits;
       uint32_t bits;
     };
-    std::vector<Out> outs(tokens.size());
+    std::vector<Out> outs(syms.size());
     uint32_t state = 0x130000;
-    for (size_t k = tokens.size(); k-- > 0;) {
-      uint32_t tok, nb, b;
-      tokenize(tokens[k].value, &tok, &nb, &b);
-      uint32_t c = cluster_of_ctx[tokens[k].ctx];
+    for (size_t k = syms.size(); k-- > 0;) {
+      const uint32_t tok = syms[k].tok;
+      uint32_t c = cluster_of_ctx[syms[k].ctx];
       uint32_t f = counts[c][tok];
       Out& o = outs[k];
-      o.nbits = uint8_t(nb);
-      o.bits = b;
+      o.nbits = uint8_t(syms[k].nbits);
+      o.bits = syms[k].bits;
       o.has_ans = 0;
       if ((state >> 20) >= f) {
         o.has_ans = 1;
@@ -332,6 +379,132 @@ struct EntropyEncoder {
     }
   }
 };
+
+// --hf-lz77: the LZ77 codes of the HF passes and how one HF stream is parsed into literals and copies. The decoder reads
+// every value of an HF stream -- non-zero counts and coefficients alike -- through read_varint_with_multiplier_clustered
+// with distance multiplier 0 (hf_coeff.rs:181-222): a length token is coded in the context of the first value it
+// replaces, its distance value D in the distance context, and the copy starts min(min(2^20 - 1, D) + 1, values so far)
+// values back. Copies run through whatever the values mean: block, channel and non-zero-count boundaries.
+//   rle:   libjxl's RLE form: min_symbol 224, min_length 3, distance value 0 (repeat the previous value).
+//   match: greedy matches at any distance (hash chains over four values), overlapping ones included; min_symbol
+//          8 + u(15) = 128, min_length 4. A match from the stream's first value is written with a distance beyond the
+//          values decoded so far, which the decoder clamps; the stream's last copy runs past its end (a copy still
+//          pending when the stream ends is ignored).
+//   bad-first / bad-length: `match`, with group 0's stream made invalid -- it starts with a copy, or its first copy has
+//          a length whose value plus min_length does not fit 32 bits.
+struct HfLz77 {
+  std::string mode;  // empty: no LZ77
+  Lz77Header header() const {
+    if (mode == "rle") return {224, 3, 0, 0, {0, 0, 0}};
+    return {128, 4, 3, 1, {kSplitExp, kMsb, kLsb}};
+  }
+};
+struct Lz77Counts {
+  uint64_t copied = 0, from_start = 0;
+};
+
+std::vector<Sym> lz77_parse(const std::vector<Token>& toks, const HfLz77& opt, uint32_t dist_ctx, bool corrupt,
+                            Lz77Counts* counts) {
+  const Lz77Header h = opt.header();
+  const size_t n = toks.size();
+  struct Item {
+    size_t pos;
+    bool copy;
+    uint32_t len_value, dist_value;  // copy: length - min_length, D
+  };
+  std::vector<Item> items;
+  auto v = [&](size_t i) { return toks[i].value; };
+  uint64_t copied = 0, from_start = 0;
+  if (opt.mode == "rle") {
+    for (size_t i = 0; i < n;) {
+      size_t r = 0;
+      if (i > 0)
+        while (i + r < n && v(i + r) == v(i - 1)) ++r;
+      if (r >= h.min_length) {
+        items.push_back({i, true, uint32_t(r - h.min_length), 0});
+        copied += r;
+        i += r;
+      } else {
+        items.push_back({i, false, 0, 0});
+        ++i;
+      }
+    }
+  } else {
+    const uint32_t kHashBits = 16;
+    std::vector<int32_t> head(size_t(1) << kHashBits, -1), prev(n, -1);
+    auto hash = [&](size_t i) {
+      const uint32_t x = v(i) * 0x9E3779B1u ^ v(i + 1) * 0x85EBCA77u ^ v(i + 2) * 0xC2B2AE3Du ^ v(i + 3) * 0x27D4EB2Fu;
+      return (x * 0x9E3779B1u) >> (32 - kHashBits);
+    };
+    auto insert = [&](size_t i) {
+      if (i + 4 > n) return;
+      const uint32_t k = hash(i);
+      prev[i] = head[k];
+      head[k] = int32_t(i);
+    };
+    auto match_len = [&](size_t j, size_t i) {
+      size_t l = 0;
+      while (i + l < n && l < 65536 && v(j + l) == v(i + l)) ++l;
+      return l;
+    };
+    for (size_t i = 0; i < n;) {
+      size_t best = 0, best_j = 0;
+      if (i > 0 && i + 4 <= n) {
+        int tries = 0;
+        for (int32_t j = head[hash(i)]; j >= 0 && tries < 32; j = prev[size_t(j)], ++tries) {
+          const size_t l = match_len(size_t(j), i);
+          if (l > best) best = l, best_j = size_t(j);
+        }
+        const size_t l0 = match_len(0, i);  // ties go to the stream's first value
+        if (l0 >= best && l0 > 0) best = l0, best_j = 0;
+      }
+      if (best >= h.min_length) {
+        uint32_t d = uint32_t(i - best_j - 1);
+        if (best_j == 0) d = (from_start++ & 1) ? uint32_t(i) + 1000 : (1u << 20) + 17;  // clamped to i by the decoder
+        items.push_back({i, true, uint32_t(best - h.min_length), d});
+        copied += best;
+        for (size_t k = i; k < i + best; ++k) insert(k);
+        i += best;
+      } else {
+        items.push_back({i, false, 0, 0});
+        insert(i);
+        ++i;
+      }
+    }
+    // the last copy runs past the end of the stream
+    if (!items.empty() && items.back().copy) {
+      items.back().len_value += 5;
+    } else if (n >= 2) {
+      for (size_t j = n - 1; j-- > 0;)
+        if (v(j) == v(n - 1)) {
+          items.back() = {n - 1, true, 2, uint32_t(n - 2 - j)};
+          ++copied;
+          break;
+        }
+    }
+    if (corrupt && opt.mode == "bad-first") items.insert(items.begin(), Item{0, true, 0, 0});
+    if (corrupt && opt.mode == "bad-length" && n >= 2)
+      items.insert(items.begin() + 1, Item{items[1].pos, true, 0xffffffffu - h.min_length + 1, 0});
+  }
+  std::vector<Sym> out;
+  for (const Item& it : items) {
+    Sym s{toks[it.pos].ctx, 0, 0, 0};
+    if (!it.copy) {
+      tokenize(v(it.pos), &s.tok, &s.nbits, &s.bits);
+      out.push_back(s);
+      continue;
+    }
+    tokenize_with(h.len_cfg, it.len_value, &s.tok, &s.nbits, &s.bits);
+    s.tok += h.min_symbol;
+    out.push_back(s);
+    Sym d{dist_ctx, 0, 0, 0};
+    tokenize(it.dist_value, &d.tok, &d.nbits, &d.bits);
+    out.push_back(d);
+  }
+  counts->copied += copied;
+  counts->from_start += from_start;
+  return out;
+}
 
 uint32_t pack_signed(int32_t v) { return v >= 0 ? uint32_t(v) << 1 : ((uint32_t(-(v + 1)) << 1) | 1); }
 
@@ -605,6 +778,7 @@ struct Args {
   bool all_types = false;  // every one of the 27 transform types in the frame (forced_layout), the rest drawn from all 27
   int only_type = -1;      // tile every group with this transform type wherever it fits, DCT8 elsewhere
   std::string dump_blocks; // write the varblock layout as text lines "x y type" (8x8 cells) in the order HfMetadata codes them
+  HfLz77 hf_lz77;          // --hf-lz77 rle | match | bad-first | bad-length: LZ77 in the HF pass codes (see HfLz77)
 };
 
 // Varblocks placed before the random layout is drawn (--all-types / --only-type): the transform type at each block's
@@ -1010,9 +1184,13 @@ int main(int argc, char** argv) {
     else if (s == "--all-types") a.all_types = true;
     else if (s == "--only-type") a.only_type = atoi(next().c_str());
     else if (s == "--dump-blocks") a.dump_blocks = next();
+    else if (s == "--hf-lz77") a.hf_lz77.mode = next();
     else if (s == "-o") a.out = next();
     else fprintf(stderr, "unknown arg %s\n", s.c_str()), exit(2);
   }
+  const std::string& lzm = a.hf_lz77.mode;
+  if (!lzm.empty() && (a.modular || (lzm != "rle" && lzm != "match" && lzm != "bad-first" && lzm != "bad-length")))
+    fprintf(stderr, "--hf-lz77 takes rle, match, bad-first or bad-length (VarDCT frames only)\n"), exit(2);
   if (a.modular) return encode_modular(a);
   if (a.only_type >= int(kNumTransformTypes) || (a.only_type >= 0 && a.all_types))
     fprintf(stderr, "--only-type takes a transform type 0..26 (not with --all-types)\n"), exit(2);
@@ -1254,6 +1432,22 @@ int main(int argc, char** argv) {
       const auto& t = hf_tokens[size_t(pass) * num_groups + g];
       hf_all[pass].insert(hf_all[pass].end(), t.begin(), t.end());
     }
+  // --hf-lz77: the same values, parsed into literals and copies; the distance context gets a cluster of its own
+  const Lz77Header lz_header = a.hf_lz77.header();
+  const uint32_t hf_num_ctx = 495 * nbc * NP;
+  std::vector<std::vector<Sym>> hf_syms(a.hf_lz77.mode.empty() ? 0 : size_t(P) * num_groups), hf_syms_all(P);
+  if (!a.hf_lz77.mode.empty()) {
+    Lz77Counts lzc;
+    for (uint32_t pass = 0; pass < P; ++pass)
+      for (uint32_t g = 0; g < num_groups; ++g) {
+        std::vector<Sym>& s = hf_syms[size_t(pass) * num_groups + g];
+        s = lz77_parse(hf_tokens[size_t(pass) * num_groups + g], a.hf_lz77, hf_num_ctx, pass == 0 && g == 0, &lzc);
+        hf_syms_all[pass].insert(hf_syms_all[pass].end(), s.begin(), s.end());
+      }
+    hf_map.push_back(uint8_t(*std::max_element(hf_map.begin(), hf_map.end()) + 1));
+    fprintf(stderr, "hf-lz77 %s: %llu values copied, %llu copies from the first value\n", a.hf_lz77.mode.c_str(),
+            (unsigned long long)lzc.copied, (unsigned long long)lzc.from_start);
+  }
 
   // ---- sections ----
   const uint32_t global_scale = uint32_t(std::lround(5111.0 / std::max(0.1, a.distance))), quant_lf = 17;
@@ -1298,7 +1492,12 @@ int main(int argc, char** argv) {
     w.write(int(ceil_log2_nonzero(num_groups)), NP - 1);  // num_hf_presets - 1
     for (uint32_t pass = 0; pass < P; ++pass) {
       write_u32(w, 2, 0, 0);  // used_orders = 0
-      hf_enc[pass].write_header(w, hf_all[pass], 495 * nbc * NP, hf_map);
+      if (a.hf_lz77.mode.empty()) {
+        hf_enc[pass].write_header(w, hf_all[pass], hf_num_ctx, hf_map);
+      } else {
+        hf_enc[pass].lz = &lz_header;
+        hf_enc[pass].write_header_syms(w, hf_syms_all[pass], hf_num_ctx + 1, hf_map);
+      }
     }
     end_section(w);
   }
@@ -1306,7 +1505,8 @@ int main(int argc, char** argv) {
     for (uint32_t g = 0; g < num_groups; ++g) {
       BitWriter& w = sections[2 + num_lf + size_t(pass) * num_groups + g];
       w.write(int(ceil_log2_nonzero(NP)), g % NP);  // hfp: 0 bits with a single preset
-      hf_enc[pass].write_tokens(w, hf_tokens[size_t(pass) * num_groups + g]);
+      if (a.hf_lz77.mode.empty()) hf_enc[pass].write_tokens(w, hf_tokens[size_t(pass) * num_groups + g]);
+      else hf_enc[pass].write_syms(w, hf_syms[size_t(pass) * num_groups + g]);
       end_section(w);
     }
 
