@@ -126,12 +126,17 @@ int32_t jxlb_set_capture(jxlb_decoder* dec, int32_t on);
 int32_t jxlb_set_fuse_filters(jxlb_decoder* dec, int32_t on);
 /* Scheduling of the HF coefficient streams (one per 256x256 group and pass, jxl-frame/src/data/pass_group.rs:31): how
  * many streams share one CTA and its staged tables. 0 (default, = 16), 4 (= 8), 8, 16, 32: one warp per stream, all
- * presets' tables staged once per CTA - the shortest time for ONE frame; 64 / 128: one thread per stream (32 streams
- * per warp): slower for a frame alone, but 16 warps instead of 510, which is what a GPU full of frames wants
+ * presets' tables staged once per CTA - the shortest time for ONE frame; 64 / 128: one thread per stream (several streams
+ * per warp, jxlb_set_hf_streams_per_warp): slower for a frame alone, but 4 CTAs instead of 32, which is what a GPU full of frames wants
  * (jxlb_pipeline_create's default). Frames whose HF presets' cluster maps together exceed 32 KB, and passes whose HF code
  * uses LZ77, always run one thread per stream, 128 per CTA. Results are identical; the process-wide default comes from the
  * environment variable JXLB_HF_LANES. */
 int32_t jxlb_set_hf_streams_per_cta(jxlb_decoder* dec, int32_t streams);
+/* How many of a CTA's thread-per-stream HF streams share one warp: 0 (default), 4, 8, 16 or 32. A CTA of S streams
+ * (jxlb_set_hf_streams_per_cta: 64 or 128) then runs S * 32 / k threads, and lane l < k of warp w decodes stream
+ * w * k + l: fewer streams per warp mean more warps per SM scheduler, each diverging across fewer streams, for the same
+ * CTAs and shared memory. No effect on the one-warp-per-stream schedules. Results are identical. */
+int32_t jxlb_set_hf_streams_per_warp(jxlb_decoder* dec, int32_t streams);
 int32_t jxlb_stage_count(const jxlb_decoder* dec, const char* name);
 int32_t jxlb_stage_get(const jxlb_decoder* dec, const char* name, int32_t idx, uint32_t* width, uint32_t* height,
                        uint32_t* out /* may be NULL */);

@@ -30,7 +30,7 @@ EXPORTED_SYMBOLS = [
     "jxlb_image_get_info", "jxlb_image_original_icc",
     "jxlb_num_frames", "jxlb_frame_get_info", "jxlb_frame_channel_to_host", "jxlb_frame_stream_channels", "jxlb_frame_write_to_buffer", "jxlb_frame_write_to_device", "jxlb_frame_channel_device",
     "jxlb_release_frames", "jxlb_sync", "jxlb_launch_count", "jxlb_set_profile", "jxlb_profile_get",
-    "jxlb_profile_reset", "jxlb_timeline_get", "jxlb_set_capture", "jxlb_set_fuse_filters", "jxlb_set_hf_streams_per_cta", "jxlb_stage_count", "jxlb_stage_get",
+    "jxlb_profile_reset", "jxlb_timeline_get", "jxlb_set_capture", "jxlb_set_fuse_filters", "jxlb_set_hf_streams_per_cta", "jxlb_set_hf_streams_per_warp", "jxlb_stage_count", "jxlb_stage_get",
     "jxlb_gaborish", "jxlb_epf", "jxlb_xyb_to_rgb", "jxlb_squeeze_inverse", "jxlb_rct_inverse", "jxlb_blend",
     "jxlb_pipeline_create", "jxlb_pipeline_destroy", "jxlb_pipeline_last_error", "jxlb_pipeline_preload", "jxlb_pipeline_submit",
     "jxlb_pipeline_wait", "jxlb_pipeline_release_output", "jxlb_pipeline_launch_count", "jxlb_pipeline_workers", "jxlb_pipeline_decoder",
@@ -127,6 +127,7 @@ def load_library():
     L.jxlb_set_capture.argtypes = [vp, i32]
     L.jxlb_set_fuse_filters.argtypes = [vp, i32]
     L.jxlb_set_hf_streams_per_cta.argtypes = [vp, i32]
+    L.jxlb_set_hf_streams_per_warp.argtypes = [vp, i32]
     L.jxlb_set_profile.argtypes = [vp, i32]
     L.jxlb_profile_get.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(ctypes.c_double)]
     L.jxlb_profile_reset.argtypes = [vp]
@@ -364,6 +365,11 @@ class Decoder:
         """HF streams per CTA: 0 (default, = 16), 4 (= 8), 8, 16, 32: one warp per stream; 64 / 128: one thread per stream."""
         if self._L.jxlb_set_hf_streams_per_cta(self._h, int(streams)) != 0:
             raise ValueError("streams per CTA must be 0, 4, 8, 16, 32, 64 or 128")
+
+    def set_hf_streams_per_warp(self, streams):
+        """Thread-per-stream HF schedules: streams per warp, 0 (default), 4, 8, 16 or 32 (jxlb_set_hf_streams_per_warp)."""
+        if self._L.jxlb_set_hf_streams_per_warp(self._h, int(streams)) != 0:
+            raise ValueError("streams per warp must be 0, 4, 8, 16 or 32")
 
     def stage(self, name, dtype=np.float32):
         n = self._L.jxlb_stage_count(self._h, name.encode())

@@ -510,6 +510,12 @@ int32_t jxlb_set_hf_streams_per_cta(jxlb_decoder* dec, int32_t streams) {
   return JXLB_OK;
 }
 
+int32_t jxlb_set_hf_streams_per_warp(jxlb_decoder* dec, int32_t streams) {
+  if (!dec || (streams != 0 && streams != 4 && streams != 8 && streams != 16 && streams != 32)) return JXLB_ERR_INVALID_ARG;
+  dec->be->hf_streams_per_warp = streams;
+  return JXLB_OK;
+}
+
 int32_t jxlb_stage_count(const jxlb_decoder* dec, const char* name) {
   if (!dec || !name) return 0;
   auto it = dec->be->stages.find(name);

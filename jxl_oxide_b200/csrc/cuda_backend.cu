@@ -766,7 +766,7 @@ void CudaBackend::decode_hf(VarDctState& st, std::vector<HfGroupJob>& jobs) {
   JXLB_CHECK(!(hf_lz77 && st.subsampled), kErrUnsupported,
              "LZ77 in the HF coefficient streams of a chroma-subsampled frame is not supported on the device");
   const DevHfParams p = build_hf_params(st, pass, *this, d_natural_orders_, natural_order_offset_);
-  const HfSchedule sched = hf_schedule(p, hf_streams_per_cta);
+  const HfSchedule sched = hf_schedule(p, hf_streams_per_cta, hf_streams_per_warp);
   const std::vector<uint32_t> perm = hf_launch_order(jobs, sched.lanes);  // launch order -> `jobs`
   std::vector<DevHfJob> dj;
   for (uint32_t i : perm) dj.push_back({jobs[i].bit_pos, jobs[i].bit_limit, jobs[i].group_idx});
@@ -794,7 +794,7 @@ void CudaBackend::decode_hf(VarDctState& st, std::vector<HfGroupJob>& jobs) {
   begin_k("decode_hf");
   if (sched.lanes)
     launch_decode_hf_lanes(active_cs_, dev_frame(st), p, d_list, d_counts, d_jobs, d_end, d_status, int(jobs.size()),
-                           pass == 0 ? 1 : 0, sched.per_cta, S(), d_lz, uint32_t(lz_len));
+                           pass == 0 ? 1 : 0, sched.per_cta, sched.per_warp, S(), d_lz, uint32_t(lz_len));
   else
     launch_decode_hf(active_cs_, dev_frame(st), p, d_jobs, d_end, d_status, int(jobs.size()), pass == 0 ? 1 : 0,
                      sched.per_cta, S());

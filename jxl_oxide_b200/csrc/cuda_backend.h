@@ -143,6 +143,8 @@ class CudaBackend : public Backend, private TableSink {
   bool fuse_filters = true;  // single-kernel Gaborish+EPF+colour (off: stage-by-stage, for stage parity tests)
   // HF coefficient streams per CTA (jxlb_set_hf_streams_per_cta, hf_schedule). Initialised from JXLB_HF_LANES.
   int hf_streams_per_cta = 0;
+  // streams per warp of the thread-per-stream HF kernel (jxlb_set_hf_streams_per_warp, hf_schedule); 0: the default
+  int hf_streams_per_warp = 0;
   bool profile = false;
   bool host_phases = false;  // wall clock per planner phase only (no CUDA events): where a frame's latency goes under load
   bool trace_device = false;  // modular streams stamp the device clock; host launch/return times are logged

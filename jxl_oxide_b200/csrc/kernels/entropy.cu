@@ -233,8 +233,10 @@ __global__ void __launch_bounds__(W * 32) decode_hf_warp_kernel(const uint8_t* _
 }
 
 // ---------------------------------------------------------------------------------------------
-// One thread per stream (hf_lanes.cuh). A CTA of `blockDim.x` threads carries blockDim.x streams and stages, once, the
-// tables of hf_lane_layout(). Its streams start from their groups' varblock lists (hf_block_list_kernel).
+// One thread per stream (hf_lanes.cuh). A CTA carries `per_cta` streams and stages, once, the tables of
+// hf_lane_layout(per_cta); its THREADS = per_cta * 32 / K threads all stage, and lane l < K of warp w then runs stream
+// slot w * K + l. Fewer streams per warp (K < 32) give each scheduler more warps that diverge across fewer streams,
+// for the same CTA count and shared memory. Its streams start from their groups' varblock lists (hf_block_list_kernel).
 
 // One CTA per group: the group's cells in raster order, 256 at a time, compacted with a ballot and a prefix over warps.
 template <bool SUB>
@@ -265,17 +267,19 @@ __global__ void __launch_bounds__(256) hf_block_list_kernel(DevFrame f, DevHfPar
 }
 
 // LZ77: stream `job_idx` keeps its values in lz_windows[job_idx * lz_window_len ...] (unused otherwise).
-template <bool SUB, bool STAGED, bool LZ77>
-__global__ void __launch_bounds__(128) decode_hf_lanes_kernel(const uint8_t* __restrict__ cs, DevFrame f, DevHfParams p,
-                                                              const uint2* __restrict__ list,
-                                                              const uint32_t* __restrict__ counts,
-                                                              const DevHfJob* __restrict__ jobs,
-                                                              uint64_t* __restrict__ end_bits, int* __restrict__ status,
-                                                              int num_jobs, int first_pass,
-                                                              uint32_t* lz_windows, uint32_t lz_window_len) {
+// The minimum-blocks hint caps every instantiation at 64 registers (65536 / 1024), as many as a 1024-thread CTA can
+// have: a CTA of more threads carries no more streams, so it should not take more of the SM's register file than it must.
+template <bool SUB, bool STAGED, bool LZ77, int THREADS>
+__global__ void __launch_bounds__(THREADS, 1024 / THREADS) decode_hf_lanes_kernel(const uint8_t* __restrict__ cs, DevFrame f, DevHfParams p,
+                                                                  const uint2* __restrict__ list,
+                                                                  const uint32_t* __restrict__ counts,
+                                                                  const DevHfJob* __restrict__ jobs,
+                                                                  uint64_t* __restrict__ end_bits, int* __restrict__ status,
+                                                                  int num_jobs, int first_pass, uint32_t per_cta,
+                                                                  uint32_t* lz_windows, uint32_t lz_window_len) {
   extern __shared__ __align__(16) uint8_t smem[];
   const uint32_t tid = threadIdx.x, nthreads = blockDim.x;
-  const HfLaneSmem L = hf_lane_layout(p, nthreads);
+  const HfLaneSmem L = hf_lane_layout(p, per_cta);
   uint8_t* s_ctx = smem + L.ctxlut;
   for (uint32_t i = tid; i < 63; i += nthreads) {
     s_ctx[i] = hftab::kCoeffFreqContext[i];
@@ -293,8 +297,10 @@ __global__ void __launch_bounds__(128) decode_hf_lanes_kernel(const uint8_t* __r
   T.order_offset = HfLds::addr(s_small + 27);
   T.ctx = HfLds::addr(s_ctx);
   T.bctx = HfLds::addr(s_bctx);
-  T.nz = HfLds::addr(smem + L.nz + tid);
-  T.nz_stride = nthreads;
+  const uint32_t k = per_cta * 32 / THREADS, lane = tid & 31;
+  const uint32_t slot = (tid >> 5) * k + lane;  // this thread's stream in the CTA, if lane < k
+  T.nz = HfLds::addr(smem + L.nz + slot);
+  T.nz_stride = per_cta;
   T.cmap_stride = L.cmap_stride;
   T.cmap = 0;
   T.cmap_ptr = p.code.cluster_map;
@@ -328,8 +334,8 @@ __global__ void __launch_bounds__(128) decode_hf_lanes_kernel(const uint8_t* __r
     T.cv.ans = reinterpret_cast<const uint64_t*>(s_ans);
   }
   __syncthreads();
-  const int job_idx = blockIdx.x * int(nthreads) + int(tid);
-  if (job_idx >= num_jobs) return;
+  const int job_idx = blockIdx.x * int(per_cta) + int(slot);
+  if (lane >= k || job_idx >= num_jobs) return;
   const DevHfJob job = jobs[job_idx];
   const uint32_t gb = p.group_dim_blocks;
   if constexpr (LZ77) {
@@ -356,26 +362,27 @@ void launch_hf_block_list(DevFrame f, DevHfParams p, uint2* list, uint32_t* coun
   else hf_block_list_kernel<false><<<groups, 256, 0, stream>>>(f, p, list, counts);
 }
 
-void launch_decode_hf_lanes(const uint8_t* cs, DevFrame f, DevHfParams p, const uint2* list, const uint32_t* counts,
-                            const DevHfJob* jobs, uint64_t* end_bits, int* status, int num_jobs, int first_pass,
-                            int streams_per_cta, cudaStream_t stream, uint32_t* lz_windows, uint32_t lz_window_len) {
-  if (num_jobs <= 0) return;
+namespace {
+template <int THREADS>
+void launch_hf_lanes(const uint8_t* cs, DevFrame f, DevHfParams p, const uint2* list, const uint32_t* counts,
+                     const DevHfJob* jobs, uint64_t* end_bits, int* status, int num_jobs, int first_pass, uint32_t per_cta,
+                     cudaStream_t stream, uint32_t* lz_windows, uint32_t lz_window_len) {
   // C++ function-local statics are initialised once, thread-safely: no worker thread launches before the limits are set
   static const bool attr_set = [] {
-    cudaFuncSetAttribute(decode_hf_lanes_kernel<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(decode_hf_lanes_kernel<true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(decode_hf_lanes_kernel<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(decode_hf_lanes_kernel<true, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(decode_hf_lanes_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    const int bytes = 200 * 1024;
+    cudaFuncSetAttribute(decode_hf_lanes_kernel<false, false, false, THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    cudaFuncSetAttribute(decode_hf_lanes_kernel<true, false, false, THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    cudaFuncSetAttribute(decode_hf_lanes_kernel<false, true, false, THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    cudaFuncSetAttribute(decode_hf_lanes_kernel<true, true, false, THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    cudaFuncSetAttribute(decode_hf_lanes_kernel<false, false, true, THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
     return true;
   }();
   (void)attr_set;
-  const int nthreads = streams_per_cta <= 64 ? 64 : 128;
-  const HfLaneSmem L = hf_lane_layout(p, uint32_t(nthreads));
-  const int ctas = (num_jobs + nthreads - 1) / nthreads;
+  const HfLaneSmem L = hf_lane_layout(p, per_cta);
+  const int ctas = (num_jobs + int(per_cta) - 1) / int(per_cta);
 #define JXLB_HF_LANES(SUB_, STAGED_, LZ77_)                                                                        \
-  decode_hf_lanes_kernel<SUB_, STAGED_, LZ77_><<<ctas, nthreads, L.total, stream>>>(                               \
-      cs, f, p, list, counts, jobs, end_bits, status, num_jobs, first_pass, lz_windows, lz_window_len)
+  decode_hf_lanes_kernel<SUB_, STAGED_, LZ77_, THREADS><<<ctas, THREADS, L.total, stream>>>(                       \
+      cs, f, p, list, counts, jobs, end_bits, status, num_jobs, first_pass, per_cta, lz_windows, lz_window_len)
   if (p.code.lz77_enabled) {  // the caller rejects chroma-subsampled frames with an LZ77 code
     JXLB_HF_LANES(false, false, true);
   } else if (hf_lane_staged(p, L)) {
@@ -386,6 +393,26 @@ void launch_decode_hf_lanes(const uint8_t* cs, DevFrame f, DevHfParams p, const 
     else JXLB_HF_LANES(false, false, false);
   }
 #undef JXLB_HF_LANES
+}
+}  // namespace
+
+void launch_decode_hf_lanes(const uint8_t* cs, DevFrame f, DevHfParams p, const uint2* list, const uint32_t* counts,
+                            const DevHfJob* jobs, uint64_t* end_bits, int* status, int num_jobs, int first_pass,
+                            int streams_per_cta, int streams_per_warp, cudaStream_t stream, uint32_t* lz_windows,
+                            uint32_t lz_window_len) {
+  if (num_jobs <= 0) return;
+  const uint32_t per_cta = streams_per_cta <= 64 ? 64 : 128;
+  const uint32_t k = streams_per_warp <= 4 ? 4 : (streams_per_warp <= 8 ? 8 : (streams_per_warp <= 16 ? 16 : 32));
+#define JXLB_HF_LANES_T(T_) \
+  launch_hf_lanes<T_>(cs, f, p, list, counts, jobs, end_bits, status, num_jobs, first_pass, per_cta, stream, lz_windows, lz_window_len)
+  switch (per_cta * 32 / k) {
+    case 64: JXLB_HF_LANES_T(64); break;
+    case 128: JXLB_HF_LANES_T(128); break;
+    case 256: JXLB_HF_LANES_T(256); break;
+    case 512: JXLB_HF_LANES_T(512); break;
+    default: JXLB_HF_LANES_T(1024); break;
+  }
+#undef JXLB_HF_LANES_T
 }
 
 namespace {

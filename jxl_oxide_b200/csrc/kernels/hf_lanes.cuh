@@ -2,7 +2,8 @@
 //
 // decode_hf_warp_kernel (entropy.cu) walks every stream from a single lane of its warp; with 510 streams
 // per 8K frame and 24 frames in flight the SM schedulers saturate on one-lane warps (DESIGN.md section 4).
-// Here a warp carries 32 independent streams. The chain of one stream is written as a flat state machine --
+// Here a warp carries up to 32 independent streams (streams per warp: launch_decode_hf_lanes). The chain of one stream is
+// written as a flat state machine --
 // every trip of the loop decodes exactly one symbol (a block's non-zero count or one coefficient) -- so the
 // lanes of a warp re-converge on the expensive part (alias-table ANS step + hybrid-uint read) no matter
 // where in their groups they are; only the short bookkeeping before / after the symbol diverges.
@@ -227,8 +228,8 @@ struct HfLaneView {
   Addr ctx;           // [0..63): coefficient frequency context, [64..127): non-zero-count context
   Addr bctx;          // block context map
   // Per-stream scratch: predicted non-zero counts of the row above, 3 channels x 32 block columns, one byte each (a
-  // count is at most 63) at `nz + (c * 32 + x) * nz_stride`: on the device the lanes of a CTA interleave
-  // (nz_stride = blockDim.x) so that a warp's accesses to one (c, x) fall into consecutive bytes.
+  // count is at most 63) at `nz + (c * 32 + x) * nz_stride`: on the device the streams of a CTA interleave
+  // (nz_stride = streams per CTA, in stream-slot order) so that a warp's accesses to one (c, x) fall into consecutive bytes.
   Addr nz;
   uint32_t nz_stride;
   Addr cmap;               // staged variant: cluster maps of all HF presets, `cmap_stride` bytes apart

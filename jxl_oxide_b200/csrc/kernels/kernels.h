@@ -174,7 +174,9 @@ constexpr uint32_t kLaneCmapSmemBytes = 32 * 1024;
 // One warp per stream, `warps_per_cta` (8, 16 or 32) streams per CTA sharing the staged tables.
 void launch_decode_hf(const uint8_t* codestream, DevFrame f, DevHfParams p, const DevHfJob* jobs, uint64_t* end_bits,
                       int* status, int num_jobs, int first_pass, int warps_per_cta, cudaStream_t stream);
-// Same contract, one thread per stream (kernels/hf_lanes.cuh); `streams_per_cta` in {64, 128}.
+// Same contract, one thread per stream (kernels/hf_lanes.cuh); `streams_per_cta` in {64, 128}, `streams_per_warp` in
+// {4, 8, 16, 32}: a CTA runs streams_per_cta * 32 / streams_per_warp threads, and the lanes past the first
+// streams_per_warp of each warp only help stage the tables.
 // `list` / `counts` come from launch_hf_block_list: per group (hf_block_list_count of them), its varblock origins in
 // raster order with their transform type and context offset, group_dim_blocks^2 records apart, and their number.
 // A code with LZ77 (not in chroma-subsampled frames) needs `lz_windows`: num_jobs windows of `lz_window_len` entries
@@ -183,7 +185,7 @@ size_t hf_block_list_count(DevFrame f, DevHfParams p);
 void launch_hf_block_list(DevFrame f, DevHfParams p, uint2* list, uint32_t* counts, cudaStream_t stream);
 void launch_decode_hf_lanes(const uint8_t* codestream, DevFrame f, DevHfParams p, const uint2* list, const uint32_t* counts,
                             const DevHfJob* jobs, uint64_t* end_bits, int* status, int num_jobs, int first_pass,
-                            int streams_per_cta, cudaStream_t stream, uint32_t* lz_windows = nullptr,
+                            int streams_per_cta, int streams_per_warp, cudaStream_t stream, uint32_t* lz_windows = nullptr,
                             uint32_t lz_window_len = 0);
 
 struct DevLfDequantJob {

@@ -361,13 +361,14 @@ DevHfParams build_hf_params(const VarDctState& st, uint32_t pass, TableSink& sin
   return p;
 }
 
-HfSchedule hf_schedule(const DevHfParams& p, int streams_per_cta) {
+HfSchedule hf_schedule(const DevHfParams& p, int streams_per_cta, int streams_per_warp) {
+  const int per_warp = streams_per_warp > 0 ? streams_per_warp : kHfStreamsPerWarpDefault;
   const bool cmaps_fit = 495u * p.num_block_clusters * p.num_hf_presets <= kLaneCmapSmemBytes;
-  if (p.code.lz77_enabled || !cmaps_fit || streams_per_cta > 64) return {true, 128};
-  if (streams_per_cta == 64) return {true, 64};
-  if (streams_per_cta >= 32) return {false, 32};
-  if (streams_per_cta >= 16 || streams_per_cta == 0) return {false, 16};
-  return {false, 8};
+  if (p.code.lz77_enabled || !cmaps_fit || streams_per_cta > 64) return {true, 128, per_warp};
+  if (streams_per_cta == 64) return {true, 64, per_warp};
+  if (streams_per_cta >= 32) return {false, 32, 1};
+  if (streams_per_cta >= 16 || streams_per_cta == 0) return {false, 16, 1};
+  return {false, 8, 1};
 }
 
 size_t hf_lz77_window_entries(uint32_t group_dim) {

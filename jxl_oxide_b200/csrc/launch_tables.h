@@ -53,15 +53,20 @@ std::vector<uint32_t> natural_order_table(uint32_t offset[13]);
 DevHfParams build_hf_params(const VarDctState& st, uint32_t pass, TableSink& sink, const uint32_t* natural_orders,
                             const uint32_t natural_offset[13]);
 // Which kernel decodes the HF streams of one pass, and how many streams share a CTA: one thread per stream
-// (launch_decode_hf_lanes, `per_cta` 64 or 128) or one warp per stream (launch_decode_hf, `per_cta` 8, 16 or 32).
+// (launch_decode_hf_lanes, `per_cta` 64 or 128, `per_warp` of them in each warp) or one warp per stream
+// (launch_decode_hf, `per_cta` 8, 16 or 32, `per_warp` 1).
 struct HfSchedule {
   bool lanes;
   int per_cta;
+  int per_warp;
 };
+// Streams per warp of the thread-per-stream kernel unless the decoder sets it (jxlb_set_hf_streams_per_warp).
+constexpr int kHfStreamsPerWarpDefault = 8;
 // `streams_per_cta` is the decoder's setting (jxlb_set_hf_streams_per_cta): 0 (one warp per stream, 16 per CTA), 4 (the
 // same as 8), 8, 16, 32, 64 or 128. Cluster maps larger than kLaneCmapSmemBytes and codes with LZ77 always run one thread
-// per stream, 128 per CTA.
-HfSchedule hf_schedule(const DevHfParams& p, int streams_per_cta);
+// per stream, 128 per CTA. `streams_per_warp` (jxlb_set_hf_streams_per_warp): 0 (kHfStreamsPerWarpDefault), 4, 8, 16 or
+// 32, for every thread-per-stream schedule.
+HfSchedule hf_schedule(const DevHfParams& p, int streams_per_cta, int streams_per_warp);
 // Entries of one HF stream's LZ77 window for groups of `group_dim` pixels: min(2^20, 3 * group_dim^2). A stream reads one
 // value per varblock channel (its non-zero count) plus at most 63 coefficients per 8x8 block of it, so at most
 // group_dim^2 values per channel; below 2^20 entries the window's `& 0xfffff` index never wraps, and at group_dim 1024

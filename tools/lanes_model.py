@@ -1,8 +1,9 @@
-"""SIMT model of the thread-per-stream HF kernel from its host emulation (tests/emu): how full the warps are and how
-often the divergent parts of a loop trip run. Usage: python tools/lanes_model.py [file.jxl ...] (default: the 8K
-synthetic bench frame and starrail.d1-e6)."""
+"""SIMT model of the thread-per-stream HF kernel from its host emulation (tests/emu, lanes_k.mk): for each number of streams per
+warp (K), how full the warps are and how often the divergent parts of a loop trip run. Usage:
+python tools/lanes_model.py [file.jxl ...] (default: the 8K synthetic bench frame and starrail.d1-e6)."""
 import ctypes
 import os
+import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -12,18 +13,33 @@ import bench  # noqa: E402
 import oracle_lib  # noqa: E402
 
 
+KS = (32, 16, 8, 4)
+EMU = os.path.join(ROOT, "tests", "emu")
+
+
+def lanes_k_lib():
+    """The HF lanes emulation with the SIMT model of every K (tests/emu/lanes_k.mk)."""
+    subprocess.check_call(["make", "-s", "-C", EMU, "-f", "lanes_k.mk"])
+    return oracle_lib._load(os.path.join(EMU, "_build", "libjxlemu_lanes_k.so"), None)
+
+
 def model(name, data):
-    L = oracle_lib.emu_lib()
+    L = lanes_k_lib()
+    oracle_lib.emu_lib = lambda: L  # OracleImage(..., emu=True) decodes with this build
     out = (ctypes.c_uint64 * 6)()
-    L.jxle_lane_stats(out, 1)
+    for k in KS:
+        L.jxle_lane_k_stats(k, out, 1)
     oracle_lib.OracleImage(data, threads=os.cpu_count() or 1, emu=True).close()
-    L.jxle_lane_stats(out, 1)
-    streams, symbols, warp_trips, hdr_trips, coef_trips, warps = [int(x) for x in out]
-    print(f"{name}: {streams} streams in {warps} warps, {symbols} symbols ({symbols / max(streams, 1):.0f} per stream)")
-    print(f"  warp trips {warp_trips} -> {symbols / max(warp_trips, 1):.1f} symbols per trip "
-          f"(lane efficiency {symbols / max(warp_trips * 32, 1):.2f}); one-lane-per-warp kernel: {symbols} trips")
-    print(f"  trips with a lane on a non-zero count (it may take its next varblock record): {hdr_trips / max(warp_trips, 1):.2f}, "
-          f"with a lane on a coefficient: {coef_trips / max(warp_trips, 1):.2f}")
+    for k in KS:
+        L.jxle_lane_k_stats(k, out, 1)
+        streams, symbols, warp_trips, hdr_trips, coef_trips, warps = [int(x) for x in out]
+        if k == KS[0]:
+            print(f"{name}: {streams} streams, {symbols} symbols ({symbols / max(streams, 1):.0f} per stream); "
+                  f"one-lane-per-warp kernel: {symbols} trips")
+        print(f"  K={k:2d}: {warps} warps, {warp_trips} warp trips -> {symbols / max(warp_trips, 1):.1f} symbols per trip "
+              f"(lane efficiency {symbols / max(warp_trips * k, 1):.2f}), {warp_trips / max(warps, 1):.0f} trips per warp; "
+              f"trips with a lane on a non-zero count {hdr_trips / max(warp_trips, 1):.2f}, "
+              f"on a coefficient {coef_trips / max(warp_trips, 1):.2f}")
 
 
 if __name__ == "__main__":
