@@ -246,8 +246,23 @@ LfGlobalSyntax parse_lf_global(BitReader& br, const ImageHeader& ih, const Frame
   g.has_global_tree = br.read_bool();
   if (g.has_global_tree) g.global_tree = parse_ma_tree(br, size_t(max_nodes));
   uint32_t cw = fh.color_sample_width(), ch = fh.color_sample_height();
-  if (fh.encoding == Encoding::kModular) {
-    JXLB_CHECK(!fh.do_ycbcr, kErrUnsupported, "YCbCr modular frames are outside the implemented hot path");
+  if (fh.encoding == Encoding::kModular && fh.do_ycbcr) {
+    // Cb, Y, Cr with ChannelShift::from_jpeg_upsampling and shift_size (jxl-modular/src/param.rs:105-165): in a
+    // direction where any channel is subsampled, a subsampled channel is ceil(n / 2) long and the others are rounded
+    // up to twice that
+    bool h_any = false, v_any = false;
+    for (uint32_t j : fh.jpeg_upsampling) {
+      h_any |= j == 1 || j == 2;
+      v_any |= j == 1 || j == 3;
+    }
+    for (int i = 0; i < 3; ++i) {
+      const uint32_t j = fh.jpeg_upsampling[i];
+      const bool hs = h_any && (j == 0 || j == 3), vs = v_any && (j == 0 || j == 2);
+      const uint32_t w = h_any ? (hs ? (cw + 1) / 2 : (cw + 1) / 2 * 2) : cw;
+      const uint32_t h = v_any ? (vs ? (ch + 1) / 2 : (ch + 1) / 2 * 2) : ch;
+      g.gmodular_image_channels.push_back({w, h, int32_t(hs), int32_t(vs)});
+    }
+  } else if (fh.encoding == Encoding::kModular) {
     for (uint32_t i = 0; i < fh.encoded_color_channels; ++i) g.gmodular_image_channels.push_back({cw, ch, 0, 0});
   }
   uint32_t color_shift = ceil_log2_nonzero(fh.upsampling);

@@ -258,6 +258,8 @@ class FramePlanner {
   void render_vardct(DecodedFrame* out);
   bool colour_params(bool is_xyb, size_t num_colour, ColorParams* p);
   void finish_colour(std::vector<View>& colour, bool is_xyb, bool already_converted, DecodedFrame* out);
+  // log2 of the factor that brings extra channel `i` from its coded size to the frame size (image.rs:487-557)
+  uint32_t ec_shift(size_t i) const { return ceil_log2_nonzero(fh_.ec_upsampling[i]) + ih_.ec_info[i].dim_shift; }
 
   Backend& be_;
   const uint8_t* cs_;
@@ -510,13 +512,11 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
     chan_vshift[c] = (j == 0 || j == 2) && v_subsampling;
   }
   const bool chroma_subsampled = h_subsampling || v_subsampling;
-  JXLB_CHECK(!chroma_subsampled || vardct, kErrUnsupported, "chroma-subsampled Modular frames are not implemented");
-  JXLB_CHECK(!chroma_subsampled || fh_.skip_adaptive_lf_smoothing(), kErrUnsupported, "adaptive LF smoothing of a chroma-subsampled frame");
+  JXLB_CHECK(!chroma_subsampled || !vardct || fh_.skip_adaptive_lf_smoothing(), kErrUnsupported,
+             "adaptive LF smoothing of a chroma-subsampled frame");
   // block counts are rounded up to even in a subsampled direction (hf_metadata.rs:70-80, vardct/mod.rs:83-95)
   auto blocks_w = [&](uint32_t px) { return h_subsampling ? ((px + 7) / 8 + 1) / 2 * 2 : (px + 7) / 8; };
   auto blocks_h = [&](uint32_t px) { return v_subsampling ? ((px + 7) / 8 + 1) / 2 * 2 : (px + 7) / 8; };
-  for (uint32_t u : fh_.ec_upsampling) JXLB_CHECK(u == fh_.upsampling, kErrUnsupported, "extra-channel upsampling differs from colour");
-  for (const auto& ec : ih_.ec_info) JXLB_CHECK(ec.dim_shift == 0, kErrUnsupported, "dim_shift extra channels not supported");
 
   const uint32_t num_lf_groups = fh_.num_lf_groups(), num_groups = fh_.num_groups();
   const uint32_t num_passes = fh_.passes.num_passes;
@@ -531,9 +531,19 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
     lfg_ = parse_lf_global(r, ih_, fh_);
     pos = r.pos();
   }
+  // With patches the reference brings an extra channel to the colour resolution first, blends, then upsamples it with
+  // the colour channels (render.rs:159-175, image.rs:487-557 with ec_to_color_only): a different chain, not restated.
+  for (size_t i = 0; i < ih_.ec_info.size(); ++i)
+    JXLB_CHECK(!lfg_.has_patches || ec_shift(i) == ceil_log2_nonzero(fh_.upsampling), kErrUnsupported,
+               "patches on a frame whose extra channel is upsampled apart from the colour channels are not implemented");
+  // full-size float planes of the extra channels upsampled here, each with at most a quarter-size chain intermediate
+  size_t ec_render_bytes = 0;
+  for (size_t i = 0; i < ih_.ec_info.size(); ++i)
+    if (ec_shift(i)) ec_render_bytes += size_t(fh_.width) * fh_.height * 4 + size_t(fh_.width) * fh_.height;
   if (lfg_.has_gmodular) {
     // a Modular image allocates its full-size channels up front (coded channels, then one plane per inverse transform)
-    if (!vardct) be_.begin_heavy_stage(size_t(cw) * chh * 4 * 2 * (lfg_.gmodular.channels.size() + 2) + (size_t(64) << 20));
+    if (!vardct)
+      be_.begin_heavy_stage(size_t(cw) * chh * 4 * 2 * (lfg_.gmodular.channels.size() + 2) + ec_render_bytes + (size_t(64) << 20));
     setup_gmodular();
     std::vector<ModularStreamJob> jobs(1);
     ModularStreamJob& job = jobs[0];
@@ -713,7 +723,7 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
   if (vardct) {
     // Everything so far worked on 1/64 of the samples; from here on the frame needs its full-resolution planes
     // (3 coefficient planes that become the pixels in place + 3 planes of filter output).
-    be_.begin_heavy_stage(size_t(st_.bw) * st_.bh * 64 * 4 * 6 + (size_t(64) << 20));
+    be_.begin_heavy_stage(size_t(st_.bw) * st_.bh * 64 * 4 * 6 + ec_render_bytes + (size_t(64) << 20));
     be_.phase_mark("heavy_wait");
     for (int c = 0; c < 3; ++c) st_.coeff[c] = new_plane(st_.bw * 8, st_.bh * 8, /*zero=*/true);
   }
@@ -790,6 +800,20 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
     } else {
       for (View& v : colour) be_.int_to_float(v, ih_.bit_depth);
     }
+    if (fh_.do_ycbcr) {  // Cb, Y, Cr at their coded sizes to the colour size (render.rs:70-72, image.rs:448-486)
+      JXLB_CHECK(colour.size() == 3, kErrBitstream, "YCbCr needs three channels");
+      for (int c = 0; c < 3; ++c) {
+        if (chan_hshift[c] || chan_vshift[c]) {
+          const int id = be_.upsample_jpeg(colour[c], chan_hshift[c] != 0, chan_vshift[c] != 0, cw, chh);
+          frame_planes_.push_back(id);
+          colour[c] = View{id, 0, 0, cw, chh};
+        } else {  // a channel rounded up to an even size in a subsampled direction is cropped
+          colour[c].w = cw;
+          colour[c].h = chh;
+        }
+      }
+      be_.stage_marker("jpeg_upsampled", colour.data(), 3);
+    }
   }
   be_.phase_mark("render_vardct");
   be_.stage_marker("pre_filter", colour.data(), int(colour.size()));
@@ -838,26 +862,31 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
 
   be_.phase_mark("filters");
   // non-separable upsampling of every channel (render.rs:136-183), cropped to the frame size
-  auto upsample_view = [&](View& v) {
-    const uint32_t factor_log2 = ceil_log2_nonzero(fh_.upsampling);
+  auto upsample_view = [&](View& v, uint32_t factor_log2) {
     int id = be_.upsample(v, factor_log2, ih_);
     frame_planes_.push_back(id);
     v = View{id, 0, 0, std::min(v.w << factor_log2, fh_.width), std::min(v.h << factor_log2, fh_.height)};
   };
   if (upsampled) {
-    for (View& v : colour) upsample_view(v);
+    for (View& v : colour) upsample_view(v, ceil_log2_nonzero(fh_.upsampling));
     out.width = fh_.width;
     out.height = fh_.height;
     be_.stage_marker("upsampled", colour.data(), int(colour.size()));
   }
-  // extra channels as floats (they take part in patch blending), upsampled like the colour channels
+  // extra channels as floats with their own bit depth (they take part in patch blending), each upsampled from its coded
+  // size by its whole factor in one chain (image.rs:487-557)
   std::vector<View> extra;
+  bool extra_upsampled = false;
   for (size_t c = ec_from; c < gm_image.size() && (c - ec_from) < ih_.ec_info.size(); ++c) {
     View v = gm_image[c].view;
     be_.int_to_float(v, ih_.ec_info[c - ec_from].bit_depth);
-    if (upsampled) upsample_view(v);
+    if (const uint32_t s = ec_shift(c - ec_from)) {
+      upsample_view(v, s);
+      extra_upsampled = true;
+    }
     extra.push_back(v);
   }
+  if (extra_upsampled) be_.stage_marker("extra_upsampled", extra.data(), int(extra.size()));
   // render_features (jxl-render/src/render.rs:159-225): patches, (splines,) noise - after upsampling, before colour
   if (lfg_.has_patches) {
     std::vector<View> all = colour;

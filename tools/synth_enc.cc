@@ -18,10 +18,13 @@
 // --modular-filters SIGMA gives a --modular frame Gaborish and --epf-iters EPF iterations with constant sigma SIGMA.
 // --sharpness-cell N makes the sharpness map (and so the EPF sigma grid) change every N blocks instead of 16.
 // --hf-lz77 rle|match codes the HF passes with LZ77 (HfLz77 below); everything else is written as without it, and the
-// number of values the decoder takes from copies goes to stderr.
+// number of values the decoder takes from copies goes to stderr. --extra TYPE:BITS:DIM_SHIFT:EC_UPSAMPLING (repeatable)
+// adds extra channels at their coded sizes to a VarDCT or --modular frame; --ycbcr and --upsampling make --modular frames
+// with chroma-subsampled Cb, Y, Cr or a reduced colour resolution (encode_channels).
 //
 // Not part of the product; not a general-purpose encoder (it does not transform an input image).
 #include <algorithm>
+#include <array>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -773,12 +776,28 @@ struct Args {
   float modular_sigma = 0; // --modular-filters S: Gaborish + `epf_iters` EPF iterations on a Modular frame, sigma S (f16)
   uint32_t sharpness_cell = 16;  // the sharpness map is constant over cells of this many 8x8 blocks (EPF sigma 0 in the first)
   uint32_t hf_presets = 1;// HF presets (hf_pass.rs): group g uses preset g % N, each preset has its own (rotated) cluster map
-  std::string dump_raw;    // --modular: also write the source image (3 planes, int32 little endian) for lossless checks
+  std::string dump_raw;    // --modular: also write the source image (3 planes, int32 little endian) for lossless checks;
+                           // with --ycbcr / --upsampling / --extra the coded Modular channels instead (dump_channels)
   bool modular = false;    // a Modular lossless frame (RGB 8 bit, RCT + default Squeeze, weighted predictor) instead of VarDCT
   bool all_types = false;  // every one of the 27 transform types in the frame (forced_layout), the rest drawn from all 27
   int only_type = -1;      // tile every group with this transform type wherever it fits, DCT8 elsewhere
   std::string dump_blocks; // write the varblock layout as text lines "x y type" (8x8 cells) in the order HfMetadata codes them
   HfLz77 hf_lz77;          // --hf-lz77 rle | match | bad-first | bad-length: LZ77 in the HF pass codes (see HfLz77)
+  // Channels coded below the frame's resolution: a --modular frame with any of these is written without transforms,
+  // from seeded integer samples at each channel's coded size (encode_channels); --extra also goes with VarDCT frames
+  std::string ycbcr;       // --ycbcr 444 | 420 | 422 | 440: Cb, Y, Cr colour channels with that chroma subsampling
+  uint32_t upsampling = 1; // --upsampling 1 | 2 | 4 | 8: the frame's colour upsampling
+  struct Extra {
+    uint32_t type, bits, dim_shift, ec_upsampling;  // type: 0 alpha, 2 spot colour, 16 optional (unknown to renderers)
+  };
+  std::vector<Extra> extras;  // --extra TYPE:BITS:DIM_SHIFT:EC_UPSAMPLING, repeatable
+  bool shifted() const { return !ycbcr.empty() || upsampling != 1 || !extras.empty(); }
+  // modular_16bit_buffers promises that every sample fits int16: not so with 16-bit extra channels
+  bool wide_samples() const {
+    for (const Extra& e : extras)
+      if (e.bits > 15) return true;
+    return false;
+  }
 };
 
 // Varblocks placed before the random layout is drawn (--all-types / --only-type): the transform type at each block's
@@ -926,10 +945,140 @@ struct SqStep {
   uint32_t begin_c, num_c;
 };
 
+int write_modular_frame(const Args& a, const std::vector<MChan>& ch, uint32_t cw, uint32_t chh);
+
+// jpeg_upsampling of the frame header for --ycbcr (Cb, Y, Cr): 1 leaves a channel at full size in both directions, 2 and 3
+// in the vertical / horizontal one; 0 subsamples it wherever another channel asks for it (param.rs:105-122)
+std::array<uint32_t, 3> jpeg_upsampling(const Args& a) {
+  const uint32_t y = a.ycbcr == "420" ? 1 : a.ycbcr == "422" ? 2 : a.ycbcr == "440" ? 3 : 0;
+  return {0, y, 0};
+}
+
+// num_extra and one ExtraChannelInfo per --extra (jxl-image/src/lib.rs:303-345)
+void write_extra_channels(BitWriter& w, const Args& a) {
+  const uint32_t n = uint32_t(a.extras.size());
+  if (n < 2) write_u32(w, int(n), 0, 0);
+  else write_u32(w, 2, 4, n - 2);
+  for (const Args::Extra& e : a.extras) {
+    w.write(1, 0);  // not the default alpha channel
+    if (e.type < 2) write_u32(w, int(e.type), 0, 0);
+    else if (e.type < 18) write_u32(w, 2, 4, e.type - 2);
+    else write_u32(w, 3, 6, e.type - 18);
+    w.write(1, 0);  // integer samples
+    if (e.bits == 8 || e.bits == 10 || e.bits == 12) write_u32(w, int((e.bits - 8) / 2), 0, 0);
+    else write_u32(w, 3, 6, e.bits - 1);
+    if (e.dim_shift == 0) write_u32(w, 0, 0, 0);
+    else if (e.dim_shift == 3) write_u32(w, 1, 0, 0);
+    else if (e.dim_shift == 4) write_u32(w, 2, 0, 0);
+    else write_u32(w, 3, 3, e.dim_shift - 1);
+    write_u32(w, 0, 0, 0);  // empty name
+    if (e.type == 0) w.write(1, 0);  // alpha not premultiplied
+    if (e.type == 2)
+      for (float f : {0.75f, 0.5f, 0.25f, 0.625f}) w.write(16, to_f16(f));  // spot colour RGB and solidity
+  }
+}
+
+// The channels of a frame-level Modular image split into streams (image.rs:187-345): the global prefix of channels
+// that fit one group, then every other channel cut by its shift into LF groups (shift >= 3) or pass groups.
+struct ModularStreams {
+  std::vector<Plane2D> global;
+  std::vector<std::vector<Plane2D>> lf, pg;
+};
+ModularStreams split_streams(const std::vector<MChan>& ch, uint32_t cw, uint32_t chh) {
+  const uint32_t gd = 256;
+  const uint32_t gcols = (cw + gd - 1) / gd, grows = (chh + gd - 1) / gd;
+  const uint32_t lcols = (cw + 2047) / 2048, lrows = (chh + 2047) / 2048;
+  ModularStreams st;
+  st.lf.resize(size_t(lcols) * lrows);
+  st.pg.resize(size_t(gcols) * grows);
+  size_t nglobal = 0;
+  while (nglobal < ch.size() && ch[nglobal].p.w <= gd && ch[nglobal].p.h <= gd) st.global.push_back(ch[nglobal++].p);
+  auto crop = [](const Plane2D& p, uint32_t x0, uint32_t y0, uint32_t w, uint32_t h) {
+    Plane2D o;
+    o.w = w, o.h = h;
+    o.v.resize(size_t(w) * h);
+    for (uint32_t y = 0; y < h; ++y)
+      for (uint32_t x = 0; x < w; ++x) o.v[size_t(y) * w + x] = p.at(x0 + x, y0 + y);
+    return o;
+  };
+  for (size_t i = nglobal; i < ch.size(); ++i) {
+    const MChan& c = ch[i];
+    const bool lf = c.hshift >= 3 && c.vshift >= 3;
+    const uint32_t gw = lf ? gd >> (c.hshift - 3) : gd >> c.hshift, gh = lf ? gd >> (c.vshift - 3) : gd >> c.vshift;
+    if (!gw || !gh) fprintf(stderr, "channel shift too large\n"), exit(1);
+    const uint32_t nx = lf ? lcols : gcols, ny = lf ? lrows : grows;
+    for (uint32_t gy = 0; gy < ny; ++gy)
+      for (uint32_t gx = 0; gx < nx; ++gx) {
+        const uint32_t x0 = gx * gw, y0 = gy * gh;
+        if (x0 >= c.p.w || y0 >= c.p.h) continue;
+        Plane2D part = crop(c.p, x0, y0, std::min(gw, c.p.w - x0), std::min(gh, c.p.h - y0));
+        (lf ? st.lf[gy * nx + gx] : st.pg[gy * nx + gx]).push_back(std::move(part));
+      }
+  }
+  return st;
+}
+
+// A channel of seeded samples in [lo, hi]: a smooth ramp plus noise
+MChan draw_channel(std::mt19937& rng, uint32_t w, uint32_t h, int hs, int vs, int32_t lo, int32_t hi) {
+  MChan c;
+  c.p.w = w, c.p.h = h, c.hshift = hs, c.vshift = vs;
+  c.p.v.resize(size_t(w) * h);
+  const double range = double(hi - lo), fx = 0.5 + double(rng() % 1000) / 500.0, fy = 0.5 + double(rng() % 1000) / 500.0;
+  for (uint32_t y = 0; y < h; ++y)
+    for (uint32_t x = 0; x < w; ++x) {
+      const double s = 0.5 + 0.35 * std::sin(fx * x / 7.0 + fy * y / 11.0) + double(int(rng() % 17) - 8) / 160.0;
+      c.p.v[size_t(y) * w + x] = lo + int32_t(std::min(range, std::max(0.0, std::floor(s * range + 0.5))));
+    }
+  return c;
+}
+
+// The --extra channels at their coded sizes over a cw x chh colour grid (lf_global.rs:270-290); a shift below zero is
+// refused by the header rules, so such a channel is drawn at the colour size
+void draw_extras(const Args& a, uint32_t cw, uint32_t chh, std::mt19937& rng, std::vector<MChan>* ch) {
+  for (const Args::Extra& e : a.extras) {
+    const int s = std::max(0, int(ceil_log2_nonzero(e.ec_upsampling) + e.dim_shift) - int(ceil_log2_nonzero(a.upsampling)));
+    const uint32_t add = (1u << s) - 1;
+    ch->push_back(draw_channel(rng, (cw + add) >> s, (chh + add) >> s, s, s, 0, int32_t((1u << e.bits) - 1)));
+  }
+}
+
+// --dump-raw of channels coded without transforms: every channel in coding order, int32 little endian
+int dump_channels(const Args& a, const std::vector<MChan>& ch) {
+  if (a.dump_raw.empty()) return 0;
+  FILE* rf = fopen(a.dump_raw.c_str(), "wb");
+  if (!rf) return perror("fopen"), 1;
+  for (const MChan& c : ch) fwrite(c.p.v.data(), 4, c.p.v.size(), rf);
+  fclose(rf);
+  return 0;
+}
+
+// --ycbcr / --upsampling / --extra: every channel drawn at its coded size (a smooth ramp plus noise over the sample
+// range), coded without transforms. --dump-raw writes the coded channels in coding order, int32 little endian.
+int encode_channels(const Args& a) {
+  const uint32_t up = a.upsampling, cw = (a.width + up - 1) / up, chh = (a.height + up - 1) / up;
+  std::mt19937 rng(a.seed);
+  std::vector<MChan> ch;
+  if (!a.ycbcr.empty()) {  // shift_size (param.rs:142-165), as host/frame_syntax.cc lays the channels out
+    const std::array<uint32_t, 3> ju = jpeg_upsampling(a);
+    bool h_any = false, v_any = false;
+    for (uint32_t j : ju) h_any |= j == 1 || j == 2, v_any |= j == 1 || j == 3;
+    for (uint32_t j : ju) {
+      const bool hs = h_any && (j == 0 || j == 3), vs = v_any && (j == 0 || j == 2);
+      const uint32_t w = h_any ? (hs ? (cw + 1) / 2 : (cw + 1) / 2 * 2) : cw;
+      const uint32_t h = v_any ? (vs ? (chh + 1) / 2 : (chh + 1) / 2 * 2) : chh;
+      ch.push_back(draw_channel(rng, w, h, hs, vs, -128, 127));  // Y is stored less 128/255 (ycbcr.rs), Cb and Cr centred on 0
+    }
+  } else {
+    for (int c = 0; c < 3; ++c) ch.push_back(draw_channel(rng, cw, chh, 0, 0, 0, 255));
+  }
+  draw_extras(a, cw, chh, rng, &ch);
+  if (int r = dump_channels(a, ch)) return r;
+  return write_modular_frame(a, ch, cw, chh);
+}
+
 int encode_modular(const Args& a) {
   const uint32_t W = a.width, H = a.height, gd = 256;
   const uint32_t gcols = (W + gd - 1) / gd, grows = (H + gd - 1) / gd, num_groups = gcols * grows;
-  const uint32_t lcols = (W + 2047) / 2048, lrows = (H + 2047) / 2048, num_lf = lcols * lrows;
   if (num_groups == 1) fprintf(stderr, "single-group frames are not produced by this tool\n"), exit(2);
   std::mt19937 rng(a.seed);
   auto uni = [&](double lo, double hi) { return lo + (hi - lo) * (double(rng()) / 4294967296.0); };
@@ -990,32 +1139,19 @@ int encode_modular(const Args& a) {
     if (sp.in_place) ch.insert(ch.begin() + sp.begin_c + sp.num_c, residu.begin(), residu.end());
     else ch.insert(ch.end(), residu.begin(), residu.end());
   }
-  // ---- streams (image.rs:187-345): global prefix, then by shift into LF groups (shift >= 3) or pass groups ----
-  size_t nglobal = 0;
-  while (nglobal < ch.size() && ch[nglobal].p.w <= gd && ch[nglobal].p.h <= gd) ++nglobal;
-  std::vector<std::vector<Plane2D>> lf_streams(num_lf), pg_streams(num_groups);
-  auto crop = [](const Plane2D& p, uint32_t x0, uint32_t y0, uint32_t w, uint32_t h) {
-    Plane2D o;
-    o.w = w, o.h = h;
-    o.v.resize(size_t(w) * h);
-    for (uint32_t y = 0; y < h; ++y)
-      for (uint32_t x = 0; x < w; ++x) o.v[size_t(y) * w + x] = p.at(x0 + x, y0 + y);
-    return o;
-  };
-  for (size_t i = nglobal; i < ch.size(); ++i) {
-    const MChan& c = ch[i];
-    const bool lf = c.hshift >= 3 && c.vshift >= 3;
-    const uint32_t gw = lf ? gd >> (c.hshift - 3) : gd >> c.hshift, gh = lf ? gd >> (c.vshift - 3) : gd >> c.vshift;
-    if (!gw || !gh) fprintf(stderr, "channel shift too large\n"), exit(1);
-    const uint32_t nx = lf ? lcols : gcols, ny = lf ? lrows : grows;
-    for (uint32_t gy = 0; gy < ny; ++gy)
-      for (uint32_t gx = 0; gx < nx; ++gx) {
-        const uint32_t x0 = gx * gw, y0 = gy * gh;
-        if (x0 >= c.p.w || y0 >= c.p.h) continue;
-        Plane2D part = crop(c.p, x0, y0, std::min(gw, c.p.w - x0), std::min(gh, c.p.h - y0));
-        (lf ? lf_streams[gy * nx + gx] : pg_streams[gy * nx + gx]).push_back(std::move(part));
-      }
-  }
+  return write_modular_frame(a, ch, W, H);
+}
+
+// Writes a Modular frame of coded channels `ch` over a cw x ch_ colour sample grid: with a.shifted() without
+// transforms and with the header fields of encode_channels, otherwise with RCT + default Squeeze.
+int write_modular_frame(const Args& a, const std::vector<MChan>& ch, uint32_t cw, uint32_t chh) {
+  const uint32_t W = a.width, H = a.height, gd = 256;
+  const uint32_t gcols = (cw + gd - 1) / gd, grows = (chh + gd - 1) / gd, num_groups = gcols * grows;
+  const uint32_t lcols = (cw + 2047) / 2048, lrows = (chh + 2047) / 2048, num_lf = lcols * lrows;
+  const ModularStreams st = split_streams(ch, cw, chh);
+  const size_t nglobal = st.global.size();
+  const std::vector<std::vector<Plane2D>>& lf_streams = st.lf;
+  const std::vector<std::vector<Plane2D>>& pg_streams = st.pg;
   // ---- tree: chain on the weighted predictor's max error, WP leaves; tokens of every stream ----
   std::vector<TreeNode> nodes;
   {
@@ -1061,15 +1197,18 @@ int encode_modular(const Args& a) {
     std::vector<uint8_t> map(size_t(tree.num_leaves()));
     for (size_t i = 0; i < map.size(); ++i) map[i] = uint8_t(i);
     enc.write_header(w, all, uint32_t(map.size()), map);
-    // GlobalModular header (lib.rs:117-125): global tree, default WP, two transforms
-    w.write(1, 1);
-    w.write(1, 1);
-    write_u32(w, 2, 4, 0);  // nb_transforms = 2
-    w.write(2, 0);          // RCT
-    write_u32(w, 0, 3, 0);  //   begin_c = 0
-    write_u32(w, 0, 0, 0);  //   rct_type = 6
-    w.write(2, 2);          // Squeeze
-    write_u32(w, 0, 0, 0);  //   num_sq = 0: default parameters
+    if (a.shifted()) {
+      write_modular_header(w);
+    } else {  // GlobalModular header (lib.rs:117-125): global tree, default WP, two transforms
+      w.write(1, 1);
+      w.write(1, 1);
+      write_u32(w, 2, 4, 0);  // nb_transforms = 2
+      w.write(2, 0);          // RCT
+      write_u32(w, 0, 3, 0);  //   begin_c = 0
+      write_u32(w, 0, 0, 0);  //   rct_type = 6
+      w.write(2, 2);          // Squeeze
+      write_u32(w, 0, 0, 0);  //   num_sq = 0: default parameters
+    }
     enc.write_tokens(w, global_tokens);
     w.pad();
   }
@@ -1103,8 +1242,8 @@ int encode_modular(const Args& a) {
   cs.write(1, 0);  // extra_fields
   cs.write(1, 0);  // integer samples
   cs.write(2, 0);  // 8 bits
-  cs.write(1, 1);  // modular_16bit_buffers
-  cs.write(2, 0);  // no extra channels
+  cs.write(1, a.wide_samples() ? 0 : 1);  // modular_16bit_buffers
+  write_extra_channels(cs, a);
   cs.write(1, 0);  // xyb_encoded = 0
   cs.write(1, 1);  // ColourEncoding all_default (sRGB)
   cs.write(2, 0);  // extensions
@@ -1115,12 +1254,16 @@ int encode_modular(const Args& a) {
   cs.write(2, 0);      // Regular
   cs.write(1, 1);      // Modular
   cs.write(2, 0);      // flags = 0
-  cs.write(1, 0);      // do_ycbcr
-  cs.write(2, 0);      // upsampling = 1
+  cs.write(1, a.ycbcr.empty() ? 0 : 1);  // do_ycbcr
+  if (!a.ycbcr.empty())
+    for (uint32_t j : jpeg_upsampling(a)) cs.write(2, j);
+  cs.write(2, ceil_log2_nonzero(a.upsampling));  // upsampling: U32 selector k is 2^k
+  for (const Args::Extra& e : a.extras) cs.write(2, ceil_log2_nonzero(e.ec_upsampling));
   cs.write(2, 1);      // group_size_shift = 1 (256)
   cs.write(2, 0);      // num_passes = 1
   cs.write(1, 0);      // have_crop
   cs.write(2, 0);      // blend mode Replace
+  for (size_t i = 0; i < a.extras.size(); ++i) cs.write(2, 0);  // extra channels: Replace as well
   cs.write(1, 1);      // is_last
   cs.write(2, 0);      // name: empty
   cs.write(1, 0);      // restoration filter: not all_default
@@ -1141,6 +1284,8 @@ int encode_modular(const Args& a) {
   cs.write(2, 0);      // frame extensions
   cs.write(1, 0);      // TOC not permuted
   cs.pad();
+  // one group: a single TOC entry; every channel fits the global stream, so LfGlobal is all there is
+  if (num_groups == 1) sections.resize(1);
   for (const BitWriter& sct : sections) {
     const uint32_t sz = uint32_t(sct.bytes.size());
     if (sz < 1024) write_u32(cs, 0, 10, sz);
@@ -1186,8 +1331,28 @@ int main(int argc, char** argv) {
     else if (s == "--dump-blocks") a.dump_blocks = next();
     else if (s == "--hf-lz77") a.hf_lz77.mode = next();
     else if (s == "-o") a.out = next();
+    else if (s == "--ycbcr") a.ycbcr = next();
+    else if (s == "--upsampling") a.upsampling = uint32_t(atoi(next().c_str()));
+    else if (s == "--extra") {
+      const std::string spec = next();
+      const size_t c1 = spec.find(':');
+      const std::string type = spec.substr(0, c1);
+      Args::Extra e{type == "alpha" ? 0u : type == "spot" ? 2u : 16u, 8, 0, 1};
+      if (c1 == std::string::npos || (type != "alpha" && type != "spot" && type != "unknown") ||
+          sscanf(spec.c_str() + c1 + 1, "%u:%u:%u", &e.bits, &e.dim_shift, &e.ec_upsampling) != 3 || e.bits < 1 ||
+          e.bits > 16 || e.dim_shift > 8 || (e.ec_upsampling != 1 && e.ec_upsampling != 2 && e.ec_upsampling != 4 && e.ec_upsampling != 8))
+        fprintf(stderr, "--extra takes alpha|spot|unknown:BITS(1..16):DIM_SHIFT(0..8):EC_UPSAMPLING(1|2|4|8)\n"), exit(2);
+      a.extras.push_back(e);
+    }
     else fprintf(stderr, "unknown arg %s\n", s.c_str()), exit(2);
   }
+  if (!a.ycbcr.empty() && a.ycbcr != "444" && a.ycbcr != "420" && a.ycbcr != "422" && a.ycbcr != "440")
+    fprintf(stderr, "--ycbcr takes 444, 420, 422 or 440\n"), exit(2);
+  if (a.upsampling != 1 && a.upsampling != 2 && a.upsampling != 4 && a.upsampling != 8)
+    fprintf(stderr, "--upsampling takes 1, 2, 4 or 8\n"), exit(2);
+  if ((!a.ycbcr.empty() || a.upsampling != 1) && !a.modular) fprintf(stderr, "--ycbcr and --upsampling make --modular frames\n"), exit(2);
+  if (!a.extras.empty() && a.lf_frame) fprintf(stderr, "--extra is not written with --lf-frame\n"), exit(2);
+  if (a.modular && a.shifted()) return encode_channels(a);
   const std::string& lzm = a.hf_lz77.mode;
   if (!lzm.empty() && (a.modular || (lzm != "rle" && lzm != "match" && lzm != "bad-first" && lzm != "bad-length")))
     fprintf(stderr, "--hf-lz77 takes rle, match, bad-first or bad-length (VarDCT frames only)\n"), exit(2);
@@ -1321,6 +1486,28 @@ int main(int argc, char** argv) {
     modular_tokens(tree, hm, int32_t(1 + 2 * num_lf + lg), &hfmeta_tokens[lg]);
     if (!a.lf_frame) lf_tokens_all.insert(lf_tokens_all.end(), lfcoeff_tokens[lg].begin(), lfcoeff_tokens[lg].end());
     lf_tokens_all.insert(lf_tokens_all.end(), hfmeta_tokens[lg].begin(), hfmeta_tokens[lg].end());
+  }
+
+  // ---- --extra: the extra channels' streams of the frame's Modular image (GlobalModular, LF groups, and pass groups
+  // of the last pass, after its HF data), coded with the global tree like the other Modular streams ----
+  std::vector<Token> ex_global_tokens;
+  std::vector<std::vector<Token>> ex_lf_tokens(num_lf), ex_pg_tokens(num_groups);
+  if (!a.extras.empty()) {
+    std::mt19937 erng(a.seed ^ 0x9e3779b9u);  // apart from the frame's own draws, which stay as without --extra
+    std::vector<MChan> ech;
+    draw_extras(a, W, H, erng, &ech);
+    if (int r = dump_channels(a, ech)) return r;
+    const ModularStreams st = split_streams(ech, W, H);
+    modular_tokens(tree, st.global, 0, &ex_global_tokens);
+    lf_tokens_all.insert(lf_tokens_all.end(), ex_global_tokens.begin(), ex_global_tokens.end());
+    for (uint32_t lg = 0; lg < num_lf; ++lg) {
+      modular_tokens(tree, st.lf[lg], int32_t(1 + num_lf + lg), &ex_lf_tokens[lg]);
+      lf_tokens_all.insert(lf_tokens_all.end(), ex_lf_tokens[lg].begin(), ex_lf_tokens[lg].end());
+    }
+    for (uint32_t g = 0; g < num_groups; ++g) {
+      modular_tokens(tree, st.pg[g], int32_t(1 + 3 * num_lf + 17 + (P - 1) * num_groups + g), &ex_pg_tokens[g]);
+      lf_tokens_all.insert(lf_tokens_all.end(), ex_pg_tokens[g].begin(), ex_pg_tokens[g].end());
+    }
   }
 
   // ---- HF tokens per group ----
@@ -1470,6 +1657,10 @@ int main(int argc, char** argv) {
     std::vector<uint8_t> map(size_t(tree.num_leaves()));
     for (size_t i = 0; i < map.size(); ++i) map[i] = uint8_t(i);
     lf_enc.write_header(w, lf_tokens_all, uint32_t(map.size()), map);
+    if (!a.extras.empty()) {  // GlobalModular stream
+      write_modular_header(w);
+      lf_enc.write_tokens(w, ex_global_tokens);
+    }
     end_section(w);
   }
   for (uint32_t lg = 0; lg < num_lf; ++lg) {
@@ -1480,6 +1671,10 @@ int main(int argc, char** argv) {
       w.write(2, 0);  // extra_precision
       write_modular_header(w);
       lf_enc.write_tokens(w, lfcoeff_tokens[lg]);
+    }
+    if (!ex_lf_tokens[lg].empty()) {  // Modular LF-group channels, between LfCoeff and HfMetadata
+      write_modular_header(w);
+      lf_enc.write_tokens(w, ex_lf_tokens[lg]);
     }
     w.write(int(ceil_log2_nonzero(lw * lh)), nb_blocks[lg] - 1);
     write_modular_header(w);
@@ -1507,6 +1702,10 @@ int main(int argc, char** argv) {
       w.write(int(ceil_log2_nonzero(NP)), g % NP);  // hfp: 0 bits with a single preset
       if (a.hf_lz77.mode.empty()) hf_enc[pass].write_tokens(w, hf_tokens[size_t(pass) * num_groups + g]);
       else hf_enc[pass].write_syms(w, hf_syms[size_t(pass) * num_groups + g]);
+      if (pass + 1 == P && !ex_pg_tokens[g].empty()) {  // Modular pass-group channels, after the HF data
+        write_modular_header(w);
+        lf_enc.write_tokens(w, ex_pg_tokens[g]);
+      }
       end_section(w);
     }
 
@@ -1523,9 +1722,27 @@ int main(int argc, char** argv) {
   write_dim(H);
   cs.write(3, 0);  // ratio
   write_dim(W);
-  if (a.colour.empty()) {
+  if (a.colour.empty() && a.extras.empty()) {
     cs.write(1, 1);  // ImageMetadata all_default
-  } else {  // ImageMetadata with an enum ColourEncoding (jxl-image/src/lib.rs:229-287, color.rs:21-58)
+  } else {  // ImageMetadata with extra channels and / or an enum ColourEncoding (jxl-image/src/lib.rs:229-287, color.rs:21-58)
+    const bool pq = a.colour == "pq";
+    cs.write(1, 0);  // all_default
+    cs.write(1, pq ? 1 : 0);  // extra_fields
+    if (pq) {
+      cs.write(3, 0);  // orientation 1
+      cs.write(1, 0);  // have_intrinsic_size
+      cs.write(1, 0);  // have_preview
+      cs.write(1, 0);  // have_animation
+    }
+    cs.write(1, 0);  // integer samples
+    cs.write(2, 0);  // 8 bits
+    cs.write(1, a.wide_samples() ? 0 : 1);  // modular_16bit_buffers
+    write_extra_channels(cs, a);
+    cs.write(1, 1);  // xyb_encoded
+    cs.write(1, a.colour.empty() ? 1 : 0);  // ColourEncoding all_default (sRGB)
+  }
+  if (!a.colour.empty()) {
+    const bool pq = a.colour == "pq";
     auto write_enum = [&](uint32_t v) {
       if (v == 0) write_u32(cs, 0, 0, 0);
       else if (v == 1) write_u32(cs, 1, 0, 0);
@@ -1541,21 +1758,6 @@ int main(int argc, char** argv) {
         else write_u32(cs, 3, 21, u - 2097152);
       }
     };
-    const bool pq = a.colour == "pq";
-    cs.write(1, 0);  // all_default
-    cs.write(1, pq ? 1 : 0);  // extra_fields
-    if (pq) {
-      cs.write(3, 0);  // orientation 1
-      cs.write(1, 0);  // have_intrinsic_size
-      cs.write(1, 0);  // have_preview
-      cs.write(1, 0);  // have_animation
-    }
-    cs.write(1, 0);  // integer samples
-    cs.write(2, 0);  // 8 bits
-    cs.write(1, 1);  // modular_16bit_buffers
-    cs.write(2, 0);  // no extra channels
-    cs.write(1, 1);  // xyb_encoded
-    cs.write(1, 0);  // ColourEncoding all_default
     cs.write(1, 0);  // want_icc
     const bool grey = a.colour == "gray";
     write_enum(grey ? 1 : 0);  // colour space: RGB / Grey
@@ -1583,8 +1785,8 @@ int main(int argc, char** argv) {
       cs.write(1, 0);        // relative_to_max_display
       cs.write(16, 0);       // linear_below
     }
-    cs.write(2, 0);  // extensions
   }
+  if (!a.colour.empty() || !a.extras.empty()) cs.write(2, 0);  // extensions
   cs.write(1, 1);  // default_m
   cs.pad();
   auto write_u64_small = [&](uint32_t v) {  // U64 (jxl-bitstream): 0 | 1 + u(4) | 17 + u(8)
@@ -1659,12 +1861,13 @@ int main(int argc, char** argv) {
     cs.write(2, 0);         // name: empty
     cs.write(1, 1);         // restoration filter all_default
     write_u64_small(0);     // frame extensions
-  } else if (P > 1 || a.epf_iters != 2 || !a.gaborish) {
+  } else if (P > 1 || a.epf_iters != 2 || !a.gaborish || !a.extras.empty()) {
     cs.write(1, 0);         // all_default
     cs.write(2, 0);         // Regular
     cs.write(1, 0);         // VarDCT
     write_u64_small(0);     // flags
     cs.write(2, 0);         // upsampling = 1
+    for (const Args::Extra& e : a.extras) cs.write(2, ceil_log2_nonzero(e.ec_upsampling));  // U32 selector k is 2^k
     cs.write(3, 3);         // x_qm_scale
     cs.write(3, 2);         // b_qm_scale
     cs.write(2, P - 1);     // num_passes (1, 2 or 3)
@@ -1674,6 +1877,7 @@ int main(int argc, char** argv) {
     }
     cs.write(1, 0);         // have_crop
     cs.write(2, 0);         // blend mode Replace
+    for (size_t i = 0; i < a.extras.size(); ++i) cs.write(2, 0);  // extra channels: Replace as well
     cs.write(1, 1);         // is_last
     cs.write(2, 0);         // name: empty
     if (a.epf_iters == 2 && a.gaborish) {
