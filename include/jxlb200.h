@@ -71,6 +71,24 @@ int32_t jxlb_decode(jxlb_decoder* dec, const uint8_t* data, size_t size, const j
 /* Keep an encoded image resident in HBM (slot id chosen by the caller) and decode from it: the
  * timed region of a device-resident benchmark then contains no host->device copy of the input. */
 int32_t jxlb_preload(jxlb_decoder* dec, int32_t slot, const uint8_t* data, size_t size);
+
+/* ---- Keyframes one at a time ----
+ * A header-only pass over the codestream (no section is decoded) records what each frame reads from and writes to the
+ * four reference slots and the four LF stores, and cuts the frames into segments: a segment starts after a keyframe
+ * and none of its frames reads a slot or store last written before it. So a segment decodes on its own, from empty
+ * slots, and an animation of full-canvas Replace frames has one segment per keyframe, while one whose every frame
+ * blends onto the previous canvas is a single segment. */
+/* The number of keyframes (what jxlb_decode renders) and of segments. Host only: needs no decoder and no device. On a
+ * stream whose image header cannot be read, the error code with both counts 0. On a stream that ends in a frame that
+ * cannot be read or is cut off, the error code with the counts of the frames before it plus one keyframe for the
+ * broken frame: jxlb_pipeline_submit_keyframes reports that many keyframes, the last one with the error. */
+int32_t jxlb_image_keyframes(const uint8_t* data, size_t size, int32_t* num_keyframes, int32_t* num_segments);
+/* JxlImage::render_frame(k) (crates/jxl-oxide/src/lib.rs:710-740): decodes the segment that holds keyframe `keyframe`
+ * up to it, releasing each earlier keyframe of the segment as soon as it is rendered, so only keyframe k stays
+ * resident, as frame 0 of the decoder: the frame accessors and packers work on it unchanged. HBM use is bounded by the
+ * segment's reference slots and LF stores plus one keyframe, whatever the animation's length. Bit-identical to frame k of
+ * jxlb_decode. opt->max_frames is ignored; the allocation budget of jxlb_decoder_create_ex applies. */
+int32_t jxlb_decode_keyframe(jxlb_decoder* dec, const uint8_t* data, size_t size, const jxlb_options* opt, int32_t keyframe);
 int32_t jxlb_decode_slot(jxlb_decoder* dec, int32_t slot, const jxlb_options* opt);
 int32_t jxlb_image_get_info(const jxlb_decoder* dec, jxlb_image_info* info);
 /* JxlImage::original_icc (crates/jxl-oxide/src/lib.rs:536-540): the embedded ICC profile, reconstructed from the
@@ -265,6 +283,23 @@ int32_t jxlb_pipeline_submit(jxlb_pipeline* p, const uint8_t* data, size_t size,
  * JXLB_ERR_INVALID_ARG when nothing is in flight. */
 int32_t jxlb_pipeline_wait(jxlb_pipeline* p, uint64_t* tag, int32_t* status, void** out, size_t* out_bytes, char* err,
                            size_t err_cap);
+/* Queue every keyframe of an animation (or of a still image: one keyframe): the image is indexed here (see
+ * jxlb_image_keyframes) and each segment becomes one task, spread over the workers like any other frame; a task holds one
+ * heavy slot from its first heavy stage to its last keyframe. Same arguments and out modes as jxlb_pipeline_submit. A
+ * caller `dst` holds num_keyframes outputs back to back: keyframe k goes at k * (dst_bytes / num_keyframes). With
+ * dst = NULL each keyframe takes its own buffer of the ring. Every keyframe is reported exactly once, through
+ * jxlb_pipeline_wait_keyframe: within a segment in order, across segments in completion order. When a segment fails,
+ * its failing keyframe and the ones after it are reported with that status and no output; other segments are
+ * unaffected. An image whose header cannot be read is reported once, as keyframe 0. jxlb_pipeline_wait returns these
+ * reports too, one per keyframe, without the keyframe index.
+ * The ring: a task waiting for a free ring buffer keeps its heavy slot, so with dst = NULL the caller must release each
+ * output (jxlb_pipeline_release_output) once it has consumed it, rather than waiting for a whole submission first;
+ * otherwise a segment with more keyframes than the ring has buffers never finishes. */
+int32_t jxlb_pipeline_submit_keyframes(jxlb_pipeline* p, const uint8_t* data, size_t size, int32_t slot, int32_t out_mode,
+                                       void* dst, size_t dst_bytes, uint64_t tag);
+/* jxlb_pipeline_wait plus the keyframe index of the report (-1 for a frame of jxlb_pipeline_submit). */
+int32_t jxlb_pipeline_wait_keyframe(jxlb_pipeline* p, uint64_t* tag, int32_t* keyframe, int32_t* status, void** out,
+                                    size_t* out_bytes, char* err, size_t err_cap);
 /* Returns a pipeline-owned output buffer (from jxlb_pipeline_wait) to the ring. */
 int32_t jxlb_pipeline_release_output(jxlb_pipeline* p, void* out);
 uint64_t jxlb_pipeline_launch_count(const jxlb_pipeline* p);

@@ -35,6 +35,7 @@ EXPORTED_SYMBOLS = [
     "jxlb_pipeline_create", "jxlb_pipeline_destroy", "jxlb_pipeline_last_error", "jxlb_pipeline_preload", "jxlb_pipeline_submit",
     "jxlb_pipeline_wait", "jxlb_pipeline_release_output", "jxlb_pipeline_launch_count", "jxlb_pipeline_workers", "jxlb_pipeline_decoder",
     "jxlb_jpeg_reconstruction_status", "jxlb_reconstruct_jpeg", "jxlb_jpeg_copy",
+    "jxlb_image_keyframes", "jxlb_decode_keyframe", "jxlb_pipeline_submit_keyframes", "jxlb_pipeline_wait_keyframe",
 ]
 
 
@@ -150,6 +151,9 @@ def load_library():
     L.jxlb_pipeline_submit.argtypes = [vp, vp, ctypes.c_size_t, i32, i32, vp, ctypes.c_size_t, ctypes.c_uint64]
     L.jxlb_pipeline_wait.argtypes = [vp, ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(i32), ctypes.POINTER(vp),
                                      ctypes.POINTER(ctypes.c_size_t), ctypes.c_char_p, ctypes.c_size_t]
+    L.jxlb_pipeline_submit_keyframes.argtypes = [vp, vp, ctypes.c_size_t, i32, i32, vp, ctypes.c_size_t, ctypes.c_uint64]
+    L.jxlb_pipeline_wait_keyframe.argtypes = [vp, ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(i32), ctypes.POINTER(i32),
+                                              ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t), ctypes.c_char_p, ctypes.c_size_t]
     L.jxlb_pipeline_release_output.argtypes = [vp, vp]
     L.jxlb_pipeline_launch_count.argtypes = [vp]
     L.jxlb_pipeline_launch_count.restype = ctypes.c_uint64
@@ -162,6 +166,9 @@ def load_library():
     L.jxlb_reconstruct_jpeg.restype = i32
     L.jxlb_jpeg_copy.argtypes = [vp, vp, ctypes.c_size_t]
     L.jxlb_jpeg_copy.restype = i32
+    L.jxlb_image_keyframes.argtypes = [ctypes.c_char_p, ctypes.c_size_t, ctypes.POINTER(i32), ctypes.POINTER(i32)]
+    L.jxlb_image_keyframes.restype = i32
+    L.jxlb_decode_keyframe.argtypes = [vp, ctypes.c_char_p, ctypes.c_size_t, ctypes.POINTER(_Options), i32]
     _lib = L
     return L
 
@@ -242,6 +249,12 @@ class Decoder:
         out = torch.empty((h * factor, w * factor), dtype=torch.float32, device=src.device)
         self._check(self._L.jxlb_upsample(self._h, int(src.data_ptr()), w, h, src.stride(0), factor, int(out.data_ptr()), out.stride(0)))
         return out
+
+    def decode_keyframe(self, data: bytes, keyframe, output_colour=0):
+        """jxlb_decode_keyframe (JxlImage::render_frame(k)): keyframe `keyframe` alone, resident as frame 0. Only the
+        segment that holds it is decoded, and only one keyframe is resident at a time."""
+        opt = _Options(output_colour, 0)
+        self._check(self._L.jxlb_decode_keyframe(self._h, data, len(data), ctypes.byref(opt), int(keyframe)))
 
     def preload(self, slot, data: bytes):
         self._check(self._L.jxlb_preload(self._h, slot, data, len(data)))
@@ -451,6 +464,8 @@ class Pipeline:
             raise JxlError(rc, "cannot create a pipeline (no CUDA device? there is no CPU fallback)")
         self._h = h
         self._keep = {}      # tag -> objects that must outlive the job (input bytes, output arrays)
+        self._reports = {}   # tag of a keyframe submission -> reports still to come
+        self._slot_reports = {}  # preloaded slot -> reports a keyframe submission of it gives
         self._next_tag = 0
         self.in_flight = 0
 
@@ -461,6 +476,28 @@ class Pipeline:
         rc = self._L.jxlb_pipeline_preload(self._h, slot, data, len(data))
         if rc != OK:
             self._err(rc)
+        self._slot_reports[slot] = _keyframe_reports(data)
+
+    def _take(self, tag):
+        """The objects kept for `tag`, released with its last report."""
+        left = self._reports.get(tag, 1) - 1
+        if left > 0:
+            self._reports[tag] = left
+            return self._keep.get(tag)
+        self._reports.pop(tag, None)
+        return self._keep.pop(tag, None)
+
+    @classmethod
+    def _dst(cls, out, mode):
+        if mode is None and not hasattr(out, "data_ptr"):  # out=None + explicit mode: pixels in a pipeline-owned pinned buffer
+            mode = cls.OUT_NONE if out is None else {np.dtype(np.float32): 1, np.dtype(np.uint8): 2, np.dtype(np.uint16): 3}[out.dtype]
+        if out is not None and hasattr(out, "data_ptr"):  # a torch CUDA tensor: packed on the device, never leaves HBM
+            if mode is None or mode < 4:
+                mode = {1: cls.OUT_U8_DEVICE, 2: cls.OUT_U16_DEVICE}[out.element_size()]
+            dst, nbytes = int(out.data_ptr()), out.numel() * out.element_size()
+        else:
+            dst, nbytes = (out.ctypes.data, out.nbytes) if out is not None else (None, 0)
+        return mode, dst, nbytes
 
     def submit(self, data=None, slot=-1, out=None, mode=None, tag=None):
         """Queues one frame: `data` (bytes) or a preloaded `slot`. `out`: None (decode only), a float32 (c, h, w) array
@@ -468,14 +505,7 @@ class Pipeline:
         if tag is None:
             tag = self._next_tag
             self._next_tag += 1
-        if mode is None and not hasattr(out, "data_ptr"):  # out=None + explicit mode: pixels in a pipeline-owned pinned buffer
-            mode = self.OUT_NONE if out is None else {np.dtype(np.float32): 1, np.dtype(np.uint8): 2, np.dtype(np.uint16): 3}[out.dtype]
-        if out is not None and hasattr(out, "data_ptr"):  # a torch CUDA tensor: packed on the device, never leaves HBM
-            if mode is None or mode < 4:
-                mode = {1: self.OUT_U8_DEVICE, 2: self.OUT_U16_DEVICE}[out.element_size()]
-            dst, nbytes = int(out.data_ptr()), out.numel() * out.element_size()
-        else:
-            dst, nbytes = (out.ctypes.data, out.nbytes) if out is not None else (None, 0)
+        mode, dst, nbytes = self._dst(out, mode)
         buf = None
         if data is not None:
             buf = ctypes.c_char_p(data)
@@ -498,7 +528,7 @@ class Pipeline:
         if rc != OK:
             raise JxlError(rc, "no frame in flight")
         self.in_flight -= 1
-        kept = self._keep.pop(tag.value, None)
+        kept = self._take(tag.value)
         if status.value != OK:
             raise JxlError(status.value, msg.value.decode(errors="replace"))
         owned = out.value is not None and (kept is None or kept[2] is None)
@@ -509,6 +539,51 @@ class Pipeline:
         if owned:
             self._L.jxlb_pipeline_release_output(self._h, out)
         return tag.value
+
+    def submit_keyframes(self, data=None, slot=-1, out=None, mode=None, tag=None):
+        """Queues every keyframe of `data` (bytes) or of a preloaded `slot`, one task per independent segment
+        (jxlb_pipeline_submit_keyframes). `out` as for submit() with a leading keyframe axis: (num_keyframes, ...);
+        keyframe k lands in out[k]. Collect the reports with wait_keyframe(); with out=None and a mode, release each
+        output as it is consumed. Returns the tag."""
+        if tag is None:
+            tag = self._next_tag
+            self._next_tag += 1
+        mode, dst, nbytes = self._dst(out, mode)
+        reports = _keyframe_reports(data) if data is not None else self._slot_reports.get(slot, 1)
+        buf = ctypes.c_char_p(data) if data is not None else None
+        rc = self._L.jxlb_pipeline_submit_keyframes(self._h, ctypes.cast(buf, ctypes.c_void_p) if buf is not None else None,
+                                                    len(data) if data is not None else 0, slot, mode, dst, nbytes, tag)
+        if rc != OK:
+            self._err(rc)
+        if reports:
+            self._keep[tag] = (data, buf, out)
+            self._reports[tag] = reports
+        self.in_flight += reports
+        return tag
+
+    def wait_keyframe(self, want_output=False):
+        """Blocks until one keyframe (or frame of submit()) has finished; returns (tag, keyframe), or
+        (tag, keyframe, address, nbytes) with want_output; keyframe is -1 for a frame of submit(). Raises JxlError, with
+        the report's `tag` and `keyframe` attributes, when that keyframe failed."""
+        tag, kf, status = ctypes.c_uint64(), ctypes.c_int32(), ctypes.c_int32()
+        out, nbytes = ctypes.c_void_p(), ctypes.c_size_t()
+        msg = ctypes.create_string_buffer(256)
+        rc = self._L.jxlb_pipeline_wait_keyframe(self._h, ctypes.byref(tag), ctypes.byref(kf), ctypes.byref(status), ctypes.byref(out),
+                                                 ctypes.byref(nbytes), msg, 256)
+        if rc != OK:
+            raise JxlError(rc, "no frame in flight")
+        self.in_flight -= 1
+        kept = self._take(tag.value)
+        if status.value != OK:
+            e = JxlError(status.value, msg.value.decode(errors="replace"))
+            e.tag, e.keyframe = tag.value, kf.value
+            raise e
+        owned = out.value is not None and (kept is None or kept[2] is None)
+        if want_output:
+            return tag.value, kf.value, out.value, nbytes.value
+        if owned:
+            self._L.jxlb_pipeline_release_output(self._h, out)
+        return tag.value, kf.value
 
     def release_output(self, address):
         self._L.jxlb_pipeline_release_output(self._h, ctypes.c_void_p(address))
@@ -616,6 +691,25 @@ class JxlImage:
         if self._jpeg_dec is None:
             self._jpeg_dec = Decoder(self._dec.device)
         return self._jpeg_dec.reconstruct_jpeg(self._data)
+
+
+def image_keyframes(data: bytes):
+    """(num_keyframes, num_segments, status) from a header-only pass (jxlb_image_keyframes; no device needed). status is
+    OK, or the error of a last frame that is malformed or cut off, which is then counted as one more keyframe; when
+    not even the image header can be read, JxlError is raised."""
+    nk, ns = ctypes.c_int32(), ctypes.c_int32()
+    rc = load_library().jxlb_image_keyframes(data, len(data), ctypes.byref(nk), ctypes.byref(ns))
+    if rc != OK and nk.value == 0:
+        raise JxlError(rc, "cannot read the image header")
+    return nk.value, ns.value, rc
+
+
+def _keyframe_reports(data):
+    """How many reports jxlb_pipeline_submit_keyframes gives for `data`: one per keyframe, or one for an unreadable header."""
+    try:
+        return image_keyframes(data)[0]
+    except JxlError:
+        return 1
 
 
 def jpeg_reconstruction_status(data: bytes) -> int:

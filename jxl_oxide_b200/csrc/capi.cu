@@ -73,6 +73,39 @@ int32_t decode_resident(jxlb_decoder* dec, const uint8_t* cs, size_t size, const
   });
 }
 
+namespace {
+struct KeyframeStop {  // thrown through decode_segment when the caller's keyframe callback fails
+  int32_t code;
+};
+}  // namespace
+
+int32_t decode_segment_keyframes(jxlb_decoder* dec, const uint8_t* cs, size_t size, const uint8_t* dptr, const FrameIndex& index,
+                                 size_t seg, uint32_t last_keyframe, const jxlb_options* opt, bool keep_last,
+                                 const std::function<int32_t(uint32_t)>& on_keyframe) {
+  if (!dec || !cs) return JXLB_ERR_INVALID_ARG;
+  int32_t stop = JXLB_OK;
+  const int32_t rc = guarded(dec, [&] {
+    release(dec);
+    DecodeOptions o;
+    if (opt) o.output_colour = opt->output_colour;
+    if (dptr) dec->be->use_resident_once(dptr);
+    try {
+      decode_segment(*dec->be, cs, size, o, index, seg, last_keyframe, [&](uint32_t k, const ImageHeader& ih, DecodedFrame&& f) {
+        dec->res.image_header = ih;
+        dec->res.frames.push_back(std::move(f));
+        dec->have_result = true;
+        const int32_t r = on_keyframe(k);
+        if (r != JXLB_OK) throw KeyframeStop{r};
+        if (!(keep_last && k == last_keyframe)) release(dec);
+      });
+    } catch (const KeyframeStop& s) {
+      stop = s.code;
+    }
+  });
+  if (rc != JXLB_OK || stop != JXLB_OK) release(dec);
+  return stop != JXLB_OK ? stop : rc;
+}
+
 int32_t frame_planar_to_host(jxlb_decoder* dec, int32_t frame, float* dst, size_t dst_bytes) {
   if (!dec || !dst || !dec->have_result || frame < 0 || size_t(frame) >= dec->res.frames.size()) return JXLB_ERR_INVALID_ARG;
   return guarded(dec, [&] {
@@ -276,6 +309,38 @@ int32_t jxlb_decode(jxlb_decoder* dec, const uint8_t* data, size_t size, const j
     dec->res = decode_codestream(*dec->be, dec->codestream.data(), dec->codestream.size(), o);
     dec->have_result = true;
   });
+}
+
+int32_t jxlb_image_keyframes(const uint8_t* data, size_t size, int32_t* num_keyframes, int32_t* num_segments) {
+  if (num_keyframes) *num_keyframes = 0;
+  if (num_segments) *num_segments = 0;
+  if (!data) return JXLB_ERR_INVALID_ARG;
+  try {
+    const std::vector<uint8_t> cs = extract_codestream(data, size);
+    const FrameIndex index = index_frames(cs.data(), cs.size());
+    if (num_keyframes) *num_keyframes = int32_t(index.num_keyframes);
+    if (num_segments) *num_segments = int32_t(index.segments.size());
+    return index.error;
+  } catch (const Error& e) {
+    return e.code;
+  } catch (const std::exception&) {
+    return JXLB_ERR_INVALID_ARG;
+  }
+}
+
+int32_t jxlb_decode_keyframe(jxlb_decoder* dec, const uint8_t* data, size_t size, const jxlb_options* opt, int32_t keyframe) {
+  if (!dec || !data || keyframe < 0) return JXLB_ERR_INVALID_ARG;
+  FrameIndex index;
+  const int32_t rc = guarded(dec, [&] {
+    release(dec);
+    dec->codestream = extract_codestream(data, size);
+    index = index_frames(dec->codestream.data(), dec->codestream.size());
+    JXLB_CHECK(uint32_t(keyframe) < index.num_keyframes, kErrInvalidArg, "keyframe index out of range");
+  });
+  if (rc != JXLB_OK) return rc;
+  return decode_segment_keyframes(dec, dec->codestream.data(), dec->codestream.size(), nullptr, index,
+                                  index.segment_of(uint32_t(keyframe)), uint32_t(keyframe), opt, true,
+                                  [](uint32_t) { return JXLB_OK; });
 }
 
 int32_t jxlb_preload(jxlb_decoder* dec, int32_t slot, const uint8_t* data, size_t size) {

@@ -1272,40 +1272,42 @@ StreamLayout stream_layout(const ImageHeader& ih, const DecodedFrame& f) {
   return l;
 }
 
-DecodeResult decode_codestream(Backend& be, const uint8_t* cs, size_t size, const DecodeOptions& opt) {
-  DecodeResult res;
-  be.set_codestream(cs, size);
+size_t parse_codestream_header(const uint8_t* cs, size_t size, ImageHeader* out) {
   BitReader br(cs, size);
-  res.image_header = parse_image_header(br);
-  const ImageHeader& ih = res.image_header;
+  *out = parse_image_header(br);
+  ImageHeader& ih = *out;
   if (ih.colour_encoding.want_icc) {  // jxl-oxide/src/lib.rs:365-372, jxl-render/src/lib.rs:100-150
-    ImageHeader& mih = res.image_header;
-    mih.icc_profile = decode_icc_stream(read_icc_stream(br));
+    ih.icc_profile = decode_icc_stream(read_icc_stream(br));
     IccInfo info;
-    const IccStatus st = icc_to_enum(mih.icc_profile, &info);
-    const bool header_gray = mih.colour_encoding.colour_space == ColourSpace::kGrey;
+    const IccStatus st = icc_to_enum(ih.icc_profile, &info);
+    const bool header_gray = ih.colour_encoding.colour_space == ColourSpace::kGrey;
     if (st != IccStatus::kMalformed)
       JXLB_CHECK(header_gray == info.is_gray, kErrBitstream, "colour channel mismatch between header and ICC profile");
-    mih.icc_is_enum = st == IccStatus::kEnum;
-    mih.icc_is_cmyk = st != IccStatus::kMalformed && info.is_cmyk;
-    if (mih.icc_is_enum) {
-      mih.icc_encoding = info.encoding;
+    ih.icc_is_enum = st == IccStatus::kEnum;
+    ih.icc_is_cmyk = st != IccStatus::kMalformed && info.is_cmyk;
+    if (ih.icc_is_enum) {
+      ih.icc_encoding = info.encoding;
     } else {  // EnumColourEncoding::{gray_srgb, srgb}
-      mih.icc_encoding = ColourEncoding();
-      if (header_gray) mih.icc_encoding.colour_space = ColourSpace::kGrey;
+      ih.icc_encoding = ColourEncoding();
+      if (header_gray) ih.icc_encoding.colour_space = ColourSpace::kGrey;
     }
   }
   br.zero_pad_to_byte();
-  size_t pos = br.pos() / 8;
+  const size_t pos = br.pos() / 8;
   if (ih.have_preview) {  // skipped, like jxl-oxide/src/lib.rs:384-411
     BitReader pr(cs, size, pos * 8);
     FrameHeader pfh = parse_frame_header(pr, ih);
     (void)pfh;
     fail(kErrUnsupported, "preview frames are not supported");
   }
+  return pos;
+}
+
+void decode_frames(Backend& be, const uint8_t* cs, size_t size, const ImageHeader& ih, const DecodeOptions& opt, size_t pos,
+                   uint64_t visible_frames, uint64_t invisible_frames, uint32_t max_shown,
+                   const std::function<void(DecodedFrame&&)>& sink) {
   LfFrameStore lf_store[4];
   RefFrameStore ref_store[4];
-  uint64_t visible_frames = 0, invisible_frames = 0;
   auto drop_lf_frames = [&] {
     for (LfFrameStore& s : lf_store)
       if (s.valid)
@@ -1314,8 +1316,9 @@ DecodeResult decode_codestream(Backend& be, const uint8_t* cs, size_t size, cons
       if (s.valid)
         for (const View& v : s.channels) be.free_plane(v.plane);
   };
+  uint32_t shown = 0;
   try {
-    while (pos < size && res.frames.size() < opt.max_frames) {
+    while (pos < size && shown < max_shown) {
       FramePlanner planner(be, cs, size, ih, opt, &lf_store, &ref_store, visible_frames, invisible_frames);
       size_t end = 0;
       DecodedFrame f = planner.decode_frame(pos, &end);
@@ -1327,20 +1330,33 @@ DecodeResult decode_codestream(Backend& be, const uint8_t* cs, size_t size, cons
           for (const View& v : f.channels) be.free_plane(v.plane);
         ++invisible_frames;
       } else {
-        res.frames.push_back(std::move(f));
+        ++shown;
         ++visible_frames;
         invisible_frames = 0;
+        sink(std::move(f));
       }
       pos = end;
       if (last) break;
     }
   } catch (...) {
     drop_lf_frames();
+    throw;
+  }
+  drop_lf_frames();
+}
+
+DecodeResult decode_codestream(Backend& be, const uint8_t* cs, size_t size, const DecodeOptions& opt) {
+  DecodeResult res;
+  be.set_codestream(cs, size);
+  const size_t pos = parse_codestream_header(cs, size, &res.image_header);
+  try {
+    decode_frames(be, cs, size, res.image_header, opt, pos, 0, 0, opt.max_frames,
+                  [&](DecodedFrame&& f) { res.frames.push_back(std::move(f)); });
+  } catch (...) {
     for (DecodedFrame& f : res.frames)  // frames finished before the failing one
       for (const View& v : f.channels) be.free_plane(v.plane);
     throw;
   }
-  drop_lf_frames();
   return res;
 }
 

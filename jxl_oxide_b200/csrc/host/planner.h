@@ -5,6 +5,7 @@
 // lib.rs:925-998). It never touches a sample itself.
 #pragma once
 #include <cstdint>
+#include <functional>
 #include <string>
 #include <vector>
 
@@ -54,5 +55,15 @@ std::vector<uint8_t> extract_codestream(const uint8_t* data, size_t size);
 // Decodes every keyframe of `codestream` (bare) through `be`. Planes referenced by the result
 // stay alive in the backend until the caller frees them.
 DecodeResult decode_codestream(Backend& be, const uint8_t* codestream, size_t size, const DecodeOptions& opt);
+
+// The two halves of decode_codestream. parse_codestream_header reads the image header and ICC profile and returns the
+// byte offset of the first frame. decode_frames decodes the frames from byte `begin` on, as if `visible_before` shown
+// and `invisible_before` hidden frames had come before and left every reference slot and LF store empty; each shown
+// frame goes to `sink` as soon as it is finished (the sink owns its planes), up to `max_shown` of them. The stores are
+// freed when it returns or throws. The caller has called be.set_codestream().
+size_t parse_codestream_header(const uint8_t* codestream, size_t size, ImageHeader* ih);
+void decode_frames(Backend& be, const uint8_t* codestream, size_t size, const ImageHeader& ih, const DecodeOptions& opt,
+                   size_t begin, uint64_t visible_before, uint64_t invisible_before, uint32_t max_shown,
+                   const std::function<void(DecodedFrame&&)>& sink);
 
 }  // namespace jxlb

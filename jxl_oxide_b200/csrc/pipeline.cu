@@ -30,7 +30,21 @@ using namespace jxlb;
 
 namespace {
 
+struct Resident {
+  std::vector<uint8_t> codestream;
+  uint8_t* dptr = nullptr;
+};
+
+// One jxlb_pipeline_submit_keyframes call, shared by the tasks of its segments.
+struct KeyframeSubmission {
+  std::vector<uint8_t> codestream;    // the bare codestream of host bytes
+  const Resident* resident = nullptr;  // or the preloaded slot's
+  FrameIndex index;
+};
+
 struct Job {
+  std::shared_ptr<const KeyframeSubmission> keyframes;  // a segment task of a keyframe submission
+  size_t segment = 0;
   const uint8_t* data = nullptr;  // host bytes (caller keeps them alive until the job is reported done) or
   size_t size = 0;
   int32_t slot = -1;              // a preloaded slot
@@ -46,17 +60,13 @@ struct Done {
   std::string error;
   void* out = nullptr;  // pipeline-owned pinned buffer (jobs submitted with dst == NULL), else the job's dst
   size_t out_bytes = 0;
+  int32_t keyframe = -1;  // the keyframe of a keyframe submission
 };
 
 struct HostBuf {  // pinned staging owned by the pipeline: allocated by a worker thread (NUMA-local to the GPU)
   void* p = nullptr;
   size_t bytes = 0;
   bool busy = false;
-};
-
-struct Resident {
-  std::vector<uint8_t> codestream;
-  uint8_t* dptr = nullptr;
 };
 
 struct Slab {  // a heavy slot: HBM for a frame's full-resolution planes + the CUDA stream its kernels run on
@@ -477,6 +487,19 @@ struct jxlb_pipeline {
       dec->be->set_stream(slabs[size_t(held)].stream);
     };
     dec->be->lf_service = batcher.get();
+    auto finish_job = [&] {
+      jxlb_release_frames(dec);
+      if (held >= 0) {
+        dec->be->end_arena();
+        try {
+          dec->be->end_lease();
+        } catch (const Error&) {
+        }
+        release_slab(held);
+        held = -1;
+        if (profiled()) add_ms("host:slot_hold", granted, std::chrono::steady_clock::now());
+      }
+    };
     for (;;) {
       Job job;
       {
@@ -485,6 +508,11 @@ struct jxlb_pipeline {
         if (queue.empty()) return;
         job = queue.front();
         queue.pop_front();
+      }
+      if (job.keyframes) {
+        run_segment(dec, job);
+        finish_job();
+        continue;
       }
       Done d{job.tag, JXLB_OK, std::string()};
       int32_t rc;
@@ -504,69 +532,100 @@ struct jxlb_pipeline {
           rc = decode_resident(dec, r->codestream.data(), r->codestream.size(), r->dptr, nullptr);
         }
       }
-      if (rc == JXLB_OK && (job.out_mode == 4 || job.out_mode == 5)) {
-        // packed straight into the caller's device buffer (input of an NCCL gather): no host link involved
-        rc = jxlb_frame_write_to_device(dec, 0, job.out_mode - 4, 0, job.dst, job.dst_bytes);
-        d.out = job.dst;
-        d.out_bytes = job.dst_bytes;
-      } else if (rc == JXLB_OK && job.out_mode != 0) {
-        void* dst = job.dst;
-        size_t dst_bytes = job.dst_bytes;
-        if (!dst) {  // library-owned pinned staging, sized from the decoded frame
-          jxlb_frame_info fi;
-          jxlb_frame_get_info(dec, 0, &fi);
-          if (job.out_mode == 1) {
-            dst_bytes = 0;
-            for (const View& v : dec->res.frames[0].channels) dst_bytes += size_t(v.w) * v.h * 4;
-          } else {
-            dst_bytes = size_t(fi.width) * fi.height * size_t(jxlb_frame_stream_channels(dec, 0)) * (job.out_mode == 2 ? 1 : 2);
-          }
-          dst = acquire_host(dst_bytes);
-          if (!dst) {
-            rc = JXLB_ERR_CUDA;
-            dec->error = "cannot allocate pinned host memory for the frame output";
-          }
-        }
-        if (rc == JXLB_OK) {
-          // Device -> host copies of different streams share the copy engines chunk by chunk; a dozen 400 MB copies
-          // in flight together were measured slower in total than one at a time. The decode work of the
-          // other frames goes on meanwhile; only the copies queue up.
-          rc = jxlb_sync(dec);
-          std::lock_guard<std::mutex> copy_lock(copy_mu);
-          if (rc != JXLB_OK) {
-          } else if (job.out_mode == 1) rc = frame_planar_to_host(dec, 0, static_cast<float*>(dst), dst_bytes);
-          else rc = jxlb_frame_write_to_buffer(dec, 0, job.out_mode - 2, 0, dst, dst_bytes);
-          d.out = dst;
-          d.out_bytes = dst_bytes;
-          if (rc != JXLB_OK && !job.dst) {
-            release_host(dst);
-            d.out = nullptr;
-          }
-        }
-      } else if (rc == JXLB_OK) {
-        rc = jxlb_sync(dec);
-      }
+      if (rc == JXLB_OK) rc = deliver(dec, job.out_mode, job.dst, job.dst_bytes, d);
       if (rc != JXLB_OK) {
         d.status = rc;
         d.error = dec->error;
         jxlb_sync(dec);
       }
-      jxlb_release_frames(dec);
-      if (held >= 0) {
-        dec->be->end_arena();
-        try {
-          dec->be->end_lease();
-        } catch (const Error&) {
+      finish_job();
+      report(std::move(d));
+    }
+  }
+
+  void report(Done&& d) {
+    {
+      std::lock_guard<std::mutex> lk(mu);
+      done.push_back(std::move(d));
+    }
+    cv_done.notify_all();
+  }
+
+  // Packs frame 0 of `dec` as `out_mode` asks into `dst` (NULL: a buffer of the ring) and records in `d` where it went.
+  int32_t deliver(jxlb_decoder* dec, int32_t out_mode, void* dst, size_t dst_bytes, Done& d) {
+    int32_t rc = JXLB_OK;
+    const bool own = !dst;
+    if (out_mode == 4 || out_mode == 5) {
+      // packed straight into the caller's device buffer (input of an NCCL gather): no host link involved
+      rc = jxlb_frame_write_to_device(dec, 0, out_mode - 4, 0, dst, dst_bytes);
+      d.out = dst;
+      d.out_bytes = dst_bytes;
+    } else if (out_mode != 0) {
+      if (!dst) {  // library-owned pinned staging, sized from the decoded frame
+        jxlb_frame_info fi;
+        jxlb_frame_get_info(dec, 0, &fi);
+        if (out_mode == 1) {
+          dst_bytes = 0;
+          for (const View& v : dec->res.frames[0].channels) dst_bytes += size_t(v.w) * v.h * 4;
+        } else {
+          dst_bytes = size_t(fi.width) * fi.height * size_t(jxlb_frame_stream_channels(dec, 0)) * (out_mode == 2 ? 1 : 2);
         }
-        release_slab(held);
-        held = -1;
-        if (profiled()) add_ms("host:slot_hold", granted, std::chrono::steady_clock::now());
+        dst = acquire_host(dst_bytes);
+        if (!dst) {
+          rc = JXLB_ERR_CUDA;
+          dec->error = "cannot allocate pinned host memory for the frame output";
+        }
       }
-      {
-        std::lock_guard<std::mutex> lk(mu);
-        done.push_back(std::move(d));
+      if (rc == JXLB_OK) {
+        // Device -> host copies of different streams share the copy engines chunk by chunk; a dozen 400 MB copies
+        // in flight together were measured slower in total than one at a time. The decode work of the
+        // other frames goes on meanwhile; only the copies queue up.
+        rc = jxlb_sync(dec);
+        std::lock_guard<std::mutex> copy_lock(copy_mu);
+        if (rc != JXLB_OK) {
+        } else if (out_mode == 1) rc = frame_planar_to_host(dec, 0, static_cast<float*>(dst), dst_bytes);
+        else rc = jxlb_frame_write_to_buffer(dec, 0, out_mode - 2, 0, dst, dst_bytes);
+        d.out = dst;
+        d.out_bytes = dst_bytes;
+        if (rc != JXLB_OK && own) {
+          release_host(dst);
+          d.out = nullptr;
+        }
       }
-      cv_done.notify_all();
+    } else {
+      rc = jxlb_sync(dec);
+    }
+    return rc;
+  }
+
+  // A segment task: its keyframes are reported one by one as they are packed. The task keeps the heavy slot its first
+  // frame takes until the segment ends (later frames share it, as the frames of one image do).
+  void run_segment(jxlb_decoder* dec, const Job& job) {
+    const KeyframeSubmission& ks = *job.keyframes;
+    const FrameSegment& seg = ks.index.segments[job.segment];
+    const std::vector<uint8_t>& cs = ks.resident ? ks.resident->codestream : ks.codestream;
+    const size_t per_keyframe = job.dst ? job.dst_bytes / ks.index.num_keyframes : 0;
+    uint32_t next = seg.keyframes.front();
+    const int32_t rc = decode_segment_keyframes(
+        dec, cs.data(), cs.size(), ks.resident ? ks.resident->dptr : nullptr, ks.index, job.segment, seg.keyframes.back(), nullptr,
+        false, [&](uint32_t k) {
+          Done d{job.tag, JXLB_OK, std::string()};
+          d.keyframe = int32_t(k);
+          void* dst = job.dst ? static_cast<uint8_t*>(job.dst) + size_t(k) * per_keyframe : nullptr;
+          const int32_t r = deliver(dec, job.out_mode, dst, per_keyframe, d);
+          if (r == JXLB_OK) {
+            report(std::move(d));
+            next = k + 1;
+          }
+          return r;
+        });
+    if (rc == JXLB_OK) return;
+    const std::string error = dec->error;
+    jxlb_sync(dec);
+    for (uint32_t k = next; k <= seg.keyframes.back(); ++k) {  // the failing keyframe and the ones after it
+      Done d{job.tag, rc, error};
+      d.keyframe = int32_t(k);
+      report(std::move(d));
     }
   }
 };
@@ -672,8 +731,54 @@ int32_t jxlb_pipeline_submit(jxlb_pipeline* p, const uint8_t* data, size_t size,
   return JXLB_OK;
 }
 
-int32_t jxlb_pipeline_wait(jxlb_pipeline* p, uint64_t* tag, int32_t* status, void** out, size_t* out_bytes, char* err,
-                           size_t err_cap) {
+int32_t jxlb_pipeline_submit_keyframes(jxlb_pipeline* p, const uint8_t* data, size_t size, int32_t slot, int32_t out_mode,
+                                       void* dst, size_t dst_bytes, uint64_t tag) {
+  if (!p || out_mode < 0 || out_mode > 5 || (!data && slot < 0) || (out_mode >= 4 && !dst)) return JXLB_ERR_INVALID_ARG;
+  auto ks = std::make_shared<KeyframeSubmission>();
+  Done fail_all{tag, JXLB_OK, std::string()};
+  try {
+    if (data) {
+      ks->codestream = extract_codestream(data, size);
+    } else {
+      std::lock_guard<std::mutex> lk(p->mu);
+      auto it = p->resident.find(slot);
+      JXLB_CHECK(it != p->resident.end(), kErrInvalidArg, "unknown preload slot");
+      ks->resident = &it->second;
+    }
+    const std::vector<uint8_t>& cs = ks->resident ? ks->resident->codestream : ks->codestream;
+    ks->index = index_frames(cs.data(), cs.size());
+  } catch (const Error& e) {  // not even the image header: one report, on keyframe 0
+    fail_all.status = e.code;
+    fail_all.error = e.what();
+    fail_all.keyframe = 0;
+  }
+  {
+    std::lock_guard<std::mutex> lk(p->mu);
+    if (p->stopping) return JXLB_ERR_INVALID_ARG;
+    if (fail_all.status != JXLB_OK) {
+      p->done.push_back(fail_all);
+      ++p->submitted;
+    } else {
+      for (size_t s = 0; s < ks->index.segments.size(); ++s) {
+        Job j;
+        j.keyframes = ks;
+        j.segment = s;
+        j.out_mode = out_mode;
+        j.dst = dst;
+        j.dst_bytes = dst_bytes;
+        j.tag = tag;
+        p->queue.push_back(j);
+      }
+      p->submitted += ks->index.num_keyframes;
+    }
+  }
+  if (fail_all.status != JXLB_OK) p->cv_done.notify_all();
+  else p->cv_job.notify_all();
+  return JXLB_OK;
+}
+
+int32_t jxlb_pipeline_wait_keyframe(jxlb_pipeline* p, uint64_t* tag, int32_t* keyframe, int32_t* status, void** out,
+                                    size_t* out_bytes, char* err, size_t err_cap) {
   if (!p || !tag || !status) return JXLB_ERR_INVALID_ARG;
   std::unique_lock<std::mutex> lk(p->mu);
   if (p->reported == p->submitted) return JXLB_ERR_INVALID_ARG;  // nothing in flight
@@ -683,10 +788,16 @@ int32_t jxlb_pipeline_wait(jxlb_pipeline* p, uint64_t* tag, int32_t* status, voi
   ++p->reported;
   *tag = d.tag;
   *status = d.status;
+  if (keyframe) *keyframe = d.keyframe;
   if (out) *out = d.out;
   if (out_bytes) *out_bytes = d.out_bytes;
   if (err && err_cap) std::snprintf(err, err_cap, "%s", d.error.c_str());
   return JXLB_OK;
+}
+
+int32_t jxlb_pipeline_wait(jxlb_pipeline* p, uint64_t* tag, int32_t* status, void** out, size_t* out_bytes, char* err,
+                           size_t err_cap) {
+  return jxlb_pipeline_wait_keyframe(p, tag, nullptr, status, out, out_bytes, err, err_cap);
 }
 
 int32_t jxlb_pipeline_release_output(jxlb_pipeline* p, void* out) {
