@@ -1064,14 +1064,21 @@ void CudaBackend::splat_splines(const View v[3], const std::vector<SplineArc>& a
 
 void CudaBackend::add_noise(const View v[3], const float lut[8], uint32_t group_dim, uint64_t seed0, float corr_x,
                             float corr_b) {
-  JXLB_CHECK(v[0].w >= 2 && v[0].h >= 2, kErrUnsupported, "noise on frames narrower than 2 samples is not supported");
+  add_noise_in_frame(v, v[0].w, v[0].h, lut, group_dim, seed0, corr_x, corr_b);
+}
+
+void CudaBackend::add_noise_in_frame(const View v[3], uint32_t field_w, uint32_t field_h, const float lut[8],
+                                     uint32_t group_dim, uint64_t seed0, float corr_x, float corr_b) {
+  // the 5x5 high-pass mirrors over the field, which needs two samples in each direction
+  JXLB_CHECK(field_w >= 2 && field_h >= 2, kErrUnsupported, "noise on frames narrower than 2 samples is not supported");
   DevView dv[3];
   float* field[3];
   for (int c = 0; c < 3; ++c) {
     JXLB_CHECK(v[c].w == v[0].w && v[c].h == v[0].h, kErrInvalidArg, "noise needs three equally sized planes");
+    JXLB_CHECK(v[c].w <= field_w && v[c].h <= field_h, kErrInvalidArg, "noise view larger than its field");
     dv[c] = dev_view(v[c]);
-    field[c] = static_cast<float*>(dmalloc(size_t(v[0].w) * v[0].h * 4));
   }
+  for (int c = 0; c < 3; ++c) field[c] = static_cast<float*>(dmalloc(size_t(field_w) * field_h * 4));
   DevNoiseParams p;
   for (int i = 0; i < 8; ++i) p.lut[i] = lut[i];
   p.lut[8] = lut[7];
@@ -1080,7 +1087,7 @@ void CudaBackend::add_noise(const View v[3], const float lut[8], uint32_t group_
   p.group_dim = group_dim;
   p.seed0 = seed0;
   begin_k("add_noise");
-  launch_add_noise(dv, field, p, S());
+  launch_add_noise(dv, field, field_w, field_h, p, S());
   end_k();
   for (int c = 0; c < 3; ++c) dfree(field[c]);
 }

@@ -81,6 +81,8 @@ class CudaBackend : public Backend, private TableSink {
   void blend_raw(const DevPatchJob& job);  // one rectangle on caller-owned device memory (jxlb_blend)
   void splat_splines(const View v[3], const std::vector<SplineArc>& arcs) override;
   void add_noise(const View v[3], const float lut[8], uint32_t group_dim, uint64_t seed0, float corr_x, float corr_b) override;
+  void add_noise_in_frame(const View v[3], uint32_t field_w, uint32_t field_h, const float lut[8], uint32_t group_dim,
+                          uint64_t seed0, float corr_x, float corr_b) override;
   void xyb_to_rgb(const View v[3], const ColorParams& p) override;
   void ycbcr_to_rgb(const View v[3], const YcbcrParams& p) override;
   bool filters_colour_fused(const View v[3], const RestorationFilter& rf, const View& sigma, bool sigma_is_constant,

@@ -222,6 +222,11 @@ class Backend {
   // from `lut`, added to the XYB planes `v` (frame_w x frame_h).
   virtual void add_noise(const View v[3], const float lut[8], uint32_t group_dim, uint64_t seed0, float corr_x,
                          float corr_b) = 0;
+  // The same with the field (its groups, seeds and mirroring) generated over field_w x field_h, of which the
+  // top-left v[0].w x v[0].h part is added to `v`: an upsampled frame takes its noise at the coded resolution from the
+  // field of the upsampled size (noise.rs:21-33, 94-100). The default runs add_noise() over field-sized copies of `v`.
+  virtual void add_noise_in_frame(const View v[3], uint32_t field_w, uint32_t field_h, const float lut[8], uint32_t group_dim,
+                                  uint64_t seed0, float corr_x, float corr_b);
   virtual void xyb_to_rgb(const View v[3], const ColorParams& p) = 0;
   // YCbCr -> RGB of JPEG-transcoded frames, planes in Cb, Y, Cr order (jxl-color/src/ycbcr.rs:40-56)
   struct YcbcrParams {

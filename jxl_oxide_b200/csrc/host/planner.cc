@@ -540,6 +540,8 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
   size_t ec_render_bytes = 0;
   for (size_t i = 0; i < ih_.ec_info.size(); ++i)
     if (ec_shift(i)) ec_render_bytes += size_t(fh_.width) * fh_.height * 4 + size_t(fh_.width) * fh_.height;
+  // noise on an upsampled frame: its three f32 field planes have the upsampled size
+  if (lfg_.has_noise && fh_.upsampling > 1) ec_render_bytes += size_t(fh_.width) * fh_.height * 4 * 3;
   if (lfg_.has_gmodular) {
     // a Modular image allocates its full-size channels up front (coded channels, then one plane per inverse transform)
     if (!vardct)
@@ -867,7 +869,37 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
     frame_planes_.push_back(id);
     v = View{id, 0, 0, std::min(v.w << factor_log2, fh_.width), std::min(v.h << factor_log2, fh_.height)};
   };
+  // render_features (jxl-render/src/render.rs:136-225) runs on the grid before it is upsampled: splines and noise land on
+  // the colour channels at the coded resolution, in frame coordinates (the upsampled size) clipped to the coded planes.
+  // Patches are blended below, after upsampling, while the reference blends them on the coded colour channels
+  // (render.rs:182-196 brings only the extra channels to the colour resolution), so an upsampled frame with patches and
+  // splines or noise is refused rather than drawn in the wrong order.
+  auto splines_and_noise = [&]() {
+    if (lfg_.has_splines) {
+      JXLB_CHECK(colour.size() == 3, kErrUnsupported, "splines need three colour channels");
+      const std::vector<Backend::SplineArc> arcs =
+          build_spline_arcs(lfg_, vardct, vardct ? lfg_.base_correlation_x : 0.0f, vardct ? lfg_.base_correlation_b : 1.0f, fh_.width, fh_.height);
+      View v[3] = {colour[0], colour[1], colour[2]};
+      be_.splat_splines(v, arcs);
+      be_.stage_marker("splines", v, 3);
+    }
+    if (lfg_.has_noise) {
+      JXLB_CHECK(colour.size() == 3 && ih_.xyb_encoded, kErrUnsupported, "noise synthesis is implemented for XYB colour frames");
+      View v[3] = {colour[0], colour[1], colour[2]};
+      const float corr_x = vardct ? lfg_.base_correlation_x : 0.0f, corr_b = vardct ? lfg_.base_correlation_b : 1.0f;
+      // a shown frame counts itself among the visible ones; a hidden one among the invisible ones
+      const bool shown = !is_lf_frame && !is_ref_frame;
+      const uint64_t seed0 = shown ? ((visible_before_ + 1) << 32) : (visible_before_ << 32) + invisible_before_ + 1;
+      // the field has the frame's size (noise.rs:94-100): the upsampled size, or the planes' own without upsampling
+      if (upsampled) be_.add_noise_in_frame(v, fh_.width, fh_.height, lfg_.noise_lut, fh_.group_dim(), seed0, corr_x, corr_b);
+      else be_.add_noise(v, lfg_.noise_lut, fh_.group_dim(), seed0, corr_x, corr_b);
+      be_.stage_marker("noise", v, 3);
+    }
+  };
   if (upsampled) {
+    JXLB_CHECK(!lfg_.has_patches || !(lfg_.has_splines || lfg_.has_noise), kErrUnsupported,
+               "splines or noise together with patches on an upsampled frame are not implemented");
+    splines_and_noise();
     for (View& v : colour) upsample_view(v, ceil_log2_nonzero(fh_.upsampling));
     out.width = fh_.width;
     out.height = fh_.height;
@@ -887,7 +919,7 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
     extra.push_back(v);
   }
   if (extra_upsampled) be_.stage_marker("extra_upsampled", extra.data(), int(extra.size()));
-  // render_features (jxl-render/src/render.rs:159-225): patches, (splines,) noise - after upsampling, before colour
+  // patches (render.rs:182-196) on the upsampled grid, then splines and noise of a frame that is not upsampled
   if (lfg_.has_patches) {
     std::vector<View> all = colour;
     all.insert(all.end(), extra.begin(), extra.end());
@@ -946,28 +978,7 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
     be_.blend_patches(jobs);
     be_.stage_marker("patches", colour.data(), int(colour.size()));
   }
-  if (lfg_.has_splines) {
-    JXLB_CHECK(colour.size() == 3, kErrUnsupported, "splines need three colour channels");
-    // the reference draws splines on the grid as it stands after patches (render.rs:182-205); with upsampling and no
-    // patches that is the pre-upsampling grid - not restated here
-    JXLB_CHECK(!upsampled, kErrUnsupported, "splines together with upsampling are not implemented");
-    const std::vector<Backend::SplineArc> arcs =
-        build_spline_arcs(lfg_, vardct, vardct ? lfg_.base_correlation_x : 0.0f, vardct ? lfg_.base_correlation_b : 1.0f, fh_.width, fh_.height);
-    View v[3] = {colour[0], colour[1], colour[2]};
-    be_.splat_splines(v, arcs);
-    be_.stage_marker("splines", v, 3);
-  }
-  if (lfg_.has_noise) {
-    JXLB_CHECK(colour.size() == 3 && ih_.xyb_encoded, kErrUnsupported, "noise synthesis is implemented for XYB colour frames");
-    JXLB_CHECK(!upsampled, kErrUnsupported, "noise synthesis together with upsampling is not implemented");
-    View v[3] = {colour[0], colour[1], colour[2]};
-    const float corr_x = vardct ? lfg_.base_correlation_x : 0.0f, corr_b = vardct ? lfg_.base_correlation_b : 1.0f;
-    // a shown frame counts itself among the visible ones; a hidden one among the invisible ones
-    const bool shown = !is_lf_frame && !is_ref_frame;
-    const uint64_t seed0 = shown ? ((visible_before_ + 1) << 32) : (visible_before_ << 32) + invisible_before_ + 1;
-    be_.add_noise(v, lfg_.noise_lut, fh_.group_dim(), seed0, corr_x, corr_b);
-    be_.stage_marker("noise", v, 3);
-  }
+  if (!upsampled) splines_and_noise();
   if (fh_.do_ycbcr && !colour_done) {  // jxl-render/src/lib.rs:950-954, util.rs:320-329
     JXLB_CHECK(colour.size() == 3, kErrBitstream, "YCbCr needs three channels");
     View v[3] = {colour[0], colour[1], colour[2]};
@@ -1301,6 +1312,24 @@ size_t parse_codestream_header(const uint8_t* cs, size_t size, ImageHeader* out)
     fail(kErrUnsupported, "preview frames are not supported");
   }
   return pos;
+}
+
+void Backend::add_noise_in_frame(const View v[3], uint32_t field_w, uint32_t field_h, const float lut[8], uint32_t group_dim,
+                                 uint64_t seed0, float corr_x, float corr_b) {
+  if (v[0].w == field_w && v[0].h == field_h) return add_noise(v, lut, group_dim, seed0, corr_x, corr_b);
+  // noise at a sample depends on the field and on the sample itself only: the planes are placed in the top-left corner
+  // of zeroed field-sized ones, which take the noise of the whole field, and copied back
+  View full[3];
+  for (int c = 0; c < 3; ++c) {
+    JXLB_CHECK(v[c].w <= field_w && v[c].h <= field_h, kErrInvalidArg, "noise view larger than its field");
+    full[c] = View{alloc_plane(field_w, field_h, /*zero=*/true), 0, 0, field_w, field_h};
+    copy_rect(v[c], View{full[c].plane, 0, 0, v[c].w, v[c].h});
+  }
+  add_noise(full, lut, group_dim, seed0, corr_x, corr_b);
+  for (int c = 0; c < 3; ++c) {
+    copy_rect(View{full[c].plane, 0, 0, v[c].w, v[c].h}, v[c]);
+    free_plane(full[c].plane);
+  }
 }
 
 void decode_frames(Backend& be, const uint8_t* cs, size_t size, const ImageHeader& ih, const DecodeOptions& opt, size_t pos,

@@ -387,13 +387,14 @@ __global__ void noise_field_kernel(float* f0, float* f1, float* f2, uint32_t wid
   }
 }
 
-// 5x5 high-pass of the field (rows added in the order of the reference's 5-row ring buffer, which depends
-// on the row's position inside its group: noise.rs:297-320) and application to the XYB planes (noise.rs:45-83).
+// 5x5 high-pass of the width x height field (rows added in the order of the reference's 5-row ring buffer, which
+// depends on the row's position inside its group: noise.rs:297-320; mirrored at the field's edges) and application to
+// the XYB planes (noise.rs:45-83), whose view is the field's top-left corner (noise.rs:21-33).
 __global__ void noise_apply_kernel(DevView vx, DevView vy, DevView vb, const float* __restrict__ f0,
-                                   const float* __restrict__ f1, const float* __restrict__ f2, DevNoiseParams p) {
+                                   const float* __restrict__ f1, const float* __restrict__ f2, int width, int height,
+                                   DevNoiseParams p) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
-  const int width = int(vx.w), height = int(vx.h);
-  if (x >= width || y >= height) return;
+  if (x >= int(vx.w) || y >= int(vx.h)) return;
   const int ly = y % int(p.group_dim);
   const float* fields[3] = {f0, f1, f2};
   float n[3];
@@ -446,14 +447,14 @@ void launch_splat_splines(const DevView v[3], const DevSplineArc* arcs, int num_
   splat_splines_kernel<<<grid, block, 0, stream>>>(v[0], v[1], v[2], arcs, num_arcs);
 }
 
-void launch_add_noise(const DevView v[3], float* const field[3], DevNoiseParams p, cudaStream_t stream) {
-  const uint32_t width = v[0].w, height = v[0].h;
-  if (!width || !height) return;
-  const uint32_t groups = ((width + p.group_dim - 1) / p.group_dim) * ((height + p.group_dim - 1) / p.group_dim);
-  noise_field_kernel<<<(groups * 8 + 63) / 64, 64, 0, stream>>>(field[0], field[1], field[2], width, height, p.group_dim, p.seed0);
+void launch_add_noise(const DevView v[3], float* const field[3], uint32_t field_w, uint32_t field_h, DevNoiseParams p,
+                      cudaStream_t stream) {
+  if (!v[0].w || !v[0].h) return;
+  const uint32_t groups = ((field_w + p.group_dim - 1) / p.group_dim) * ((field_h + p.group_dim - 1) / p.group_dim);
+  noise_field_kernel<<<(groups * 8 + 63) / 64, 64, 0, stream>>>(field[0], field[1], field[2], field_w, field_h, p.group_dim, p.seed0);
   dim3 block(32, 8);
-  dim3 grid((width + 31) / 32, (height + 7) / 8);
-  noise_apply_kernel<<<grid, block, 0, stream>>>(v[0], v[1], v[2], field[0], field[1], field[2], p);
+  dim3 grid((v[0].w + 31) / 32, (v[0].h + 7) / 8);
+  noise_apply_kernel<<<grid, block, 0, stream>>>(v[0], v[1], v[2], field[0], field[1], field[2], int(field_w), int(field_h), p);
 }
 
 void launch_pack_interleaved(DevPackParams p, void* out, cudaStream_t stream) {

@@ -279,7 +279,10 @@ struct DevNoiseParams {
   uint32_t group_dim;
   unsigned long long seed0;
 };
-void launch_add_noise(const DevView v[3], float* const field[3], DevNoiseParams p, cudaStream_t stream);
+// `field` holds three field_w x field_h planes (the frame size); noise is added over the views, which lie in the field's
+// top-left corner.
+void launch_add_noise(const DevView v[3], float* const field[3], uint32_t field_w, uint32_t field_h, DevNoiseParams p,
+                      cudaStream_t stream);
 // Gaborish -> EPF -> colour in one kernel (kernels/filters_fused.cu); `in` and `out` must not alias.
 struct DevFusedFilterParams {
   int gab_enabled;

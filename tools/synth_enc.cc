@@ -20,7 +20,9 @@
 // --hf-lz77 rle|match codes the HF passes with LZ77 (HfLz77 below); everything else is written as without it, and the
 // number of values the decoder takes from copies goes to stderr. --extra TYPE:BITS:DIM_SHIFT:EC_UPSAMPLING (repeatable)
 // adds extra channels at their coded sizes to a VarDCT or --modular frame; --ycbcr and --upsampling make --modular frames
-// with chroma-subsampled Cb, Y, Cr or a reduced colour resolution (encode_channels).
+// with chroma-subsampled Cb, Y, Cr or a reduced colour resolution (encode_channels). --upsampling K also codes a VarDCT
+// frame at ceil(W / K) x ceil(H / K), and --noise / --noise-zero, --splines N and --dangling-patch give a VarDCT frame
+// those LfGlobal features (write_features).
 //
 // Not part of the product; not a general-purpose encoder (it does not transform an input image).
 #include <algorithm>
@@ -786,7 +788,13 @@ struct Args {
   // Channels coded below the frame's resolution: a --modular frame with any of these is written without transforms,
   // from seeded integer samples at each channel's coded size (encode_channels); --extra also goes with VarDCT frames
   std::string ycbcr;       // --ycbcr 444 | 420 | 422 | 440: Cb, Y, Cr colour channels with that chroma subsampling
-  uint32_t upsampling = 1; // --upsampling 1 | 2 | 4 | 8: the frame's colour upsampling
+  uint32_t upsampling = 1; // --upsampling 1 | 2 | 4 | 8: the frame's colour upsampling (a VarDCT frame is coded at
+                           // ceil(W / k) x ceil(H / k))
+  // LfGlobal features of a VarDCT frame, drawn from generators of their own (the frame's other draws stay as without them)
+  enum { kNoNoise, kSeededNoise, kZeroNoise } noise = kNoNoise;  // --noise / --noise-zero: noise parameters, seeded or all-zero LUT
+  uint32_t splines = 0;    // --splines N: N seeded splines in frame coordinates (write_features)
+  bool dangling_patch = false;  // --dangling-patch: one patch from reference slot 0, which no frame fills (a frame a
+                                // decoder refuses, for tests of which check refuses it first)
   struct Extra {
     uint32_t type, bits, dim_shift, ec_upsampling;  // type: 0 alpha, 2 spot colour, 16 optional (unknown to renderers)
   };
@@ -799,6 +807,68 @@ struct Args {
     return false;
   }
 };
+
+// The LfGlobal feature fields a VarDCT frame has before its LF dequantisation (lf_global.rs:60-105): splines, then noise.
+// Spline i starts at a seeded point of the W x H frame: every even one in its top-left eighth (inside the coded-size
+// planes of an upsampled frame, whatever its factor), every odd one in its right half (past them). Each has 1-3 further
+// control points inside the frame. The splines depend on the
+// seed and the frame size only. Their colour DCTs have a few low-frequency coefficients, their sigma DCT a positive DC of
+// 3-10 quantised units.
+void write_features(BitWriter& w, const Args& a, uint32_t W, uint32_t H) {
+  if (a.dangling_patch) {  // Patches::parse (jxl-frame/src/data/patch.rs): an 8x8 patch at (0, 0), Replace
+    const std::vector<Token> t = {{0, 1}, {1, 0}, {3, 0}, {3, 0}, {2, 7}, {2, 7}, {7, 0}, {4, 0}, {4, 0}, {5, 1}};
+    EntropyEncoder enc;
+    enc.write_header(w, t, 10, std::vector<uint8_t>(10, 0));
+    enc.write_tokens(w, t);
+  }
+  if (a.splines) {  // Splines::parse + QuantSpline::parse (jxl-frame/src/data/spline.rs:18-66, 155-224)
+    std::mt19937 srng(a.seed ^ 0x51ed27a5u);
+    auto pick = [&](uint32_t lo, uint32_t hi) { return int64_t(lo + srng() % (hi - lo)); };  // [lo, hi)
+    std::vector<std::vector<std::pair<int64_t, int64_t>>> pts(a.splines);
+    for (uint32_t i = 0; i < a.splines; ++i) {
+      if (i & 1) pts[i].push_back({W > 1 ? pick((W + 1) / 2, W) : 0, pick(0, H)});
+      else pts[i].push_back({pick(0, (W + 7) / 8), pick(0, (H + 7) / 8)});
+      const uint32_t n = 1 + srng() % 3;
+      while (pts[i].size() <= n) {
+        const std::pair<int64_t, int64_t> p{pick(0, W), pick(0, H)};
+        if (p != pts[i].back()) pts[i].push_back(p);
+        else if (W * H == 1) break;  // a 1 x 1 frame has no second point
+      }
+    }
+    std::vector<Token> t;
+    t.push_back({2, a.splines - 1});
+    t.push_back({1, uint32_t(pts[0][0].first)});
+    t.push_back({1, uint32_t(pts[0][0].second)});
+    for (uint32_t i = 1; i < a.splines; ++i) {
+      t.push_back({1, pack_signed(int32_t(pts[i][0].first - pts[i - 1][0].first))});
+      t.push_back({1, pack_signed(int32_t(pts[i][0].second - pts[i - 1][0].second))});
+    }
+    t.push_back({0, pack_signed(int32_t(srng() % 5) - 2)});  // quant_adjust
+    for (uint32_t i = 0; i < a.splines; ++i) {
+      t.push_back({3, uint32_t(pts[i].size() - 1)});
+      int64_t dx = 0, dy = 0;  // the points are coded as second differences
+      for (size_t k = 1; k < pts[i].size(); ++k) {
+        const int64_t nx = pts[i][k].first - pts[i][k - 1].first, ny = pts[i][k].second - pts[i][k - 1].second;
+        t.push_back({4, pack_signed(int32_t(nx - dx))});
+        t.push_back({4, pack_signed(int32_t(ny - dy))});
+        dx = nx, dy = ny;
+      }
+      for (int c = 0; c < 3; ++c)  // X, Y, B
+        for (int k = 0; k < 32; ++k) {
+          const int32_t range[3] = {40, 12, 12};
+          t.push_back({5, pack_signed(k < 4 ? int32_t(srng() % (2 * range[c] + 1)) - range[c] : 0)});
+        }
+      for (int k = 0; k < 32; ++k) t.push_back({5, pack_signed(k == 0 ? 3 + int32_t(srng() % 8) : (k < 3 ? int32_t(srng() % 3) - 1 : 0))});
+    }
+    EntropyEncoder enc;
+    enc.write_header(w, t, 6, std::vector<uint8_t>(6, 0));
+    enc.write_tokens(w, t);
+  }
+  if (a.noise != Args::kNoNoise) {  // NoiseParameters (jxl-frame/src/data/noise.rs): eight u(10) LUT entries / 1024
+    std::mt19937 nrng(a.seed ^ 0x6e015e00u);
+    for (int i = 0; i < 8; ++i) w.write(10, a.noise == Args::kZeroNoise ? 0 : 64 + nrng() % 512);
+  }
+}
 
 // Varblocks placed before the random layout is drawn (--all-types / --only-type): the transform type at each block's
 // top-left cell, -1 elsewhere. Groups are 32 x 32 cells.
@@ -1333,6 +1403,10 @@ int main(int argc, char** argv) {
     else if (s == "-o") a.out = next();
     else if (s == "--ycbcr") a.ycbcr = next();
     else if (s == "--upsampling") a.upsampling = uint32_t(atoi(next().c_str()));
+    else if (s == "--noise") a.noise = Args::kSeededNoise;
+    else if (s == "--dangling-patch") a.dangling_patch = true;
+    else if (s == "--noise-zero") a.noise = Args::kZeroNoise;
+    else if (s == "--splines") a.splines = uint32_t(std::max(1, atoi(next().c_str())));
     else if (s == "--extra") {
       const std::string spec = next();
       const size_t c1 = spec.find(':');
@@ -1350,7 +1424,11 @@ int main(int argc, char** argv) {
     fprintf(stderr, "--ycbcr takes 444, 420, 422 or 440\n"), exit(2);
   if (a.upsampling != 1 && a.upsampling != 2 && a.upsampling != 4 && a.upsampling != 8)
     fprintf(stderr, "--upsampling takes 1, 2, 4 or 8\n"), exit(2);
-  if ((!a.ycbcr.empty() || a.upsampling != 1) && !a.modular) fprintf(stderr, "--ycbcr and --upsampling make --modular frames\n"), exit(2);
+  if (!a.ycbcr.empty() && !a.modular) fprintf(stderr, "--ycbcr makes --modular frames\n"), exit(2);
+  if ((a.noise != Args::kNoNoise || a.splines || a.dangling_patch) && a.modular)
+    fprintf(stderr, "--noise, --splines and --dangling-patch go with VarDCT frames\n"), exit(2);
+  if (a.upsampling != 1 && !a.modular && (a.lf_frame || !a.extras.empty()))
+    fprintf(stderr, "--upsampling of a VarDCT frame is not written with --lf-frame or --extra\n"), exit(2);
   if (!a.extras.empty() && a.lf_frame) fprintf(stderr, "--extra is not written with --lf-frame\n"), exit(2);
   if (a.modular && a.shifted()) return encode_channels(a);
   const std::string& lzm = a.hf_lz77.mode;
@@ -1361,7 +1439,8 @@ int main(int argc, char** argv) {
     fprintf(stderr, "--only-type takes a transform type 0..26 (not with --all-types)\n"), exit(2);
   std::mt19937 rng(a.seed);
   auto uni = [&](double lo, double hi) { return lo + (hi - lo) * (double(rng()) / 4294967296.0); };
-  const uint32_t W = a.width, H = a.height;
+  // the frame's content at its coded size; the image (and frame) size is width x height
+  const uint32_t up = a.upsampling, W = (a.width + up - 1) / up, H = (a.height + up - 1) / up;
   const uint32_t bw = (W + 7) / 8, bh = (H + 7) / 8;
   const uint32_t gcols = (W + 255) / 256, grows = (H + 255) / 256, num_groups = gcols * grows;
   const uint32_t lcols = (W + 2047) / 2048, lrows = (H + 2047) / 2048, num_lf = lcols * lrows;
@@ -1643,6 +1722,7 @@ int main(int argc, char** argv) {
   std::vector<EntropyEncoder> hf_enc(P);
   {  // LfGlobal
     BitWriter& w = sections[0];
+    write_features(w, a, a.width, a.height);
     w.write(1, 1);  // LfChannelDequantization all_default
     // Quantizer: global_scale U32(1+u11, 2049+u11, 4097+u12, 8193+u16), quant_lf U32(16, 1+u5, 1+u8, 1+u16)
     if (global_scale <= 2048) write_u32(w, 0, 11, global_scale - 1);
@@ -1719,9 +1799,9 @@ int main(int argc, char** argv) {
     else if (v <= 8192) write_u32(cs, 1, 13, v - 1);
     else write_u32(cs, 2, 18, v - 1);
   };
-  write_dim(H);
+  write_dim(a.height);
   cs.write(3, 0);  // ratio
-  write_dim(W);
+  write_dim(a.width);
   if (a.colour.empty() && a.extras.empty()) {
     cs.write(1, 1);  // ImageMetadata all_default
   } else {  // ImageMetadata with extra channels and / or an enum ColourEncoding (jxl-image/src/lib.rs:229-287, color.rs:21-58)
@@ -1861,12 +1941,12 @@ int main(int argc, char** argv) {
     cs.write(2, 0);         // name: empty
     cs.write(1, 1);         // restoration filter all_default
     write_u64_small(0);     // frame extensions
-  } else if (P > 1 || a.epf_iters != 2 || !a.gaborish || !a.extras.empty()) {
+  } else if (P > 1 || a.epf_iters != 2 || !a.gaborish || !a.extras.empty() || up != 1 || a.noise != Args::kNoNoise || a.splines || a.dangling_patch) {
     cs.write(1, 0);         // all_default
     cs.write(2, 0);         // Regular
     cs.write(1, 0);         // VarDCT
-    write_u64_small(0);     // flags
-    cs.write(2, 0);         // upsampling = 1
+    write_u64_small((a.noise != Args::kNoNoise ? 0x1 : 0) | (a.dangling_patch ? 0x2 : 0) | (a.splines ? 0x10 : 0));  // flags: noise, patches, splines
+    cs.write(2, ceil_log2_nonzero(up));  // upsampling: U32 selector k is 2^k
     for (const Args::Extra& e : a.extras) cs.write(2, ceil_log2_nonzero(e.ec_upsampling));  // U32 selector k is 2^k
     cs.write(3, 3);         // x_qm_scale
     cs.write(3, 2);         // b_qm_scale
