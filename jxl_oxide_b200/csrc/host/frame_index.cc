@@ -41,8 +41,8 @@ FrameIndex index_frames(const uint8_t* cs, size_t size) {
   if (ih.colour_encoding.want_icc) skip_icc_profile(br);
   br.check();
   br.zero_pad_to_byte();
-  size_t pos = br.pos() / 8;
-  JXLB_CHECK(!ih.have_preview, kErrUnsupported, "preview frames are not supported");
+  // the preview is neither a visible nor an invisible frame: it takes no part in the noise seeds
+  size_t pos = skip_preview_frame(cs, size, ih, br.pos() / 8);
 
   uint64_t visible = 0, invisible = 0;
   while (pos < size) {

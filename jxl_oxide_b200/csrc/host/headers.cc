@@ -534,4 +534,14 @@ Toc parse_toc(BitReader& br, const FrameHeader& fh) {  // data/toc.rs:177-271
   return toc;
 }
 
+size_t skip_preview_frame(const uint8_t* cs, size_t size, const ImageHeader& ih, size_t pos) {
+  if (!ih.have_preview) return pos;
+  BitReader br(cs, size, pos * 8);
+  const FrameHeader fh = parse_frame_header(br, ih);
+  const Toc toc = parse_toc(br, fh);
+  const size_t end = toc.data_begin + toc.total_size;
+  JXLB_CHECK(end <= size, kErrEof, "preview frame beyond end of codestream");
+  return end;
+}
+
 }  // namespace jxlb

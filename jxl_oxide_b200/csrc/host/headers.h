@@ -193,5 +193,9 @@ void skip_icc_profile(BitReader& br);
 std::vector<uint8_t> read_icc_stream(BitReader& br);
 FrameHeader parse_frame_header(BitReader& br, const ImageHeader& ih);
 Toc parse_toc(BitReader& br, const FrameHeader& fh);
+// The byte after the preview frame that starts at byte `pos` (the first byte after the image header), or `pos` when the
+// image has no preview. Only its frame header and TOC are read, as jxl-oxide/src/lib.rs:384-411 does; the header's
+// size fields default to the image's size, not the preview's.
+size_t skip_preview_frame(const uint8_t* cs, size_t size, const ImageHeader& ih, size_t pos);
 
 }  // namespace jxlb

@@ -253,9 +253,9 @@ void first_frame_header(const std::vector<uint8_t>& cs, ImageHeader* ih, FrameHe
   *ih = parse_image_header(br);
   if (ih->colour_encoding.want_icc) skip_icc_profile(br);
   br.zero_pad_to_byte();
-  JXLB_CHECK(!ih->have_preview, kErrUnsupported, "preview frames are not supported");
-  *fh = parse_frame_header(br, *ih);
-  br.check();
+  BitReader fr(cs.data(), cs.size(), skip_preview_frame(cs.data(), cs.size(), *ih, br.pos() / 8) * 8);
+  *fh = parse_frame_header(fr, *ih);
+  fr.check();
 }
 
 bool normal_frame(const FrameHeader& fh) {

@@ -198,11 +198,12 @@ std::vector<Backend::SplineArc> build_spline_arcs(const LfGlobalSyntax& g, bool 
   return arcs;
 }
 
-// Reference slots (jxl-render/src/state.rs, lib.rs:296-330): a frame saved for later frames' patches. Only
-// reference-only frames saved before the colour transform are kept (what libjxl's patch detector emits).
+// Reference slots (jxl-render/src/state.rs, lib.rs:296-330): a frame saved for later frames' patches and blending.
+// The reference reads a slot as it is, whatever it holds (blend.rs:179-219, the patch blend).
 struct RefFrameStore {
   bool valid = false;
-  bool ct_done = false;  // saved after the colour transform (regular frames) or before it (reference-only)
+  // false when the saving frame left or deferred its colour transform: the slot holds samples from before it
+  bool ct_done = false;
   uint32_t width = 0, height = 0;
   std::vector<View> channels;  // colour (XYB / as coded, f32) then extra channels (f32)
 };
@@ -256,8 +257,11 @@ class FramePlanner {
   void setup_gmodular();
   std::vector<LfGroupRect> lf_rect_;
   void render_vardct(DecodedFrame* out);
-  bool colour_params(bool is_xyb, size_t num_colour, ColorParams* p);
-  void finish_colour(std::vector<View>& colour, bool is_xyb, bool already_converted, DecodedFrame* out);
+  void ycbcr_to_rgb(std::vector<View>& colour);
+  // `output_colour` as in DecodeOptions: the encoding a colour conversion targets
+  bool colour_params(bool is_xyb, size_t num_colour, int output_colour, ColorParams* p);
+  // true when it converted the planes
+  bool finish_colour(std::vector<View>& colour, bool is_xyb, bool already_converted, int output_colour, DecodedFrame* out);
   // log2 of the factor that brings extra channel `i` from its coded size to the frame size (image.rs:487-557)
   uint32_t ec_shift(size_t i) const { return ceil_log2_nonzero(fh_.ec_upsampling[i]) + ih_.ec_info[i].dim_shift; }
 
@@ -486,14 +490,27 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
   const bool vardct = fh_.encoding == Encoding::kVarDct;
   const bool is_lf_frame = fh_.frame_type == FrameType::kLfFrame;
   const bool is_ref_frame = fh_.frame_type == FrameType::kReferenceOnly;
-  if (is_ref_frame) {
-    JXLB_CHECK(fh_.save_before_ct, kErrUnsupported, "reference frames saved after the colour transform are not supported");
-    JXLB_CHECK(fh_.upsampling == 1, kErrUnsupported, "upsampled reference frames are not supported");
-  } else if (!is_lf_frame) {
-    // regular frames are composed onto the canvas after the colour transform (jxl-render/src/blend.rs:178-415)
-    JXLB_CHECK(!fh_.save_before_ct || fh_.is_last, kErrUnsupported, "regular frames saved before the colour transform are not supported");
-  } else {
+  const bool normal_frame = !is_lf_frame && !is_ref_frame;
+  if (is_lf_frame)
     JXLB_CHECK(fh_.lf_level >= 1 && fh_.lf_level <= 4 && fh_.upsampling == 1, kErrBitstream, "invalid LF frame header");
+  // The colour transform a frame applies to its own samples, as an output_colour value, or -1 for none
+  // (render.rs:151-153, image.rs:807-809, util.rs:311-374). An LF frame stays in XYB: it is the next frame's LF image.
+  // A frame saved before the transform keeps its samples as coded (XYB, or YCbCr with do_ycbcr); a regular one that
+  // is not the last frame defers the transform to its keyframe's composed canvas (postprocess_keyframe, lib.rs:925-998).
+  // A reference-only frame saved after it converts to the signalled encoding whatever output was asked for, and
+  // leaves its samples alone under an ICC profile or an XYB / unknown colour space. Every other regular frame converts to
+  // the requested encoding before it is composed; for output_colour 0 with an enum encoding that is the reference's
+  // record conversion.
+  const bool defer_ct = normal_frame && fh_.save_before_ct && !fh_.is_last;
+  const ColourSpace space = ih_.colour_encoding.colour_space;
+  const bool enum_rgb_or_grey = !ih_.colour_encoding.want_icc && (space == ColourSpace::kRgb || space == ColourSpace::kGrey);
+  // the reference's record conversion leaves XYB samples alone: the frame keeps ct_done false
+  const bool record_keeps_xyb = !fh_.do_ycbcr && ih_.xyb_encoded && !enum_rgb_or_grey;
+  int ct_target = opt_.output_colour;
+  if (is_lf_frame || defer_ct || (is_ref_frame && fh_.save_before_ct)) {
+    ct_target = -1;
+  } else if (is_ref_frame) {
+    ct_target = record_keeps_xyb || !(fh_.do_ycbcr || ih_.xyb_encoded) ? -1 : 0;
   }
   if (fh_.use_lf_frame()) {
     JXLB_CHECK(vardct, kErrBitstream, "use_lf_frame on a Modular frame");
@@ -823,9 +840,8 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
   // restoration filters (render.rs:76-131)
   const RestorationFilter& rf = fh_.restoration_filter;
   const bool upsampled = fh_.upsampling > 1;
-  // an LF frame stays in XYB (it is the next frame's LF image), so does a reference frame saved before the
-  // colour transform
-  bool colour_done = is_lf_frame || is_ref_frame;
+  bool colour_done = ct_target < 0;
+  bool converted = false;  // the frame's samples went through a colour transform here
   if (rf.gab_enabled || rf.epf.iters > 0) {
     // a grayscale frame is filtered as three identical channels and truncated again (render.rs:74-134)
     JXLB_CHECK(colour.size() == 3 || colour.size() == 1, kErrUnsupported, "restoration filters need one or three colour channels");
@@ -845,10 +861,10 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
     ColorParams cp;
     // colour conversion follows upsampling (render.rs:136-149), so it is fused only without it
     const bool want_colour = !upsampled && !colour_done && !lfg_.has_noise && !lfg_.has_patches && !lfg_.has_splines &&
-                             colour_params(ih_.xyb_encoded, colour.size(), &cp) && !cp.second_stage && cp.gamma == 0.0f &&
+                             colour_params(ih_.xyb_encoded, colour.size(), ct_target, &cp) && !cp.second_stage && cp.gamma == 0.0f &&
                              cp.pq_intensity_target == 0.0f;
     if (be_.filters_colour_fused(v, rf, sigma_view, !vardct, want_colour ? &cp : nullptr)) {
-      colour_done = want_colour;
+      colour_done = converted = want_colour;
       if (want_colour) be_.stage_marker("rgb", v, 3);
     } else {
       if (rf.gab_enabled) {
@@ -979,14 +995,11 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
     be_.stage_marker("patches", colour.data(), int(colour.size()));
   }
   if (!upsampled) splines_and_noise();
-  if (fh_.do_ycbcr && !colour_done) {  // jxl-render/src/lib.rs:950-954, util.rs:320-329
-    JXLB_CHECK(colour.size() == 3, kErrBitstream, "YCbCr needs three channels");
-    View v[3] = {colour[0], colour[1], colour[2]};
-    be_.ycbcr_to_rgb(v, Backend::YcbcrParams());
-    be_.stage_marker("rgb", v, 3);
-    if (ih_.colour_encoding.colour_space == ColourSpace::kGrey) colour.resize(1);
+  if (fh_.do_ycbcr && !colour_done) {
+    ycbcr_to_rgb(colour);
+    converted = true;
   }
-  finish_colour(colour, ih_.xyb_encoded, colour_done, &out);
+  converted |= finish_colour(colour, ih_.xyb_encoded, colour_done, ct_target, &out);
   out.channels.insert(out.channels.end(), extra.begin(), extra.end());
   if (is_lf_frame) {
     JXLB_CHECK(colour.size() == 3, kErrUnsupported, "grayscale LF frames are not supported");
@@ -997,7 +1010,6 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
     slot.valid = true;
     out.internal = true;
   }
-  const bool normal_frame = !is_lf_frame && !is_ref_frame;
   const bool can_reference = !fh_.is_last && (fh_.duration == 0 || fh_.save_as_reference != 0) && !is_lf_frame;  // header.rs:221-225
   if (normal_frame && !(fh_.resets_canvas && out.width == ih_.width && out.height == ih_.height)) {
     // ---- composition onto the image canvas (blend.rs:178-415 as a full-canvas model): every channel starts from
@@ -1016,8 +1028,13 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
       int id = new_plane(ih_.width, ih_.height, /*zero=*/true);
       canvas[idx] = View{id, 0, 0, ih_.width, ih_.height};
       const bool have_base = base.valid && idx < base.channels.size();
-      if (have_base) {
-        JXLB_CHECK(base.ct_done || !ih_.xyb_encoded, kErrUnsupported, "blending onto a frame saved before the colour transform");
+      if (have_base) {  // as the slot holds it, before or after the colour transform
+        // Under an ICC profile or an XYB / unknown colour space the reference composes this frame unconverted and
+        // converts the whole canvas at the end (lib.rs:934-995), base included. This frame was converted here already,
+        // so it would be composed in a different space from the base: not implemented.
+        JXLB_CHECK(base.ct_done || !converted || !record_keeps_xyb, kErrUnsupported,
+                   "blending a converted frame onto a slot saved before the colour transform under an ICC profile or an "
+                   "XYB / unknown colour space");
         const View& bv = base.channels[idx];
         const uint32_t cw = std::min(bv.w, ih_.width), chh = std::min(bv.h, ih_.height);
         be_.copy_rect(View{bv.plane, bv.x0, bv.y0, cw, chh}, View{id, 0, 0, cw, chh});
@@ -1074,8 +1091,17 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
     }
     slot.width = out.width;
     slot.height = out.height;
-    slot.ct_done = !is_ref_frame;
+    slot.ct_done = ct_target >= 0;
     slot.valid = true;
+  }
+  if (defer_ct && fh_.is_keyframe()) {
+    // the composed canvas takes the transform to the requested encoding the frame deferred, the base's region included
+    // (blend.rs:219 gives the canvas the new frame's state); the slot above keeps the samples from before it
+    std::vector<View> canvas_colour(out.channels.begin(), out.channels.begin() + out.num_color);
+    const std::vector<View> canvas_extra(out.channels.begin() + out.num_color, out.channels.end());
+    if (fh_.do_ycbcr) ycbcr_to_rgb(canvas_colour);
+    finish_colour(canvas_colour, ih_.xyb_encoded, false, opt_.output_colour, &out);
+    out.channels.insert(out.channels.end(), canvas_extra.begin(), canvas_extra.end());
   }
   if (is_ref_frame || (normal_frame && !fh_.is_keyframe())) out.internal = true;
   // release everything not exported
@@ -1210,12 +1236,12 @@ void target_matrix(const ColourEncoding& ce, bool grey, ColorParams* p) {
 }
 }  // namespace
 
-bool FramePlanner::colour_params(bool is_xyb, size_t num_colour, ColorParams* p) {
-  if (!is_xyb || opt_.output_colour == 2) return false;
+bool FramePlanner::colour_params(bool is_xyb, size_t num_colour, int output_colour, ColorParams* p) {
+  if (!is_xyb || output_colour < 0 || output_colour == 2) return false;
   JXLB_CHECK(num_colour == 3, kErrBitstream, "XYB needs three channels");
   // with an embedded ICC profile the target is the equivalent enum encoding, or sRGB (jxl-render/src/lib.rs:104-150)
   const ColourEncoding& ce = ih_.colour_encoding.want_icc ? ih_.icc_encoding : ih_.colour_encoding;
-  const bool linear_srgb_out = opt_.output_colour == 1;
+  const bool linear_srgb_out = output_colour == 1;
   if (!linear_srgb_out) {
     JXLB_CHECK(ce.colour_space == ColourSpace::kRgb || ce.colour_space == ColourSpace::kGrey, kErrUnsupported,
                "unsupported output colour space");
@@ -1224,7 +1250,7 @@ bool FramePlanner::colour_params(bool is_xyb, size_t num_colour, ColorParams* p)
   }
   // an HDR target keeps the image's range (convert.rs:478-499: tone mapping only towards non-HDR targets)
   const bool hdr_target = !linear_srgb_out && ce.tf == TransferFunctionKind::kPq;
-  JXLB_CHECK(ih_.tone_mapping.intensity_target <= 255.0f || opt_.output_colour == 1 || hdr_target, kErrUnsupported,
+  JXLB_CHECK(ih_.tone_mapping.intensity_target <= 255.0f || output_colour == 1 || hdr_target, kErrUnsupported,
              "HDR tone mapping is outside the implemented hot path");
   const OpsinInverseMatrix& oim = ih_.opsin_inverse_matrix;
   for (int i = 0; i < 3; ++i) {
@@ -1233,8 +1259,8 @@ bool FramePlanner::colour_params(bool is_xyb, size_t num_colour, ColorParams* p)
     for (int j = 0; j < 3; ++j) p->matrix[i * 3 + j] = oim.inv_mat[i][j];
   }
   p->itscale = 255.0f / ih_.tone_mapping.intensity_target;
-  p->apply_srgb_tf = (opt_.output_colour == 0) && ce.tf == TransferFunctionKind::kSrgb;
-  p->apply_bt709_tf = (opt_.output_colour == 0) && ce.tf == TransferFunctionKind::kBt709;
+  p->apply_srgb_tf = (output_colour == 0) && ce.tf == TransferFunctionKind::kSrgb;
+  p->apply_bt709_tf = (output_colour == 0) && ce.tf == TransferFunctionKind::kBt709;
   if (!linear_srgb_out) {
     if (ce.tf == TransferFunctionKind::kGamma)  // convert.rs:972-989
       p->gamma = ce.gamma_inverted ? float(ce.gamma) / 1e7f : 1e7f / float(ce.gamma);
@@ -1246,9 +1272,19 @@ bool FramePlanner::colour_params(bool is_xyb, size_t num_colour, ColorParams* p)
   return true;
 }
 
-void FramePlanner::finish_colour(std::vector<View>& colour, bool is_xyb, bool already_converted, DecodedFrame* out) {
+void FramePlanner::ycbcr_to_rgb(std::vector<View>& colour) {  // jxl-render/src/lib.rs:950-954, util.rs:320-329
+  JXLB_CHECK(colour.size() == 3, kErrBitstream, "YCbCr needs three channels");
+  View v[3] = {colour[0], colour[1], colour[2]};
+  be_.ycbcr_to_rgb(v, Backend::YcbcrParams());
+  be_.stage_marker("rgb", v, 3);
+  if (ih_.colour_encoding.colour_space == ColourSpace::kGrey) colour.resize(1);
+}
+
+bool FramePlanner::finish_colour(std::vector<View>& colour, bool is_xyb, bool already_converted, int output_colour,
+                                 DecodedFrame* out) {
   ColorParams p;
-  if (!already_converted && colour_params(is_xyb, colour.size(), &p)) {
+  const bool convert = !already_converted && colour_params(is_xyb, colour.size(), output_colour, &p);
+  if (convert) {
     View v[3] = {colour[0], colour[1], colour[2]};
     be_.xyb_to_rgb(v, p);
     if (p.to_luma) colour.resize(1);  // XyzToLuma leaves Y in the first channel (convert.rs:866-872)
@@ -1256,6 +1292,7 @@ void FramePlanner::finish_colour(std::vector<View>& colour, bool is_xyb, bool al
   }
   out->num_color = uint32_t(colour.size());
   out->channels = colour;
+  return convert;
 }
 
 }  // namespace
@@ -1304,14 +1341,7 @@ size_t parse_codestream_header(const uint8_t* cs, size_t size, ImageHeader* out)
     }
   }
   br.zero_pad_to_byte();
-  const size_t pos = br.pos() / 8;
-  if (ih.have_preview) {  // skipped, like jxl-oxide/src/lib.rs:384-411
-    BitReader pr(cs, size, pos * 8);
-    FrameHeader pfh = parse_frame_header(pr, ih);
-    (void)pfh;
-    fail(kErrUnsupported, "preview frames are not supported");
-  }
-  return pos;
+  return skip_preview_frame(cs, size, ih, br.pos() / 8);
 }
 
 void Backend::add_noise_in_frame(const View v[3], uint32_t field_w, uint32_t field_h, const float lut[8], uint32_t group_dim,

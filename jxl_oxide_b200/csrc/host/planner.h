@@ -56,8 +56,8 @@ std::vector<uint8_t> extract_codestream(const uint8_t* data, size_t size);
 // stay alive in the backend until the caller frees them.
 DecodeResult decode_codestream(Backend& be, const uint8_t* codestream, size_t size, const DecodeOptions& opt);
 
-// The two halves of decode_codestream. parse_codestream_header reads the image header and ICC profile and returns the
-// byte offset of the first frame. decode_frames decodes the frames from byte `begin` on, as if `visible_before` shown
+// The two halves of decode_codestream. parse_codestream_header reads the image header and ICC profile, skips the
+// preview frame if there is one, and returns the byte offset of the first frame. decode_frames decodes the frames from byte `begin` on, as if `visible_before` shown
 // and `invisible_before` hidden frames had come before and left every reference slot and LF store empty; each shown
 // frame goes to `sink` as soon as it is finished (the sink owns its planes), up to `max_shown` of them. The stores are
 // freed when it returns or throws. The caller has called be.set_codestream().
