@@ -7,22 +7,18 @@ namespace jxlb {
 
 namespace {
 
-// The state a frame reads and writes, as FramePlanner::decode_frame uses it (planner.cc).
+// The state a frame reads and writes (frame_role, planner.h).
 void frame_state(const FrameHeader& fh, const ImageHeader& ih, IndexedFrame* f) {
-  const bool is_lf_frame = fh.frame_type == FrameType::kLfFrame;
-  const bool is_ref_frame = fh.frame_type == FrameType::kReferenceOnly;
-  const bool normal = !is_lf_frame && !is_ref_frame;
-  if (fh.use_lf_frame() && fh.lf_level < 4) f->reads |= 1u << (4 + fh.lf_level);
+  const FrameRole role = frame_role(fh, ih);
+  if (role.lf_read >= 0) f->reads |= 1u << (4 + role.lf_read);
   if (fh.patches()) f->reads |= 0xfu;  // the patch list (in LfGlobal) may name any slot
-  // composition onto the canvas reads the blending sources unless the frame replaces the whole canvas
-  if (normal && !(fh.resets_canvas && fh.width == ih.width && fh.height == ih.height)) {
+  if (role.composes) {  // composition onto the canvas reads the blending sources
     f->reads |= 1u << fh.blending_info.source;
     for (const BlendingInfo& b : fh.ec_blending_info) f->reads |= 1u << b.source;
   }
-  if (is_lf_frame) f->writes |= 1u << (4 + fh.lf_level - 1);
-  const bool can_reference = !fh.is_last && (fh.duration == 0 || fh.save_as_reference != 0) && !is_lf_frame;
-  if (is_ref_frame || (normal && can_reference)) f->writes |= 1u << fh.save_as_reference;
-  f->shown = normal && fh.is_keyframe();
+  if (role.lf_write >= 0) f->writes |= 1u << (4 + role.lf_write);
+  if (role.saved_to >= 0) f->writes |= 1u << role.saved_to;
+  f->shown = role.shown;
 }
 
 }  // namespace

@@ -54,12 +54,6 @@ struct GroupChannel {
   int32_t hshift, vshift;
 };
 
-// Rendered LF frames by level (RenderContext::lf_frame, jxl-render/src/lib.rs:46, 294-318): slot k holds
-// the frame whose lf_level is k + 1; a frame with use_lf_frame reads slot `lf_level`.
-struct LfFrameStore {
-  bool valid = false;
-  View planes[3];  // X, Y, B (f32)
-};
 
 // Splines: dequantisation, centripetal Catmull-Rom upsampling, unit arc-length resampling and the per-arc colour /
 // thickness (jxl-render/src/features/spline.rs:41-178 and the head of render_spline :180-218). Scalar host work - a
@@ -153,8 +147,7 @@ std::vector<ArcSample> unit_arc_samples(const std::vector<Pt>& up) {
 }
 }  // namespace
 
-std::vector<Backend::SplineArc> build_spline_arcs(const LfGlobalSyntax& g, bool /*vardct*/, float corr_x, float corr_b, uint32_t width,
-                                                  uint32_t height) {
+std::vector<Backend::SplineArc> build_spline_arcs(const LfGlobalSyntax& g, float corr_x, float corr_b, uint32_t width, uint32_t height) {
   std::vector<Backend::SplineArc> arcs;
   const float qa = float(g.spline_quant_adjust);
   const float inverted_qa = qa >= 0.0f ? 1.0f / (1.0f + qa / 8.0f) : 1.0f - qa / 8.0f;
@@ -198,14 +191,51 @@ std::vector<Backend::SplineArc> build_spline_arcs(const LfGlobalSyntax& g, bool 
   return arcs;
 }
 
-// Reference slots (jxl-render/src/state.rs, lib.rs:296-330): a frame saved for later frames' patches and blending.
-// The reference reads a slot as it is, whatever it holds (blend.rs:179-219, the patch blend).
-struct RefFrameStore {
+// A frame kept for later frames. A reference slot (jxl-render/src/state.rs, lib.rs:296-330) holds a frame saved for
+// later frames' patches and blending; the reference reads it as it is, whatever it holds (blend.rs:179-219, the patch
+// blend). An LF store (RenderContext::lf_frame, lib.rs:46, 294-318) holds the X, Y, B planes of a rendered LF frame:
+// store k the frame whose lf_level is k + 1, which a frame with use_lf_frame reads as store `lf_level`.
+struct StoredFrame {
   bool valid = false;
   // false when the saving frame left or deferred its colour transform: the slot holds samples from before it
   bool ct_done = false;
   uint32_t width = 0, height = 0;
   std::vector<View> channels;  // colour (XYB / as coded, f32) then extra channels (f32)
+};
+
+// The reference slots and LF stores a run of frames shares. They own the planes they hold.
+struct FrameStores {
+  Backend& be;
+  StoredFrame ref[4], lf[4];
+
+  void release(StoredFrame& s) {
+    if (s.valid)
+      for (const View& v : s.channels) be.free_plane(v.plane);
+    s = StoredFrame();
+  }
+  // Frees what `s` held and stores `f` in it: with `copy` the slot keeps copies of f's planes (the frame may also be
+  // shown), else it takes them over.
+  void replace(StoredFrame& s, StoredFrame f, bool copy) {
+    release(s);
+    if (copy)
+      for (View& v : f.channels) {
+        const View dst{be.alloc_plane(std::max(v.w, 1u), std::max(v.h, 1u), false), 0, 0, v.w, v.h};
+        if (v.w && v.h) be.copy_rect(v, dst);
+        v = dst;
+      }
+    s = std::move(f);
+  }
+  void release_all() {
+    for (StoredFrame& s : lf) release(s);
+    for (StoredFrame& s : ref) release(s);
+  }
+};
+
+// The colour transform a frame applies to its own samples (render.rs:151-153, image.rs:807-809, util.rs:311-374).
+struct ColourPlan {
+  int ct_target = -1;  // as an output_colour value, or -1 for none
+  bool defer_ct = false;  // the transform is applied to the keyframe's composed canvas instead
+  bool record_keeps_xyb = false;  // the reference's record conversion leaves XYB samples alone: the frame keeps ct_done false
 };
 
 // A parsed Modular stream whose channel data is about to be (or has been) decoded.
@@ -214,17 +244,17 @@ struct PendingStream {
   std::vector<ChanBuf> coded;    // buffers of the coded channels
   std::vector<View> targets;     // where image channels must end up (empty view = stay in `coded`)
   bool direct = true;            // coded channels alias the targets (no local transforms)
-  size_t job_index = 0;
 };
 
 class FramePlanner {
  public:
   FramePlanner(Backend& be, const uint8_t* cs, size_t size, const ImageHeader& ih, const DecodeOptions& opt,
-               LfFrameStore (*lf_store)[4], RefFrameStore (*ref_store)[4], uint64_t visible_before,
-               uint64_t invisible_before)
-      : be_(be), cs_(cs), size_(size), ih_(ih), opt_(opt), lf_store_(lf_store), ref_store_(ref_store),
-        visible_before_(visible_before), invisible_before_(invisible_before) {}
+               FrameStores& stores, uint64_t visible_before, uint64_t invisible_before)
+      : be_(be), cs_(cs), size_(size), ih_(ih), opt_(opt), stores_(stores), visible_before_(visible_before),
+        invisible_before_(invisible_before) {}
 
+  // Decodes the frame at `frame_begin_byte`. A frame that is not shown comes back `internal` and without planes:
+  // what later frames need of it is in the stores.
   DecodedFrame decode_frame(size_t frame_begin_byte, size_t* frame_end_byte);
   // A frame that fails half way (malformed or unsupported stream) must not keep its planes: they are
   // cleared from the list once exported or freed at the end of decode_frame().
@@ -253,50 +283,103 @@ class FramePlanner {
   PendingStream prepare_stream(BitReader& br, size_t limit_byte, const std::vector<GroupChannel>& image_channels,
                                uint32_t stream_index, std::vector<ModularStreamJob>* jobs);
   void finish_stream(PendingStream& ps);
+  // Stream i of a batch: reads what precedes the stream's header at `r` and returns the stream's channels, none when
+  // the stream is absent. It may give an HfMetadata stream its LF group's varblock placement.
+  using StreamOpener = std::function<std::vector<GroupChannel>(uint32_t i, BitReader& r, VarblockPlacement* placement)>;
+  // Decodes the streams i < pos.size() (stream i at bit pos[i] of a section ending at byte limit[i], MA-tree stream
+  // index first_index + i) in one decode_modular call, finishes each and moves pos[i] to its end. Returns the jobs of
+  // the streams present, in order.
+  std::vector<ModularStreamJob> decode_streams(std::vector<size_t>& pos, const std::vector<size_t>& limit,
+                                               uint32_t first_index, const StreamOpener& open);
   void run_inverse_transforms(const ModularStreamSyntax& s, std::vector<ChanBuf>& bufs);
   void setup_gmodular();
-  std::vector<LfGroupRect> lf_rect_;
-  void render_vardct(DecodedFrame* out);
-  void ycbcr_to_rgb(std::vector<View>& colour);
+
+  // the stages of decode_frame, in order
+  void begin_frame(size_t frame_begin_byte, size_t* frame_end_byte);
+  ColourPlan colour_plan() const;
+  void decode_lf_global();
+  void init_vardct_state();
+  void decode_lf_groups();
+  void decode_hf_metadata();
+  void decode_hf_global();
+  void decode_pass_groups();
+  std::vector<View> samples_to_float(DecodedFrame* out);
+  void render_vardct();
+  bool restoration_filters(const std::vector<View>& colour);
+  std::vector<View> render_features(std::vector<View>& colour, DecodedFrame* out);
+  void splines_and_noise(const std::vector<View>& colour);
+  void apply_patches(const std::vector<View>& colour, const std::vector<View>& extra);
+  void compose(DecodedFrame* out, bool converted);
+  void record(const DecodedFrame& out);
+  void release_planes(DecodedFrame* out);
+
   // `output_colour` as in DecodeOptions: the encoding a colour conversion targets
   bool colour_params(bool is_xyb, size_t num_colour, int output_colour, ColorParams* p);
-  // true when it converted the planes
-  bool finish_colour(std::vector<View>& colour, bool is_xyb, bool already_converted, int output_colour, DecodedFrame* out);
+  bool colour_transform(std::vector<View> colour, const std::vector<View>& extra, bool done, int target, DecodedFrame* out);
   // log2 of the factor that brings extra channel `i` from its coded size to the frame size (image.rs:487-557)
   uint32_t ec_shift(size_t i) const { return ceil_log2_nonzero(fh_.ec_upsampling[i]) + ih_.ec_info[i].dim_shift; }
+  // block counts are rounded up to even in a subsampled direction (hf_metadata.rs:70-80, vardct/mod.rs:83-95)
+  uint32_t blocks_w(uint32_t px) const { return h_subsampled_ ? ((px + 7) / 8 + 1) / 2 * 2 : (px + 7) / 8; }
+  uint32_t blocks_h(uint32_t px) const { return v_subsampled_ ? ((px + 7) / 8 + 1) / 2 * 2 : (px + 7) / 8; }
 
   Backend& be_;
   const uint8_t* cs_;
   size_t size_;
   const ImageHeader& ih_;
   DecodeOptions opt_;
-  LfFrameStore (*lf_store_)[4];
-  RefFrameStore (*ref_store_)[4];
+  FrameStores& stores_;
   // frames shown before this one / hidden frames since the last shown one: the noise generator's seed
   // (jxl-render/src/lib.rs:563-585, features/noise.rs:180-185)
   uint64_t visible_before_, invisible_before_;
   FrameHeader fh_;
+  FrameRole role_;
+  ColourPlan colour_;
+  bool vardct_ = false;
+  // JPEG chroma subsampling: per-channel shifts (ChannelShift::from_jpeg_upsampling, jxl-modular/src/param.rs:105-122)
+  bool h_subsampled_ = false, v_subsampled_ = false;
+  uint32_t chan_hshift_[3] = {0, 0, 0}, chan_vshift_[3] = {0, 0, 0};
   Toc toc_;
+  size_t pos_ = 0, limit_ = 0;  // the LfGlobal section: bit position reached, byte limit
   LfGlobalSyntax lfg_;
   HfGlobalSyntax hfg_;
   VarDctState st_;
-  std::vector<int> frame_planes_;  // freed at the end of the frame unless exported
+  // full-size float planes of the extra channels upsampled here and the noise field of an upsampled frame
+  size_t ec_render_bytes_ = 0;
+  std::vector<size_t> lf_pos_, lf_limit_;  // [lf_group]: bit position reached, byte limit of its section
+  std::vector<LfGroupRect> lf_rect_;
+  std::vector<int> frame_planes_;  // freed at the end of the frame unless exported or handed to a store
   // global modular
   std::vector<ChanBuf> gm_coded_;
+  std::vector<ChanBuf> gm_image_;  // gm_coded_ after the global inverse transforms
   size_t gm_global_count_ = 0;
   std::vector<std::vector<GroupChannel>> gm_lf_groups_;               // [lf_group]
   std::vector<std::vector<std::vector<GroupChannel>>> gm_pass_groups_;  // [pass][group]
   std::vector<uint32_t> extra_precision_;
+  size_t ec_from_ = 0;  // index of the first extra channel in gm_image_
 
-  int new_plane(uint32_t w, uint32_t h, bool zero = false) {
-    int id = be_.alloc_plane(std::max(w, 1u), std::max(h, 1u), zero);
+  int adopt(int id) {
     frame_planes_.push_back(id);
     return id;
   }
+  int new_plane(uint32_t w, uint32_t h, bool zero = false) {
+    return adopt(be_.alloc_plane(std::max(w, 1u), std::max(h, 1u), zero));
+  }
+  void disown(int id) { frame_planes_.erase(std::remove(frame_planes_.begin(), frame_planes_.end(), id), frame_planes_.end()); }
   void drop_plane(int id) {
-    auto it = std::find(frame_planes_.begin(), frame_planes_.end(), id);
-    if (it != frame_planes_.end()) frame_planes_.erase(it);
+    disown(id);
     be_.free_plane(id);
+  }
+  // chroma upsampling (upsample_jpeg, jxl-render/src/image.rs:448-486, filter/ycbcr.rs) of colour channel c from its
+  // coded size to the colour size; a channel rounded up to an even size in a subsampled direction is cropped
+  View upsample_chroma(const View& v, int c) {
+    const uint32_t cw = fh_.color_sample_width(), chh = fh_.color_sample_height();
+    if (!chan_hshift_[c] && !chan_vshift_[c]) return View{v.plane, v.x0, v.y0, cw, chh};
+    return View{adopt(be_.upsample_jpeg(v, chan_hshift_[c] != 0, chan_vshift_[c] != 0, cw, chh)), 0, 0, cw, chh};
+  }
+  // non-separable upsampling (render.rs:136-183), cropped to the frame size
+  void upsample_view(View& v, uint32_t factor_log2) {
+    const int id = adopt(be_.upsample(v, factor_log2, ih_));
+    v = View{id, 0, 0, std::min(v.w << factor_log2, fh_.width), std::min(v.h << factor_log2, fh_.height)};
   }
 };
 
@@ -331,9 +414,31 @@ PendingStream FramePlanner::prepare_stream(BitReader& br, size_t limit_byte,
       job.channels.push_back({v, c.hshift, c.vshift});
     }
   }
-  ps.job_index = jobs->size();
   jobs->push_back(std::move(job));
   return ps;
+}
+
+std::vector<ModularStreamJob> FramePlanner::decode_streams(std::vector<size_t>& pos, const std::vector<size_t>& limit,
+                                                           uint32_t first_index, const StreamOpener& open) {
+  std::vector<ModularStreamJob> jobs;
+  std::vector<PendingStream> pend;
+  std::vector<size_t> owner;
+  for (uint32_t i = 0; i < pos.size(); ++i) {
+    BitReader r = reader_at(pos[i], limit[i]);
+    VarblockPlacement placement;
+    const std::vector<GroupChannel> chans = open(i, r, &placement);
+    if (chans.empty()) continue;
+    pend.push_back(prepare_stream(r, limit[i], chans, first_index + i, &jobs));
+    // without Modular transforms the stream's own output is final: the backend may place right after the stream
+    if (pend.back().direct) jobs.back().placement = placement;
+    owner.push_back(i);
+  }
+  if (!jobs.empty()) be_.decode_modular(jobs);
+  for (size_t k = 0; k < pend.size(); ++k) {
+    finish_stream(pend[k]);
+    pos[owner[k]] = jobs[k].end_bit;
+  }
+  return jobs;
 }
 
 void FramePlanner::run_inverse_transforms(const ModularStreamSyntax& s, std::vector<ChanBuf>& bufs) {
@@ -351,8 +456,7 @@ void FramePlanner::run_inverse_transforms(const ModularStreamSyntax& s, std::vec
         for (size_t c = 0; c < n; ++c) {
           ChanBuf& avg = bufs[begin + c];
           ChanBuf& res = bufs[res0 + c];
-          int merged = merged_ids[c];
-          frame_planes_.push_back(merged);
+          const int merged = adopt(merged_ids[c]);
           View mv;
           mv.plane = merged;
           mv.w = sp.horizontal ? avg.view.w + res.view.w : avg.view.w;
@@ -433,16 +537,15 @@ void FramePlanner::setup_gmodular() {
   pass_shifts[fh_.passes.num_passes - 1] = {0, maxshift};
   const uint32_t num_passes = fh_.passes.num_passes;
   const uint32_t cw = fh_.color_sample_width(), chh = fh_.color_sample_height();
-  gm_lf_groups_.assign(fh_.num_lf_groups(), {});
-  gm_pass_groups_.assign(num_passes, std::vector<std::vector<GroupChannel>>(fh_.num_groups()));
   for (; i < s.channels.size(); ++i) {
     const ChannelInfo& c = s.channels[i];
     JXLB_CHECK(c.hshift >= 0 && c.vshift >= 0, kErrBitstream, "unshiftable channel outside the global stream");
-    // original size of the image channel this coded channel derives from: every non-meta channel
-    // of a frame-level Modular image spans the colour sample grid (possibly dim-shifted extra
-    // channels, whose original size is still the colour size; lf_global.rs:270-290).
-    uint32_t ow = cw, oh = chh;
-    if (c.hshift < 3 || c.vshift < 3) {
+    // A channel shifted by 3 or more in both directions is coded in the LF groups (8x the group size, in units of
+    // 1 << 3 samples), any other in the pass groups of the pass its shift belongs to.
+    const bool in_lf_groups = c.hshift >= 3 && c.vshift >= 3;
+    const int32_t unit = in_lf_groups ? 3 : 0;
+    std::vector<std::vector<GroupChannel>>* groups = &gm_lf_groups_;
+    if (!in_lf_groups) {
       int32_t shift = std::min(c.hshift, c.vshift);
       int pass = -1;
       for (auto& kv : pass_shifts)
@@ -451,34 +554,60 @@ void FramePlanner::setup_gmodular() {
           break;
         }
       JXLB_CHECK(pass >= 0 && uint32_t(pass) < num_passes, kErrBitstream, "no pass for modular channel shift");
-      uint32_t gw = gd >> c.hshift, gh = gd >> c.vshift;
-      JXLB_CHECK(gw && gh, kErrBitstream, "channel shift too large after transform");
-      uint32_t nx = (ow + gd - 1) >> gshift, ny = (oh + gd - 1) >> gshift;
-      JXLB_CHECK(nx * ny == fh_.num_groups(), kErrBitstream, "modular group count mismatch");
-      for (uint32_t gy = 0; gy < ny; ++gy)
-        for (uint32_t gx = 0; gx < nx; ++gx) {
-          uint32_t x0 = gx * gw, y0 = gy * gh;
-          if (x0 >= c.width || y0 >= c.height) continue;
-          View v{gm_coded_[i].view.plane, x0, y0, std::min(gw, c.width - x0), std::min(gh, c.height - y0)};
-          gm_pass_groups_[pass][gy * nx + gx].push_back({v, c.hshift, c.vshift});
-        }
-    } else {
-      uint32_t gw = gd >> (c.hshift - 3), gh = gd >> (c.vshift - 3);
-      JXLB_CHECK(gw && gh, kErrBitstream, "channel shift too large after transform");
-      uint32_t nx = (ow + (gd << 3) - 1) >> (gshift + 3), ny = (oh + (gd << 3) - 1) >> (gshift + 3);
-      JXLB_CHECK(nx * ny == fh_.num_lf_groups(), kErrBitstream, "modular LF group count mismatch");
-      for (uint32_t gy = 0; gy < ny; ++gy)
-        for (uint32_t gx = 0; gx < nx; ++gx) {
-          uint32_t x0 = gx * gw, y0 = gy * gh;
-          if (x0 >= c.width || y0 >= c.height) continue;
-          View v{gm_coded_[i].view.plane, x0, y0, std::min(gw, c.width - x0), std::min(gh, c.height - y0)};
-          gm_lf_groups_[gy * nx + gx].push_back({v, c.hshift, c.vshift});
-        }
+      groups = &gm_pass_groups_[pass];
     }
+    uint32_t gw = gd >> (c.hshift - unit), gh = gd >> (c.vshift - unit);
+    JXLB_CHECK(gw && gh, kErrBitstream, "channel shift too large after transform");
+    // original size of the image channel this coded channel derives from: every non-meta channel
+    // of a frame-level Modular image spans the colour sample grid (possibly dim-shifted extra
+    // channels, whose original size is still the colour size; lf_global.rs:270-290).
+    uint32_t nx = (cw + (gd << unit) - 1) >> (gshift + unit), ny = (chh + (gd << unit) - 1) >> (gshift + unit);
+    JXLB_CHECK(nx * ny == groups->size(), kErrBitstream,
+               in_lf_groups ? "modular LF group count mismatch" : "modular group count mismatch");
+    for (uint32_t gy = 0; gy < ny; ++gy)
+      for (uint32_t gx = 0; gx < nx; ++gx) {
+        uint32_t x0 = gx * gw, y0 = gy * gh;
+        if (x0 >= c.width || y0 >= c.height) continue;
+        View v{gm_coded_[i].view.plane, x0, y0, std::min(gw, c.width - x0), std::min(gh, c.height - y0)};
+        (*groups)[gy * nx + gx].push_back({v, c.hshift, c.vshift});
+      }
   }
 }
 
 DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_end_byte) {
+  begin_frame(frame_begin_byte, frame_end_byte);
+  decode_lf_global();
+  be_.phase_mark("lf_global");
+  if (vardct_) init_vardct_state();
+  be_.phase_mark("alloc");
+  decode_lf_groups();
+  decode_hf_global();
+  be_.phase_mark("hf_global");
+  decode_pass_groups();
+
+  DecodedFrame out;
+  std::vector<View> colour = samples_to_float(&out);
+  const bool fused_colour = restoration_filters(colour);
+  be_.phase_mark("filters");
+  const std::vector<View> extra = render_features(colour, &out);
+  // the frame's own colour transform, unless the filters applied it
+  const bool converted =
+      colour_transform(colour, extra, colour_.ct_target < 0 || fused_colour, colour_.ct_target, &out) || fused_colour;
+  compose(&out, converted);
+  record(out);
+  if (colour_.defer_ct && role_.shown) {
+    // the composed canvas takes the transform to the requested encoding the frame deferred, the base's region
+    // included (blend.rs:219 gives the canvas the new frame's state); the slot keeps the samples from before it
+    const std::vector<View> canvas = out.channels;
+    colour_transform({canvas.begin(), canvas.begin() + out.num_color}, {canvas.begin() + out.num_color, canvas.end()},
+                     false, opt_.output_colour, &out);
+  }
+  release_planes(&out);
+  be_.phase_mark("filters_colour");
+  return out;
+}
+
+void FramePlanner::begin_frame(size_t frame_begin_byte, size_t* frame_end_byte) {
   BitReader br(cs_, size_, frame_begin_byte * 8);
   be_.phase_mark(nullptr);
   be_.new_frame();
@@ -486,67 +615,56 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
   toc_ = parse_toc(br, fh_);
   *frame_end_byte = toc_.data_begin + toc_.total_size;
   JXLB_CHECK(*frame_end_byte <= size_, kErrEof, "frame data beyond end of codestream");
-
-  const bool vardct = fh_.encoding == Encoding::kVarDct;
-  const bool is_lf_frame = fh_.frame_type == FrameType::kLfFrame;
-  const bool is_ref_frame = fh_.frame_type == FrameType::kReferenceOnly;
-  const bool normal_frame = !is_lf_frame && !is_ref_frame;
-  if (is_lf_frame)
+  role_ = frame_role(fh_, ih_);
+  vardct_ = fh_.encoding == Encoding::kVarDct;
+  if (role_.kind == FrameType::kLfFrame)
     JXLB_CHECK(fh_.lf_level >= 1 && fh_.lf_level <= 4 && fh_.upsampling == 1, kErrBitstream, "invalid LF frame header");
-  // The colour transform a frame applies to its own samples, as an output_colour value, or -1 for none
-  // (render.rs:151-153, image.rs:807-809, util.rs:311-374). An LF frame stays in XYB: it is the next frame's LF image.
-  // A frame saved before the transform keeps its samples as coded (XYB, or YCbCr with do_ycbcr); a regular one that
-  // is not the last frame defers the transform to its keyframe's composed canvas (postprocess_keyframe, lib.rs:925-998).
-  // A reference-only frame saved after it converts to the signalled encoding whatever output was asked for, and
-  // leaves its samples alone under an ICC profile or an XYB / unknown colour space. Every other regular frame converts to
-  // the requested encoding before it is composed; for output_colour 0 with an enum encoding that is the reference's
-  // record conversion.
-  const bool defer_ct = normal_frame && fh_.save_before_ct && !fh_.is_last;
-  const ColourSpace space = ih_.colour_encoding.colour_space;
-  const bool enum_rgb_or_grey = !ih_.colour_encoding.want_icc && (space == ColourSpace::kRgb || space == ColourSpace::kGrey);
-  // the reference's record conversion leaves XYB samples alone: the frame keeps ct_done false
-  const bool record_keeps_xyb = !fh_.do_ycbcr && ih_.xyb_encoded && !enum_rgb_or_grey;
-  int ct_target = opt_.output_colour;
-  if (is_lf_frame || defer_ct || (is_ref_frame && fh_.save_before_ct)) {
-    ct_target = -1;
-  } else if (is_ref_frame) {
-    ct_target = record_keeps_xyb || !(fh_.do_ycbcr || ih_.xyb_encoded) ? -1 : 0;
+  colour_ = colour_plan();
+  if (role_.lf_read >= 0) {
+    JXLB_CHECK(vardct_, kErrBitstream, "use_lf_frame on a Modular frame");
+    JXLB_CHECK(fh_.lf_level < 4 && stores_.lf[fh_.lf_level].valid, kErrBitstream, "frame refers to an LF frame that was not decoded");
   }
-  if (fh_.use_lf_frame()) {
-    JXLB_CHECK(vardct, kErrBitstream, "use_lf_frame on a Modular frame");
-    JXLB_CHECK(fh_.lf_level < 4 && (*lf_store_)[fh_.lf_level].valid, kErrBitstream, "frame refers to an LF frame that was not decoded");
-  }
-  // JPEG chroma subsampling: per-channel shifts (ChannelShift::from_jpeg_upsampling, jxl-modular/src/param.rs:105-122)
-  bool h_subsampling = false, v_subsampling = false;
-  uint32_t chan_hshift[3] = {0, 0, 0}, chan_vshift[3] = {0, 0, 0};
   for (uint32_t j : fh_.jpeg_upsampling) {
-    h_subsampling |= j == 1 || j == 2;
-    v_subsampling |= j == 1 || j == 3;
+    h_subsampled_ |= j == 1 || j == 2;
+    v_subsampled_ |= j == 1 || j == 3;
   }
   for (int c = 0; c < 3; ++c) {
     const uint32_t j = fh_.jpeg_upsampling[c];
-    chan_hshift[c] = (j == 0 || j == 3) && h_subsampling;
-    chan_vshift[c] = (j == 0 || j == 2) && v_subsampling;
+    chan_hshift_[c] = (j == 0 || j == 3) && h_subsampled_;
+    chan_vshift_[c] = (j == 0 || j == 2) && v_subsampled_;
   }
-  const bool chroma_subsampled = h_subsampling || v_subsampling;
-  JXLB_CHECK(!chroma_subsampled || !vardct || fh_.skip_adaptive_lf_smoothing(), kErrUnsupported,
+  JXLB_CHECK(!(h_subsampled_ || v_subsampled_) || !vardct_ || fh_.skip_adaptive_lf_smoothing(), kErrUnsupported,
              "adaptive LF smoothing of a chroma-subsampled frame");
-  // block counts are rounded up to even in a subsampled direction (hf_metadata.rs:70-80, vardct/mod.rs:83-95)
-  auto blocks_w = [&](uint32_t px) { return h_subsampling ? ((px + 7) / 8 + 1) / 2 * 2 : (px + 7) / 8; };
-  auto blocks_h = [&](uint32_t px) { return v_subsampling ? ((px + 7) / 8 + 1) / 2 * 2 : (px + 7) / 8; };
+}
 
-  const uint32_t num_lf_groups = fh_.num_lf_groups(), num_groups = fh_.num_groups();
-  const uint32_t num_passes = fh_.passes.num_passes;
-  const bool single = toc_.single_entry();
-  const uint32_t cw = fh_.color_sample_width(), chh = fh_.color_sample_height();
+// An LF frame stays in XYB: it is the next frame's LF image. A frame saved before the transform keeps its samples as
+// coded (XYB, or YCbCr with do_ycbcr); a regular one that is not the last frame defers the transform to its keyframe's
+// composed canvas (postprocess_keyframe, lib.rs:925-998). A reference-only frame saved after it converts to the
+// signalled encoding whatever output was asked for, and leaves its samples alone under an ICC profile or an XYB /
+// unknown colour space. Every other regular frame converts to the requested encoding before it is composed; for
+// output_colour 0 with an enum encoding that is the reference's record conversion.
+ColourPlan FramePlanner::colour_plan() const {
+  const bool ref_only = role_.kind == FrameType::kReferenceOnly;
+  ColourPlan p;
+  p.defer_ct = role_.regular() && fh_.save_before_ct && !fh_.is_last;
+  const ColourSpace space = ih_.colour_encoding.colour_space;
+  const bool enum_rgb_or_grey = !ih_.colour_encoding.want_icc && (space == ColourSpace::kRgb || space == ColourSpace::kGrey);
+  p.record_keeps_xyb = !fh_.do_ycbcr && ih_.xyb_encoded && !enum_rgb_or_grey;
+  p.ct_target = opt_.output_colour;
+  if (role_.kind == FrameType::kLfFrame || p.defer_ct || (ref_only && fh_.save_before_ct)) {
+    p.ct_target = -1;
+  } else if (ref_only) {
+    p.ct_target = p.record_keeps_xyb || !(fh_.do_ycbcr || ih_.xyb_encoded) ? -1 : 0;
+  }
+  return p;
+}
 
-  // ---- LfGlobal ----
-  size_t pos, limit;
-  section(0, &pos, &limit);
+void FramePlanner::decode_lf_global() {
+  section(0, &pos_, &limit_);
   {
-    BitReader r = reader_at(pos, limit);
+    BitReader r = reader_at(pos_, limit_);
     lfg_ = parse_lf_global(r, ih_, fh_);
-    pos = r.pos();
+    pos_ = r.pos();
   }
   // With patches the reference brings an extra channel to the colour resolution first, blends, then upsamples it with
   // the colour channels (render.rs:159-175, image.rs:487-557 with ec_to_color_only): a different chain, not restated.
@@ -554,227 +672,176 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
     JXLB_CHECK(!lfg_.has_patches || ec_shift(i) == ceil_log2_nonzero(fh_.upsampling), kErrUnsupported,
                "patches on a frame whose extra channel is upsampled apart from the colour channels are not implemented");
   // full-size float planes of the extra channels upsampled here, each with at most a quarter-size chain intermediate
-  size_t ec_render_bytes = 0;
+  ec_render_bytes_ = 0;
   for (size_t i = 0; i < ih_.ec_info.size(); ++i)
-    if (ec_shift(i)) ec_render_bytes += size_t(fh_.width) * fh_.height * 4 + size_t(fh_.width) * fh_.height;
+    if (ec_shift(i)) ec_render_bytes_ += size_t(fh_.width) * fh_.height * 4 + size_t(fh_.width) * fh_.height;
   // noise on an upsampled frame: its three f32 field planes have the upsampled size
-  if (lfg_.has_noise && fh_.upsampling > 1) ec_render_bytes += size_t(fh_.width) * fh_.height * 4 * 3;
-  if (lfg_.has_gmodular) {
-    // a Modular image allocates its full-size channels up front (coded channels, then one plane per inverse transform)
-    if (!vardct)
-      be_.begin_heavy_stage(size_t(cw) * chh * 4 * 2 * (lfg_.gmodular.channels.size() + 2) + ec_render_bytes + (size_t(64) << 20));
-    setup_gmodular();
-    std::vector<ModularStreamJob> jobs(1);
-    ModularStreamJob& job = jobs[0];
-    job.bit_pos = pos;
-    job.bit_limit = limit * 8;
-    job.tree = tree_for(lfg_.gmodular);
-    job.wp = lfg_.gmodular.header.wp;
-    job.stream_index = 0;
-    for (size_t i = 0; i < gm_global_count_; ++i) {
-      const ChannelInfo& c = lfg_.gmodular.channels[i];
-      job.channels.push_back({gm_coded_[i].view, c.hshift, c.vshift});
-    }
-    be_.decode_modular(jobs);
-    pos = jobs[0].end_bit;
-  } else {
-    gm_lf_groups_.assign(num_lf_groups, {});
-    gm_pass_groups_.assign(num_passes, std::vector<std::vector<GroupChannel>>(num_groups));
+  if (lfg_.has_noise && fh_.upsampling > 1) ec_render_bytes_ += size_t(fh_.width) * fh_.height * 4 * 3;
+  gm_lf_groups_.assign(fh_.num_lf_groups(), {});
+  gm_pass_groups_.assign(fh_.passes.num_passes, std::vector<std::vector<GroupChannel>>(fh_.num_groups()));
+  if (!lfg_.has_gmodular) return;
+  // a Modular image allocates its full-size channels up front (coded channels, then one plane per inverse transform)
+  if (!vardct_)
+    be_.begin_heavy_stage(size_t(fh_.color_sample_width()) * fh_.color_sample_height() * 4 * 2 *
+                              (lfg_.gmodular.channels.size() + 2) + ec_render_bytes_ + (size_t(64) << 20));
+  setup_gmodular();
+  std::vector<ModularStreamJob> jobs(1);
+  ModularStreamJob& job = jobs[0];
+  job.bit_pos = pos_;
+  job.bit_limit = limit_ * 8;
+  job.tree = tree_for(lfg_.gmodular);
+  job.wp = lfg_.gmodular.header.wp;
+  job.stream_index = 0;
+  for (size_t i = 0; i < gm_global_count_; ++i) {
+    const ChannelInfo& c = lfg_.gmodular.channels[i];
+    job.channels.push_back({gm_coded_[i].view, c.hshift, c.vshift});
   }
+  be_.decode_modular(jobs);
+  pos_ = jobs[0].end_bit;
+}
 
-  be_.phase_mark("lf_global");
-  // ---- VarDCT frame state ----
-  if (vardct) {
-    st_ = VarDctState();
-    st_.width = cw;
-    st_.height = chh;
-    st_.bw = blocks_w(cw);
-    st_.bh = blocks_h(chh);
-    st_.subsampled = chroma_subsampled;
-    for (int c = 0; c < 3; ++c) st_.hshift[c] = chan_hshift[c], st_.vshift[c] = chan_vshift[c];
-    st_.group_dim = fh_.group_dim();
-    st_.groups_per_row = fh_.groups_per_row();
-    st_.num_groups = num_groups;
-    st_.lfg = &lfg_;
-    st_.hfg = &hfg_;
-    st_.fh = &fh_;
-    st_.ih = &ih_;
-    st_.use_lf_frame = fh_.use_lf_frame();
-    if (st_.use_lf_frame) {
-      const LfFrameStore& lf = (*lf_store_)[fh_.lf_level];
-      JXLB_CHECK(lf.planes[0].w == st_.bw && lf.planes[0].h == st_.bh, kErrBitstream, "LF frame size does not match the frame");
-    }
-    for (int c = 0; c < 3; ++c) {
-      st_.lf_quant[c] = new_plane(st_.bw, st_.bh);
-      st_.lf[c] = new_plane(st_.bw, st_.bh);
-    }  // the coefficient planes are allocated when the pass groups are reached (begin_heavy_stage)
-    st_.x_from_y = new_plane((cw + 63) / 64, (chh + 63) / 64);
-    st_.b_from_y = new_plane((cw + 63) / 64, (chh + 63) / 64);
-    st_.sharpness = new_plane(st_.bw, st_.bh);
-    st_.blk_type = new_plane(st_.bw, st_.bh);
-    st_.blk_mul = new_plane(st_.bw, st_.bh);
-    st_.epf_sigma = new_plane(st_.bw, st_.bh);
+void FramePlanner::init_vardct_state() {
+  const uint32_t cw = fh_.color_sample_width(), chh = fh_.color_sample_height();
+  st_ = VarDctState();
+  st_.width = cw;
+  st_.height = chh;
+  st_.bw = blocks_w(cw);
+  st_.bh = blocks_h(chh);
+  st_.subsampled = h_subsampled_ || v_subsampled_;
+  for (int c = 0; c < 3; ++c) st_.hshift[c] = chan_hshift_[c], st_.vshift[c] = chan_vshift_[c];
+  st_.group_dim = fh_.group_dim();
+  st_.groups_per_row = fh_.groups_per_row();
+  st_.num_groups = fh_.num_groups();
+  st_.lfg = &lfg_;
+  st_.hfg = &hfg_;
+  st_.fh = &fh_;
+  st_.ih = &ih_;
+  st_.use_lf_frame = fh_.use_lf_frame();
+  if (st_.use_lf_frame) {
+    const StoredFrame& lf = stores_.lf[fh_.lf_level];
+    JXLB_CHECK(lf.channels[0].w == st_.bw && lf.channels[0].h == st_.bh, kErrBitstream, "LF frame size does not match the frame");
   }
+  for (int c = 0; c < 3; ++c) {
+    st_.lf_quant[c] = new_plane(st_.bw, st_.bh);
+    st_.lf[c] = new_plane(st_.bw, st_.bh);
+  }  // the coefficient planes are allocated when the pass groups are reached (begin_heavy_stage)
+  st_.x_from_y = new_plane((cw + 63) / 64, (chh + 63) / 64);
+  st_.b_from_y = new_plane((cw + 63) / 64, (chh + 63) / 64);
+  st_.sharpness = new_plane(st_.bw, st_.bh);
+  st_.blk_type = new_plane(st_.bw, st_.bh);
+  st_.blk_mul = new_plane(st_.bw, st_.bh);
+  st_.epf_sigma = new_plane(st_.bw, st_.bh);
+}
 
-  be_.phase_mark("alloc");
-  // ---- LfGroups: three entropy-coded streams each, at data-dependent bit offsets ----
-  std::vector<size_t> lf_pos(num_lf_groups), lf_limit(num_lf_groups);
-  std::vector<LfGroupRect> lf_rect(num_lf_groups);
+// LfGroups: three entropy-coded streams each, at data-dependent bit offsets
+void FramePlanner::decode_lf_groups() {
+  const uint32_t num_lf_groups = fh_.num_lf_groups();
+  const uint32_t cw = fh_.color_sample_width(), chh = fh_.color_sample_height();
+  lf_pos_.assign(num_lf_groups, pos_);
+  lf_limit_.assign(num_lf_groups, limit_);
+  lf_rect_.assign(num_lf_groups, {});
   for (uint32_t g = 0; g < num_lf_groups; ++g) {
-    if (single) {
-      lf_pos[g] = pos;
-      lf_limit[g] = limit;
-    } else {
-      section(1 + g, &lf_pos[g], &lf_limit[g]);
-    }
+    if (!toc_.single_entry()) section(1 + g, &lf_pos_[g], &lf_limit_[g]);
     uint32_t gx = g % fh_.lf_groups_per_row(), gy = g / fh_.lf_groups_per_row();
     uint32_t lfd = fh_.lf_group_dim();
     uint32_t lw = std::min(lfd, cw - gx * lfd), lh = std::min(lfd, chh - gy * lfd);
-    lf_rect[g] = {gx * (lfd / 8), gy * (lfd / 8), blocks_w(lw), blocks_h(lh)};
+    lf_rect_[g] = {gx * (lfd / 8), gy * (lfd / 8), blocks_w(lw), blocks_h(lh)};
   }
-  lf_rect_ = lf_rect;
   extra_precision_.assign(num_lf_groups, 0);
-  if (vardct && !fh_.use_lf_frame()) {  // LfCoeff (jxl-vardct/src/lf.rs:138-181; absent with an LF frame)
-    std::vector<ModularStreamJob> jobs;
-    std::vector<PendingStream> pend;
-    for (uint32_t g = 0; g < num_lf_groups; ++g) {
-      BitReader r = reader_at(lf_pos[g], lf_limit[g]);
+  if (vardct_ && !fh_.use_lf_frame()) {  // LfCoeff (jxl-vardct/src/lf.rs:138-181; absent with an LF frame)
+    decode_streams(lf_pos_, lf_limit_, 1, [&](uint32_t g, BitReader& r, VarblockPlacement*) {
       extra_precision_[g] = r.read(2);
-      const LfGroupRect& rc = lf_rect[g];
       std::vector<GroupChannel> chans;
       for (int mc : {1, 0, 2}) {  // modular channel order is Y, X, B
-        const LfGroupRect sr = shifted_rect(rc, st_.hshift[mc], st_.vshift[mc]);
+        const LfGroupRect sr = shifted_rect(lf_rect_[g], st_.hshift[mc], st_.vshift[mc]);
         chans.push_back({View{st_.lf_quant[mc], sr.bx0, sr.by0, sr.bw, sr.bh}, int32_t(st_.hshift[mc]), int32_t(st_.vshift[mc])});
       }
-      pend.push_back(prepare_stream(r, lf_limit[g], chans, 1 + g, &jobs));
-    }
-    be_.decode_modular(jobs);
-    for (uint32_t g = 0; g < num_lf_groups; ++g) {
-      finish_stream(pend[g]);
-      lf_pos[g] = jobs[pend[g].job_index].end_bit;
-    }
+      return chans;
+    });
   }
   be_.phase_mark("lf_coeff");
-  {  // Modular LF-group channels (jxl-frame/src/data/lf_group.rs:76-91)
-    std::vector<ModularStreamJob> jobs;
-    std::vector<PendingStream> pend;
-    std::vector<uint32_t> owner;
-    for (uint32_t g = 0; g < num_lf_groups; ++g) {
-      if (gm_lf_groups_[g].empty()) continue;
-      BitReader r = reader_at(lf_pos[g], lf_limit[g]);
-      pend.push_back(prepare_stream(r, lf_limit[g], gm_lf_groups_[g], 1 + num_lf_groups + g, &jobs));
-      owner.push_back(g);
-    }
-    if (!jobs.empty()) be_.decode_modular(jobs);
-    for (size_t k = 0; k < pend.size(); ++k) {
-      finish_stream(pend[k]);
-      lf_pos[owner[k]] = jobs[pend[k].job_index].end_bit;
-    }
-  }
+  // Modular LF-group channels (jxl-frame/src/data/lf_group.rs:76-91)
+  decode_streams(lf_pos_, lf_limit_, 1 + num_lf_groups,
+                 [&](uint32_t g, BitReader&, VarblockPlacement*) { return gm_lf_groups_[g]; });
   be_.phase_mark("mlf");
-  if (vardct) {  // HfMetadata (jxl-vardct/src/hf_metadata.rs:52-230)
-    std::vector<ModularStreamJob> jobs;
-    std::vector<PendingStream> pend;
-    std::vector<BlockInfoJob> bjobs;
-    for (uint32_t g = 0; g < num_lf_groups; ++g) {
-      BitReader r = reader_at(lf_pos[g], lf_limit[g]);
-      const LfGroupRect& rc = lf_rect[g];
-      uint32_t nb_blocks = 1 + r.read(ceil_log2_nonzero(rc.bw * rc.bh));
-      uint32_t w64 = (rc.bw + 7) / 8, h64 = (rc.bh + 7) / 8;
-      int raw = new_plane(nb_blocks, 2);
-      std::vector<GroupChannel> chans;
-      chans.push_back({View{st_.x_from_y, rc.bx0 / 8, rc.by0 / 8, w64, h64}, 0, 0});
-      chans.push_back({View{st_.b_from_y, rc.bx0 / 8, rc.by0 / 8, w64, h64}, 0, 0});
-      chans.push_back({View{raw, 0, 0, nb_blocks, 2}, 0, 0});
-      chans.push_back({View{st_.sharpness, rc.bx0, rc.by0, rc.bw, rc.bh}, 0, 0});
-      pend.push_back(prepare_stream(r, lf_limit[g], chans, 1 + 2 * num_lf_groups + g, &jobs));
-      bjobs.push_back({rc, raw, nb_blocks});
-      // without Modular transforms the stream's own output is final: the backend may place right after the stream
-      if (pend.back().direct) jobs[pend.back().job_index].placement = varblock_placement(st_, bjobs.back());
-    }
-    be_.decode_modular(jobs);
-    for (uint32_t g = 0; g < num_lf_groups; ++g) {
-      finish_stream(pend[g]);
-      lf_pos[g] = jobs[pend[g].job_index].end_bit;
-    }
-    std::vector<BlockInfoJob> rest;  // LF groups the backend did not place with their stream
-    for (uint32_t g = 0; g < num_lf_groups; ++g) {
-      const ModularStreamJob& j = jobs[pend[g].job_index];
-      if (j.placed) JXLB_CHECK(j.layout_ok, kErrBitstream, "invalid HfMetadata block layout");
-      else rest.push_back(bjobs[g]);
-    }
-    if (!rest.empty()) be_.build_block_info(st_, rest);
-    for (auto& b : bjobs) drop_plane(b.raw_plane);
-  }
+  if (vardct_) decode_hf_metadata();
   be_.phase_mark("hf_metadata");
-  if (single) pos = lf_pos[0];
+  if (toc_.single_entry()) pos_ = lf_pos_[0];
+}
 
-  // ---- HfGlobal ----
-  if (vardct) {
-    size_t hpos = pos, hlimit = limit;
-    if (!single) section(1 + num_lf_groups, &hpos, &hlimit);
-    BitReader r = reader_at(hpos, hlimit);
-    // raw dequant tables (JPEG transcodes): an inline Modular image per table, decoded by the backend like any other
-    // stream and read back - the matrices are built on the host
-    RawTableDecoder raw_decoder = [&](BitReader& br, uint32_t w, uint32_t h, uint32_t stream_index, std::vector<int32_t> out[3]) {
-      std::vector<GroupChannel> chans;
-      std::vector<int> planes;
-      for (int c = 0; c < 3; ++c) {
-        planes.push_back(new_plane(w, h));
-        chans.push_back({View{planes[c], 0, 0, w, h}, 0, 0});
-      }
-      std::vector<ModularStreamJob> jobs;
-      PendingStream ps = prepare_stream(br, hlimit, chans, stream_index, &jobs);
-      be_.decode_modular(jobs);
-      finish_stream(ps);
-      for (int c = 0; c < 3; ++c) {
-        out[c].resize(size_t(w) * h);
-        be_.download_rect(chans[c].view, out[c].data());
-        drop_plane(planes[c]);
-      }
-      br = BitReader(cs_, hlimit, jobs[ps.job_index].end_bit);
-    };
-    hfg_ = parse_hf_global(r, ih_, fh_, lfg_, raw_decoder);
-    if (single) pos = r.pos();
+// HfMetadata (jxl-vardct/src/hf_metadata.rs:52-230)
+void FramePlanner::decode_hf_metadata() {
+  std::vector<BlockInfoJob> bjobs;
+  const std::vector<ModularStreamJob> jobs =
+      decode_streams(lf_pos_, lf_limit_, 1 + 2 * fh_.num_lf_groups(), [&](uint32_t g, BitReader& r, VarblockPlacement* placement) {
+        const LfGroupRect& rc = lf_rect_[g];
+        uint32_t nb_blocks = 1 + r.read(ceil_log2_nonzero(rc.bw * rc.bh));
+        uint32_t w64 = (rc.bw + 7) / 8, h64 = (rc.bh + 7) / 8;
+        int raw = new_plane(nb_blocks, 2);
+        bjobs.push_back({rc, raw, nb_blocks});
+        *placement = varblock_placement(st_, bjobs.back());
+        return std::vector<GroupChannel>{{View{st_.x_from_y, rc.bx0 / 8, rc.by0 / 8, w64, h64}, 0, 0},
+                                         {View{st_.b_from_y, rc.bx0 / 8, rc.by0 / 8, w64, h64}, 0, 0},
+                                         {View{raw, 0, 0, nb_blocks, 2}, 0, 0},
+                                         {View{st_.sharpness, rc.bx0, rc.by0, rc.bw, rc.bh}, 0, 0}};
+      });
+  std::vector<BlockInfoJob> rest;  // LF groups the backend did not place with their stream
+  for (size_t g = 0; g < jobs.size(); ++g) {
+    if (jobs[g].placed) JXLB_CHECK(jobs[g].layout_ok, kErrBitstream, "invalid HfMetadata block layout");
+    else rest.push_back(bjobs[g]);
   }
+  if (!rest.empty()) be_.build_block_info(st_, rest);
+  for (auto& b : bjobs) drop_plane(b.raw_plane);
+}
 
-  be_.phase_mark("hf_global");
-  if (vardct) {
+void FramePlanner::decode_hf_global() {
+  if (!vardct_) return;
+  size_t hpos = pos_, hlimit = limit_;
+  if (!toc_.single_entry()) section(1 + fh_.num_lf_groups(), &hpos, &hlimit);
+  BitReader r = reader_at(hpos, hlimit);
+  // raw dequant tables (JPEG transcodes): an inline Modular image per table, decoded by the backend like any other
+  // stream and read back - the matrices are built on the host
+  RawTableDecoder raw_decoder = [&](BitReader& br, uint32_t w, uint32_t h, uint32_t stream_index, std::vector<int32_t> out[3]) {
+    std::vector<size_t> pos{br.pos()};
+    std::vector<GroupChannel> chans;
+    decode_streams(pos, {hlimit}, stream_index, [&](uint32_t, BitReader&, VarblockPlacement*) {
+      for (int c = 0; c < 3; ++c) chans.push_back({View{new_plane(w, h), 0, 0, w, h}, 0, 0});
+      return chans;
+    });
+    for (int c = 0; c < 3; ++c) {
+      out[c].resize(size_t(w) * h);
+      be_.download_rect(chans[c].view, out[c].data());
+      drop_plane(chans[c].view.plane);
+    }
+    br = BitReader(cs_, hlimit, pos[0]);
+  };
+  hfg_ = parse_hf_global(r, ih_, fh_, lfg_, raw_decoder);
+  if (toc_.single_entry()) pos_ = r.pos();
+}
+
+// PassGroups, then the global inverse transforms of the frame's Modular image
+void FramePlanner::decode_pass_groups() {
+  const uint32_t num_lf_groups = fh_.num_lf_groups(), num_groups = fh_.num_groups();
+  if (vardct_) {
     // Everything so far worked on 1/64 of the samples; from here on the frame needs its full-resolution planes
     // (3 coefficient planes that become the pixels in place + 3 planes of filter output).
-    be_.begin_heavy_stage(size_t(st_.bw) * st_.bh * 64 * 4 * 6 + ec_render_bytes + (size_t(64) << 20));
+    be_.begin_heavy_stage(size_t(st_.bw) * st_.bh * 64 * 4 * 6 + ec_render_bytes_ + (size_t(64) << 20));
     be_.phase_mark("heavy_wait");
     for (int c = 0; c < 3; ++c) st_.coeff[c] = new_plane(st_.bw * 8, st_.bh * 8, /*zero=*/true);
   }
-  // ---- PassGroups ----
-  for (uint32_t p = 0; p < num_passes; ++p) {
-    std::vector<size_t> gpos(num_groups), glimit(num_groups);
-    for (uint32_t g = 0; g < num_groups; ++g) {
-      if (single) {
-        gpos[g] = pos;
-        glimit[g] = limit;
-      } else {
-        section(2 + num_lf_groups + p * num_groups + g, &gpos[g], &glimit[g]);
-      }
-    }
-    if (vardct) {
+  for (uint32_t p = 0; p < fh_.passes.num_passes; ++p) {
+    std::vector<size_t> gpos(num_groups, pos_), glimit(num_groups, limit_);
+    if (!toc_.single_entry())
+      for (uint32_t g = 0; g < num_groups; ++g) section(2 + num_lf_groups + p * num_groups + g, &gpos[g], &glimit[g]);
+    if (vardct_) {
       std::vector<HfGroupJob> jobs(num_groups);
       for (uint32_t g = 0; g < num_groups; ++g) jobs[g] = {gpos[g], glimit[g] * 8, g, p, 0};
       be_.decode_hf(st_, jobs);
       for (uint32_t g = 0; g < num_groups; ++g) gpos[g] = jobs[g].end_bit;
     }
-    std::vector<ModularStreamJob> jobs;
-    std::vector<PendingStream> pend;
-    for (uint32_t g = 0; g < num_groups; ++g) {
-      if (gm_pass_groups_[p][g].empty()) continue;
-      BitReader r = reader_at(gpos[g], glimit[g]);
-      pend.push_back(prepare_stream(r, glimit[g], gm_pass_groups_[p][g],
-                                    1 + 3 * num_lf_groups + 17 + p * num_groups + g, &jobs));
-    }
-    if (!jobs.empty()) be_.decode_modular(jobs);
-    for (auto& ps : pend) finish_stream(ps);
+    decode_streams(gpos, glimit, 1 + 3 * num_lf_groups + 17 + p * num_groups,
+                   [&](uint32_t g, BitReader&, VarblockPlacement*) { return gm_pass_groups_[p][g]; });
   }
-
   be_.phase_mark("pass_groups");
   {  // the decoded (still transformed) channels of the frame's Modular image, coding order; none when it has no such image
     std::vector<View> coded;
@@ -782,35 +849,29 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
       for (const ChanBuf& c : gm_coded_) coded.push_back(c.view);
     be_.stage_marker("modular_coded", coded.data(), int(coded.size()));
   }
-  // ---- global inverse transforms ----
-  std::vector<ChanBuf> gm_image = gm_coded_;
-  if (lfg_.has_gmodular) run_inverse_transforms(lfg_.gmodular, gm_image);
-
+  gm_image_ = gm_coded_;
+  if (lfg_.has_gmodular) run_inverse_transforms(lfg_.gmodular, gm_image_);
   be_.phase_mark("inverse_transforms");
-  // ---- render ----
-  DecodedFrame out;
-  out.header = fh_;
-  out.width = cw;
-  out.height = chh;
+}
+
+// The frame's colour channels as float samples at the colour sample size: VarDCT rendered, Modular converted, chroma
+// upsampled. The extra channels stay in gm_image_ from ec_from_ on.
+std::vector<View> FramePlanner::samples_to_float(DecodedFrame* out) {
+  const uint32_t cw = fh_.color_sample_width(), chh = fh_.color_sample_height();
+  out->header = fh_;
+  out->width = cw;
+  out->height = chh;
   std::vector<View> colour;
-  size_t ec_from = 0;
-  if (vardct) {
-    render_vardct(&out);
-    for (int c = 0; c < 3; ++c) {
-      if (st_.hshift[c] || st_.vshift[c]) {  // upsample_jpeg (jxl-render/src/image.rs:448-486, filter/ycbcr.rs)
-        const View sub{st_.coeff[c], 0, 0, (cw + st_.hshift[c]) >> st_.hshift[c], (chh + st_.vshift[c]) >> st_.vshift[c]};
-        const int id = be_.upsample_jpeg(sub, st_.hshift[c] != 0, st_.vshift[c] != 0, cw, chh);
-        frame_planes_.push_back(id);
-        colour.push_back(View{id, 0, 0, cw, chh});
-      } else {
-        colour.push_back(View{st_.coeff[c], 0, 0, cw, chh});
-      }
-    }
+  ec_from_ = 0;
+  if (vardct_) {
+    render_vardct();
+    for (int c = 0; c < 3; ++c)
+      colour.push_back(upsample_chroma(View{st_.coeff[c], 0, 0, (cw + st_.hshift[c]) >> st_.hshift[c], (chh + st_.vshift[c]) >> st_.vshift[c]}, c));
     if (st_.subsampled) be_.stage_marker("jpeg_upsampled", colour.data(), 3);
   } else {
-    ec_from = fh_.encoded_color_channels;
-    JXLB_CHECK(gm_image.size() >= ec_from, kErrBitstream, "missing modular colour channels");
-    for (size_t c = 0; c < ec_from; ++c) colour.push_back(gm_image[c].view);
+    ec_from_ = fh_.encoded_color_channels;
+    JXLB_CHECK(gm_image_.size() >= ec_from_, kErrBitstream, "missing modular colour channels");
+    for (size_t c = 0; c < ec_from_; ++c) colour.push_back(gm_image_[c].view);
     if (ih_.xyb_encoded) {
       JXLB_CHECK(colour.size() == 3, kErrBitstream, "XYB modular frame needs three channels");
       View yxb[3] = {colour[0], colour[1], colour[2]};
@@ -821,306 +882,283 @@ DecodedFrame FramePlanner::decode_frame(size_t frame_begin_byte, size_t* frame_e
     }
     if (fh_.do_ycbcr) {  // Cb, Y, Cr at their coded sizes to the colour size (render.rs:70-72, image.rs:448-486)
       JXLB_CHECK(colour.size() == 3, kErrBitstream, "YCbCr needs three channels");
-      for (int c = 0; c < 3; ++c) {
-        if (chan_hshift[c] || chan_vshift[c]) {
-          const int id = be_.upsample_jpeg(colour[c], chan_hshift[c] != 0, chan_vshift[c] != 0, cw, chh);
-          frame_planes_.push_back(id);
-          colour[c] = View{id, 0, 0, cw, chh};
-        } else {  // a channel rounded up to an even size in a subsampled direction is cropped
-          colour[c].w = cw;
-          colour[c].h = chh;
-        }
-      }
+      for (int c = 0; c < 3; ++c) colour[c] = upsample_chroma(colour[c], c);
       be_.stage_marker("jpeg_upsampled", colour.data(), 3);
     }
   }
   be_.phase_mark("render_vardct");
   be_.stage_marker("pre_filter", colour.data(), int(colour.size()));
+  return colour;
+}
 
-  // restoration filters (render.rs:76-131)
+// The restoration filters (render.rs:76-131), with the frame's colour transform fused in when the backend offers it and
+// nothing runs between the two. Returns true when the planes were converted.
+bool FramePlanner::restoration_filters(const std::vector<View>& colour) {
   const RestorationFilter& rf = fh_.restoration_filter;
-  const bool upsampled = fh_.upsampling > 1;
-  bool colour_done = ct_target < 0;
-  bool converted = false;  // the frame's samples went through a colour transform here
-  if (rf.gab_enabled || rf.epf.iters > 0) {
-    // a grayscale frame is filtered as three identical channels and truncated again (render.rs:74-134)
-    JXLB_CHECK(colour.size() == 3 || colour.size() == 1, kErrUnsupported, "restoration filters need one or three colour channels");
-    View v[3];
-    for (int c = 0; c < 3; ++c) {
-      if (size_t(c) < colour.size()) {
-        v[c] = colour[c];
-      } else {
-        int id = new_plane(colour[0].w, colour[0].h);
-        v[c] = View{id, 0, 0, colour[0].w, colour[0].h};
-        be_.copy_rect(colour[0], v[c]);
-      }
-    }
-    View sigma_view;
-    if (vardct) sigma_view = View{st_.epf_sigma, 0, 0, st_.bw, st_.bh};
-    if (vardct && rf.epf.iters > 0) be_.stage_marker("epf_sigma", &sigma_view, 1);
-    ColorParams cp;
-    // colour conversion follows upsampling (render.rs:136-149), so it is fused only without it
-    const bool want_colour = !upsampled && !colour_done && !lfg_.has_noise && !lfg_.has_patches && !lfg_.has_splines &&
-                             colour_params(ih_.xyb_encoded, colour.size(), ct_target, &cp) && !cp.second_stage && cp.gamma == 0.0f &&
-                             cp.pq_intensity_target == 0.0f;
-    if (be_.filters_colour_fused(v, rf, sigma_view, !vardct, want_colour ? &cp : nullptr)) {
-      colour_done = converted = want_colour;
-      if (want_colour) be_.stage_marker("rgb", v, 3);
+  if (!(rf.gab_enabled || rf.epf.iters > 0)) return false;
+  // a grayscale frame is filtered as three identical channels and truncated again (render.rs:74-134)
+  JXLB_CHECK(colour.size() == 3 || colour.size() == 1, kErrUnsupported, "restoration filters need one or three colour channels");
+  View v[3];
+  for (int c = 0; c < 3; ++c) {
+    if (size_t(c) < colour.size()) {
+      v[c] = colour[c];
     } else {
-      if (rf.gab_enabled) {
-        be_.gaborish(v, rf.gab_weights);
-        be_.stage_marker("gaborish", v, 3);
-      }
-      if (rf.epf.iters > 0) {
-        be_.epf(v, sigma_view, rf.epf, !vardct);
-        be_.stage_marker("epf", v, 3);
-      }
+      int id = new_plane(colour[0].w, colour[0].h);
+      v[c] = View{id, 0, 0, colour[0].w, colour[0].h};
+      be_.copy_rect(colour[0], v[c]);
     }
   }
+  View sigma_view;
+  if (vardct_) sigma_view = View{st_.epf_sigma, 0, 0, st_.bw, st_.bh};
+  if (vardct_ && rf.epf.iters > 0) be_.stage_marker("epf_sigma", &sigma_view, 1);
+  ColorParams cp;
+  // colour conversion follows upsampling (render.rs:136-149), so it is fused only without it
+  const bool want_colour = fh_.upsampling == 1 && colour_.ct_target >= 0 && !lfg_.has_noise && !lfg_.has_patches &&
+                           !lfg_.has_splines && colour_params(ih_.xyb_encoded, colour.size(), colour_.ct_target, &cp) &&
+                           !cp.second_stage && cp.gamma == 0.0f && cp.pq_intensity_target == 0.0f;
+  if (be_.filters_colour_fused(v, rf, sigma_view, !vardct_, want_colour ? &cp : nullptr)) {
+    if (want_colour) be_.stage_marker("rgb", v, 3);
+    return want_colour;
+  }
+  if (rf.gab_enabled) {
+    be_.gaborish(v, rf.gab_weights);
+    be_.stage_marker("gaborish", v, 3);
+  }
+  if (rf.epf.iters > 0) {
+    be_.epf(v, sigma_view, rf.epf, !vardct_);
+    be_.stage_marker("epf", v, 3);
+  }
+  return false;
+}
 
-  be_.phase_mark("filters");
-  // non-separable upsampling of every channel (render.rs:136-183), cropped to the frame size
-  auto upsample_view = [&](View& v, uint32_t factor_log2) {
-    int id = be_.upsample(v, factor_log2, ih_);
-    frame_planes_.push_back(id);
-    v = View{id, 0, 0, std::min(v.w << factor_log2, fh_.width), std::min(v.h << factor_log2, fh_.height)};
-  };
-  // render_features (jxl-render/src/render.rs:136-225) runs on the grid before it is upsampled: splines and noise land on
-  // the colour channels at the coded resolution, in frame coordinates (the upsampled size) clipped to the coded planes.
-  // Patches are blended below, after upsampling, while the reference blends them on the coded colour channels
-  // (render.rs:182-196 brings only the extra channels to the colour resolution), so an upsampled frame with patches and
-  // splines or noise is refused rather than drawn in the wrong order.
-  auto splines_and_noise = [&]() {
-    if (lfg_.has_splines) {
-      JXLB_CHECK(colour.size() == 3, kErrUnsupported, "splines need three colour channels");
-      const std::vector<Backend::SplineArc> arcs =
-          build_spline_arcs(lfg_, vardct, vardct ? lfg_.base_correlation_x : 0.0f, vardct ? lfg_.base_correlation_b : 1.0f, fh_.width, fh_.height);
-      View v[3] = {colour[0], colour[1], colour[2]};
-      be_.splat_splines(v, arcs);
-      be_.stage_marker("splines", v, 3);
-    }
-    if (lfg_.has_noise) {
-      JXLB_CHECK(colour.size() == 3 && ih_.xyb_encoded, kErrUnsupported, "noise synthesis is implemented for XYB colour frames");
-      View v[3] = {colour[0], colour[1], colour[2]};
-      const float corr_x = vardct ? lfg_.base_correlation_x : 0.0f, corr_b = vardct ? lfg_.base_correlation_b : 1.0f;
-      // a shown frame counts itself among the visible ones; a hidden one among the invisible ones
-      const bool shown = !is_lf_frame && !is_ref_frame;
-      const uint64_t seed0 = shown ? ((visible_before_ + 1) << 32) : (visible_before_ << 32) + invisible_before_ + 1;
-      // the field has the frame's size (noise.rs:94-100): the upsampled size, or the planes' own without upsampling
-      if (upsampled) be_.add_noise_in_frame(v, fh_.width, fh_.height, lfg_.noise_lut, fh_.group_dim(), seed0, corr_x, corr_b);
-      else be_.add_noise(v, lfg_.noise_lut, fh_.group_dim(), seed0, corr_x, corr_b);
-      be_.stage_marker("noise", v, 3);
-    }
-  };
+// render_features (jxl-render/src/render.rs:136-225) and upsampling, in the reference's order. Splines and noise land
+// on the colour channels at the coded resolution, before upsampling, in frame coordinates (the upsampled size) clipped
+// to the coded planes. Patches are blended after upsampling, while the reference blends them on the coded colour
+// channels (render.rs:182-196 brings only the extra channels to the colour resolution), so an upsampled frame with
+// patches and splines or noise is refused rather than drawn in the wrong order. Returns the extra channels as floats
+// with their own bit depth (they take part in patch blending), each upsampled from its coded size by its whole factor
+// in one chain (image.rs:487-557).
+std::vector<View> FramePlanner::render_features(std::vector<View>& colour, DecodedFrame* out) {
+  const bool upsampled = fh_.upsampling > 1;
   if (upsampled) {
     JXLB_CHECK(!lfg_.has_patches || !(lfg_.has_splines || lfg_.has_noise), kErrUnsupported,
                "splines or noise together with patches on an upsampled frame are not implemented");
-    splines_and_noise();
+    splines_and_noise(colour);
     for (View& v : colour) upsample_view(v, ceil_log2_nonzero(fh_.upsampling));
-    out.width = fh_.width;
-    out.height = fh_.height;
+    out->width = fh_.width;
+    out->height = fh_.height;
     be_.stage_marker("upsampled", colour.data(), int(colour.size()));
   }
-  // extra channels as floats with their own bit depth (they take part in patch blending), each upsampled from its coded
-  // size by its whole factor in one chain (image.rs:487-557)
   std::vector<View> extra;
   bool extra_upsampled = false;
-  for (size_t c = ec_from; c < gm_image.size() && (c - ec_from) < ih_.ec_info.size(); ++c) {
-    View v = gm_image[c].view;
-    be_.int_to_float(v, ih_.ec_info[c - ec_from].bit_depth);
-    if (const uint32_t s = ec_shift(c - ec_from)) {
+  for (size_t c = ec_from_; c < gm_image_.size() && (c - ec_from_) < ih_.ec_info.size(); ++c) {
+    View v = gm_image_[c].view;
+    be_.int_to_float(v, ih_.ec_info[c - ec_from_].bit_depth);
+    if (const uint32_t s = ec_shift(c - ec_from_)) {
       upsample_view(v, s);
       extra_upsampled = true;
     }
     extra.push_back(v);
   }
   if (extra_upsampled) be_.stage_marker("extra_upsampled", extra.data(), int(extra.size()));
-  // patches (render.rs:182-196) on the upsampled grid, then splines and noise of a frame that is not upsampled
-  if (lfg_.has_patches) {
-    std::vector<View> all = colour;
-    all.insert(all.end(), extra.begin(), extra.end());
-    std::vector<Backend::PatchJob> jobs;
-    for (const PatchRef& pr : lfg_.patches) {
-      const RefFrameStore& ref = (*ref_store_)[pr.ref_idx];
-      JXLB_CHECK(ref.valid, kErrBitstream, "patch refers to a reference frame that was not decoded");
-      JXLB_CHECK(ref.channels.size() == all.size(), kErrBitstream, "patch reference has a different channel count");
-      for (const PatchTarget& t : pr.targets)
-        for (size_t idx = 0; idx < all.size(); ++idx) {  // blend.rs:418-545
-          const PatchBlending& b = idx < colour.size() ? t.blending[0] : t.blending[1 + idx - colour.size()];
-          if (b.mode == 0) continue;
-          // BlendParams::from_patch_blending_info (blend.rs:104-163)
-          uint32_t job_mode = b.mode;
-          bool with_alpha = false, swapped = false;
-          const size_t alpha_view = colour.size() + b.alpha_channel;
-          if (b.mode >= 4) {
-            JXLB_CHECK(alpha_view < all.size(), kErrBitstream, "patch blending refers to a missing alpha channel");
-            swapped = b.mode == 5 || b.mode == 7;
-            const bool is_alpha = idx == alpha_view;
-            if (b.mode <= 5) {  // BlendAbove / BlendBelow
-              job_mode = is_alpha ? 6 : 4;
-            } else {  // MulAddAbove / MulAddBelow: the alpha channel itself is replaced (below) or kept (above)
-              if (is_alpha && !swapped) continue;
-              job_mode = is_alpha ? 1 : 5;
-            }
-            with_alpha = !is_alpha;
+  if (lfg_.has_patches) apply_patches(colour, extra);
+  if (!upsampled) splines_and_noise(colour);
+  return extra;
+}
+
+void FramePlanner::splines_and_noise(const std::vector<View>& colour) {
+  // the base correlations of a VarDCT frame; a Modular frame has none (X += 0 * Y, B += 1 * Y)
+  const float corr_x = vardct_ ? lfg_.base_correlation_x : 0.0f, corr_b = vardct_ ? lfg_.base_correlation_b : 1.0f;
+  if (lfg_.has_splines) {
+    JXLB_CHECK(colour.size() == 3, kErrUnsupported, "splines need three colour channels");
+    const std::vector<Backend::SplineArc> arcs = build_spline_arcs(lfg_, corr_x, corr_b, fh_.width, fh_.height);
+    View v[3] = {colour[0], colour[1], colour[2]};
+    be_.splat_splines(v, arcs);
+    be_.stage_marker("splines", v, 3);
+  }
+  if (lfg_.has_noise) {
+    JXLB_CHECK(colour.size() == 3 && ih_.xyb_encoded, kErrUnsupported, "noise synthesis is implemented for XYB colour frames");
+    View v[3] = {colour[0], colour[1], colour[2]};
+    // a regular frame counts itself among the visible ones; any other among the invisible ones
+    const uint64_t seed0 = role_.regular() ? ((visible_before_ + 1) << 32) : (visible_before_ << 32) + invisible_before_ + 1;
+    // the field has the frame's size (noise.rs:94-100): the upsampled size, or the planes' own without upsampling
+    if (fh_.upsampling > 1) be_.add_noise_in_frame(v, fh_.width, fh_.height, lfg_.noise_lut, fh_.group_dim(), seed0, corr_x, corr_b);
+    else be_.add_noise(v, lfg_.noise_lut, fh_.group_dim(), seed0, corr_x, corr_b);
+    be_.stage_marker("noise", v, 3);
+  }
+}
+
+// patches (render.rs:182-196), blended onto the colour and extra channels
+void FramePlanner::apply_patches(const std::vector<View>& colour, const std::vector<View>& extra) {
+  std::vector<View> all = colour;
+  all.insert(all.end(), extra.begin(), extra.end());
+  std::vector<Backend::PatchJob> jobs;
+  for (const PatchRef& pr : lfg_.patches) {
+    const StoredFrame& ref = stores_.ref[pr.ref_idx];
+    JXLB_CHECK(ref.valid, kErrBitstream, "patch refers to a reference frame that was not decoded");
+    JXLB_CHECK(ref.channels.size() == all.size(), kErrBitstream, "patch reference has a different channel count");
+    for (const PatchTarget& t : pr.targets)
+      for (size_t idx = 0; idx < all.size(); ++idx) {  // blend.rs:418-545
+        const PatchBlending& b = idx < colour.size() ? t.blending[0] : t.blending[1 + idx - colour.size()];
+        if (b.mode == 0) continue;
+        // BlendParams::from_patch_blending_info (blend.rs:104-163)
+        uint32_t job_mode = b.mode;
+        bool with_alpha = false, swapped = false;
+        const size_t alpha_view = colour.size() + b.alpha_channel;
+        if (b.mode >= 4) {
+          JXLB_CHECK(alpha_view < all.size(), kErrBitstream, "patch blending refers to a missing alpha channel");
+          swapped = b.mode == 5 || b.mode == 7;
+          const bool is_alpha = idx == alpha_view;
+          if (b.mode <= 5) {  // BlendAbove / BlendBelow
+            job_mode = is_alpha ? 6 : 4;
+          } else {  // MulAddAbove / MulAddBelow: the alpha channel itself is replaced (below) or kept (above)
+            if (is_alpha && !swapped) continue;
+            job_mode = is_alpha ? 1 : 5;
           }
-          // target rectangle clipped to the frame, then the matching reference rectangle clipped to the reference
-          const int64_t fw = all[idx].w, fhh = all[idx].h;
-          const int64_t tl = std::max<int64_t>(t.x, 0), tt = std::max<int64_t>(t.y, 0);
-          const int64_t tr = std::min<int64_t>(int64_t(t.x) + pr.width, fw), tb = std::min<int64_t>(int64_t(t.y) + pr.height, fhh);
-          if (tr <= tl || tb <= tt) continue;
-          const int64_t left = tl - t.x, top = tt - t.y;
-          const int64_t rl = int64_t(pr.x0) + left, rt = int64_t(pr.y0) + top;
-          const int64_t rr = std::min<int64_t>(rl + (tr - tl), ref.width), rb = std::min<int64_t>(rt + (tb - tt), ref.height);
-          if (rr <= rl || rb <= rt) continue;
-          const View& rv = ref.channels[idx];
-          const View& dv = all[idx];
-          Backend::PatchJob j;
-          j.src = View{rv.plane, rv.x0 + uint32_t(rl), rv.y0 + uint32_t(rt), uint32_t(rr - rl), uint32_t(rb - rt)};
-          j.dst = View{dv.plane, dv.x0 + uint32_t(tl), dv.y0 + uint32_t(tt), uint32_t(rr - rl), uint32_t(rb - rt)};
-          j.mode = job_mode;
-          j.clamp = b.clamp;
-          j.swapped = swapped && job_mode != 1;
-          if (with_alpha) {  // the frame's and the reference's alpha over the same rectangles (blend.rs:470-505)
-            const View& fa = all[alpha_view];
-            const View& ra = ref.channels[alpha_view];
-            j.base_alpha = View{fa.plane, fa.x0 + uint32_t(tl), fa.y0 + uint32_t(tt), j.dst.w, j.dst.h};
-            j.new_alpha = View{ra.plane, ra.x0 + uint32_t(rl), ra.y0 + uint32_t(rt), j.dst.w, j.dst.h};
-            j.premultiplied = ih_.ec_info[b.alpha_channel].alpha_associated;
-          }
-          jobs.push_back(j);
+          with_alpha = !is_alpha;
         }
-    }
-    be_.blend_patches(jobs);
-    be_.stage_marker("patches", colour.data(), int(colour.size()));
-  }
-  if (!upsampled) splines_and_noise();
-  if (fh_.do_ycbcr && !colour_done) {
-    ycbcr_to_rgb(colour);
-    converted = true;
-  }
-  converted |= finish_colour(colour, ih_.xyb_encoded, colour_done, ct_target, &out);
-  out.channels.insert(out.channels.end(), extra.begin(), extra.end());
-  if (is_lf_frame) {
-    JXLB_CHECK(colour.size() == 3, kErrUnsupported, "grayscale LF frames are not supported");
-    LfFrameStore& slot = (*lf_store_)[fh_.lf_level - 1];
-    if (slot.valid)
-      for (const View& v : slot.planes) be_.free_plane(v.plane);
-    for (int c = 0; c < 3; ++c) slot.planes[c] = colour[c];
-    slot.valid = true;
-    out.internal = true;
-  }
-  const bool can_reference = !fh_.is_last && (fh_.duration == 0 || fh_.save_as_reference != 0) && !is_lf_frame;  // header.rs:221-225
-  if (normal_frame && !(fh_.resets_canvas && out.width == ih_.width && out.height == ih_.height)) {
-    // ---- composition onto the image canvas (blend.rs:178-415 as a full-canvas model): every channel starts from
-    // its source slot's canvas (transparent black when the slot is empty) and the frame's rectangle is blended in
-    const size_t ncol = colour.size();
-    const bool has_extra = !fh_.ec_blending_info.empty();
-    std::vector<View> frame_ch = out.channels;
-    std::vector<View> canvas(frame_ch.size());
-    std::vector<Backend::PatchJob> colour_jobs, extra_jobs;
-    // the frame's rectangle clipped to the canvas
-    const int64_t fx0 = std::max<int64_t>(fh_.x0, 0), fy0 = std::max<int64_t>(fh_.y0, 0);
-    const int64_t fx1 = std::min<int64_t>(int64_t(fh_.x0) + out.width, ih_.width), fy1 = std::min<int64_t>(int64_t(fh_.y0) + out.height, ih_.height);
-    for (size_t idx = 0; idx < frame_ch.size(); ++idx) {
-      const BlendingInfo& bi = idx < ncol ? fh_.blending_info : fh_.ec_blending_info[idx - ncol];
-      const RefFrameStore& base = (*ref_store_)[bi.source];
-      int id = new_plane(ih_.width, ih_.height, /*zero=*/true);
-      canvas[idx] = View{id, 0, 0, ih_.width, ih_.height};
-      const bool have_base = base.valid && idx < base.channels.size();
-      if (have_base) {  // as the slot holds it, before or after the colour transform
-        // Under an ICC profile or an XYB / unknown colour space the reference composes this frame unconverted and
-        // converts the whole canvas at the end (lib.rs:934-995), base included. This frame was converted here already,
-        // so it would be composed in a different space from the base: not implemented.
-        JXLB_CHECK(base.ct_done || !converted || !record_keeps_xyb, kErrUnsupported,
-                   "blending a converted frame onto a slot saved before the colour transform under an ICC profile or an "
-                   "XYB / unknown colour space");
-        const View& bv = base.channels[idx];
-        const uint32_t cw = std::min(bv.w, ih_.width), chh = std::min(bv.h, ih_.height);
-        be_.copy_rect(View{bv.plane, bv.x0, bv.y0, cw, chh}, View{id, 0, 0, cw, chh});
-      }
-      if (fx1 <= fx0 || fy1 <= fy0) continue;
-      Backend::PatchJob j;
-      const uint32_t rw = uint32_t(fx1 - fx0), rh = uint32_t(fy1 - fy0);
-      const uint32_t sx = uint32_t(fx0 - fh_.x0), sy = uint32_t(fy0 - fh_.y0);
-      j.src = View{frame_ch[idx].plane, frame_ch[idx].x0 + sx, frame_ch[idx].y0 + sy, rw, rh};
-      j.dst = View{id, uint32_t(fx0), uint32_t(fy0), rw, rh};
-      j.clamp = bi.clamp;
-      const bool uses_alpha = (bi.mode == BlendMode::kBlend || bi.mode == BlendMode::kMulAdd) && has_extra;
-      const size_t alpha_ch = ncol + bi.alpha_channel;
-      if (uses_alpha) {
-        JXLB_CHECK(alpha_ch < frame_ch.size(), kErrBitstream, "blend alpha channel out of range");
-        j.new_alpha = View{frame_ch[alpha_ch].plane, frame_ch[alpha_ch].x0 + sx, frame_ch[alpha_ch].y0 + sy, rw, rh};
-        if (base.valid && alpha_ch < base.channels.size()) {
-          const View& av = base.channels[alpha_ch];
-          if (uint32_t(fx1) <= av.w && uint32_t(fy1) <= av.h) j.base_alpha = View{av.plane, av.x0 + uint32_t(fx0), av.y0 + uint32_t(fy0), rw, rh};
-          else JXLB_CHECK(false, kErrUnsupported, "blend base smaller than the frame rectangle");
+        // target rectangle clipped to the frame, then the matching reference rectangle clipped to the reference
+        const int64_t fw = all[idx].w, fhh = all[idx].h;
+        const int64_t tl = std::max<int64_t>(t.x, 0), tt = std::max<int64_t>(t.y, 0);
+        const int64_t tr = std::min<int64_t>(int64_t(t.x) + pr.width, fw), tb = std::min<int64_t>(int64_t(t.y) + pr.height, fhh);
+        if (tr <= tl || tb <= tt) continue;
+        const int64_t left = tl - t.x, top = tt - t.y;
+        const int64_t rl = int64_t(pr.x0) + left, rt = int64_t(pr.y0) + top;
+        const int64_t rr = std::min<int64_t>(rl + (tr - tl), ref.width), rb = std::min<int64_t>(rt + (tb - tt), ref.height);
+        if (rr <= rl || rb <= rt) continue;
+        const View& rv = ref.channels[idx];
+        const View& dv = all[idx];
+        Backend::PatchJob j;
+        j.src = View{rv.plane, rv.x0 + uint32_t(rl), rv.y0 + uint32_t(rt), uint32_t(rr - rl), uint32_t(rb - rt)};
+        j.dst = View{dv.plane, dv.x0 + uint32_t(tl), dv.y0 + uint32_t(tt), uint32_t(rr - rl), uint32_t(rb - rt)};
+        j.mode = job_mode;
+        j.clamp = b.clamp;
+        j.swapped = swapped && job_mode != 1;
+        if (with_alpha) {  // the frame's and the reference's alpha over the same rectangles (blend.rs:470-505)
+          const View& fa = all[alpha_view];
+          const View& ra = ref.channels[alpha_view];
+          j.base_alpha = View{fa.plane, fa.x0 + uint32_t(tl), fa.y0 + uint32_t(tt), j.dst.w, j.dst.h};
+          j.new_alpha = View{ra.plane, ra.x0 + uint32_t(rl), ra.y0 + uint32_t(rt), j.dst.w, j.dst.h};
+          j.premultiplied = ih_.ec_info[b.alpha_channel].alpha_associated;
         }
-        j.premultiplied = ih_.ec_info[bi.alpha_channel].alpha_associated;
+        jobs.push_back(j);
       }
-      switch (bi.mode) {  // BlendParams::from_blending_info (blend.rs:55-103)
-        case BlendMode::kReplace: j.mode = 1; break;
-        case BlendMode::kAdd: j.mode = 2; break;
-        case BlendMode::kMul: j.mode = 3; break;
-        case BlendMode::kBlend: j.mode = !uses_alpha ? 1 : (idx == alpha_ch ? 6 : 4); break;
-        default: j.mode = !uses_alpha ? 2 : (idx == alpha_ch ? 0 : 5); break;  // MulAdd; Skip on its alpha channel
-      }
-      if (j.mode == 6) j.new_alpha = j.base_alpha = View();
-      if (j.mode == 0) continue;
-      (idx < ncol ? colour_jobs : extra_jobs).push_back(j);
+  }
+  be_.blend_patches(jobs);
+  be_.stage_marker("patches", colour.data(), int(colour.size()));
+}
+
+// Composition onto the image canvas (blend.rs:178-415 as a full-canvas model): every channel starts from its source
+// slot's canvas (transparent black when the slot is empty) and the frame's rectangle is blended in.
+void FramePlanner::compose(DecodedFrame* out, bool converted) {
+  if (!role_.composes) return;
+  const size_t ncol = out->num_color;
+  const bool has_extra = !fh_.ec_blending_info.empty();
+  const std::vector<View>& frame_ch = out->channels;
+  std::vector<View> canvas(frame_ch.size());
+  std::vector<Backend::PatchJob> colour_jobs, extra_jobs;
+  // the frame's rectangle clipped to the canvas
+  const int64_t fx0 = std::max<int64_t>(fh_.x0, 0), fy0 = std::max<int64_t>(fh_.y0, 0);
+  const int64_t fx1 = std::min<int64_t>(int64_t(fh_.x0) + out->width, ih_.width), fy1 = std::min<int64_t>(int64_t(fh_.y0) + out->height, ih_.height);
+  for (size_t idx = 0; idx < frame_ch.size(); ++idx) {
+    const BlendingInfo& bi = idx < ncol ? fh_.blending_info : fh_.ec_blending_info[idx - ncol];
+    const StoredFrame& base = stores_.ref[bi.source];
+    int id = new_plane(ih_.width, ih_.height, /*zero=*/true);
+    canvas[idx] = View{id, 0, 0, ih_.width, ih_.height};
+    const bool have_base = base.valid && idx < base.channels.size();
+    if (have_base) {  // as the slot holds it, before or after the colour transform
+      // Under an ICC profile or an XYB / unknown colour space the reference composes this frame unconverted and
+      // converts the whole canvas at the end (lib.rs:934-995), base included. This frame was converted here already,
+      // so it would be composed in a different space from the base: not implemented.
+      JXLB_CHECK(base.ct_done || !converted || !colour_.record_keeps_xyb, kErrUnsupported,
+                 "blending a converted frame onto a slot saved before the colour transform under an ICC profile or an "
+                 "XYB / unknown colour space");
+      const View& bv = base.channels[idx];
+      const uint32_t cw = std::min(bv.w, ih_.width), chh = std::min(bv.h, ih_.height);
+      be_.copy_rect(View{bv.plane, bv.x0, bv.y0, cw, chh}, View{id, 0, 0, cw, chh});
     }
-    be_.blend_patches(colour_jobs);
-    be_.blend_patches(extra_jobs);
-    out.channels = canvas;
-    out.width = ih_.width;
-    out.height = ih_.height;
-  }
-  if (is_ref_frame || (normal_frame && can_reference)) {
-    RefFrameStore& slot = (*ref_store_)[fh_.save_as_reference];
-    if (slot.valid)
-      for (const View& v : slot.channels) be_.free_plane(v.plane);
-    slot.channels.clear();
-    if (is_ref_frame) {
-      slot.channels = out.channels;  // never shown: the slot takes the planes over
-    } else {
-      for (const View& v : out.channels) {  // the frame may also be shown: the slot keeps a copy
-        int id = be_.alloc_plane(std::max(v.w, 1u), std::max(v.h, 1u), false);
-        if (v.w && v.h) be_.copy_rect(v, View{id, 0, 0, v.w, v.h});
-        slot.channels.push_back(View{id, 0, 0, v.w, v.h});
+    if (fx1 <= fx0 || fy1 <= fy0) continue;
+    Backend::PatchJob j;
+    const uint32_t rw = uint32_t(fx1 - fx0), rh = uint32_t(fy1 - fy0);
+    const uint32_t sx = uint32_t(fx0 - fh_.x0), sy = uint32_t(fy0 - fh_.y0);
+    j.src = View{frame_ch[idx].plane, frame_ch[idx].x0 + sx, frame_ch[idx].y0 + sy, rw, rh};
+    j.dst = View{id, uint32_t(fx0), uint32_t(fy0), rw, rh};
+    j.clamp = bi.clamp;
+    const bool uses_alpha = (bi.mode == BlendMode::kBlend || bi.mode == BlendMode::kMulAdd) && has_extra;
+    const size_t alpha_ch = ncol + bi.alpha_channel;
+    if (uses_alpha) {
+      JXLB_CHECK(alpha_ch < frame_ch.size(), kErrBitstream, "blend alpha channel out of range");
+      j.new_alpha = View{frame_ch[alpha_ch].plane, frame_ch[alpha_ch].x0 + sx, frame_ch[alpha_ch].y0 + sy, rw, rh};
+      if (base.valid && alpha_ch < base.channels.size()) {
+        const View& av = base.channels[alpha_ch];
+        if (uint32_t(fx1) <= av.w && uint32_t(fy1) <= av.h) j.base_alpha = View{av.plane, av.x0 + uint32_t(fx0), av.y0 + uint32_t(fy0), rw, rh};
+        else JXLB_CHECK(false, kErrUnsupported, "blend base smaller than the frame rectangle");
       }
+      j.premultiplied = ih_.ec_info[bi.alpha_channel].alpha_associated;
     }
-    slot.width = out.width;
-    slot.height = out.height;
-    slot.ct_done = ct_target >= 0;
-    slot.valid = true;
+    switch (bi.mode) {  // BlendParams::from_blending_info (blend.rs:55-103)
+      case BlendMode::kReplace: j.mode = 1; break;
+      case BlendMode::kAdd: j.mode = 2; break;
+      case BlendMode::kMul: j.mode = 3; break;
+      case BlendMode::kBlend: j.mode = !uses_alpha ? 1 : (idx == alpha_ch ? 6 : 4); break;
+      default: j.mode = !uses_alpha ? 2 : (idx == alpha_ch ? 0 : 5); break;  // MulAdd; Skip on its alpha channel
+    }
+    if (j.mode == 6) j.new_alpha = j.base_alpha = View();
+    if (j.mode == 0) continue;
+    (idx < ncol ? colour_jobs : extra_jobs).push_back(j);
   }
-  if (defer_ct && fh_.is_keyframe()) {
-    // the composed canvas takes the transform to the requested encoding the frame deferred, the base's region included
-    // (blend.rs:219 gives the canvas the new frame's state); the slot above keeps the samples from before it
-    std::vector<View> canvas_colour(out.channels.begin(), out.channels.begin() + out.num_color);
-    const std::vector<View> canvas_extra(out.channels.begin() + out.num_color, out.channels.end());
-    if (fh_.do_ycbcr) ycbcr_to_rgb(canvas_colour);
-    finish_colour(canvas_colour, ih_.xyb_encoded, false, opt_.output_colour, &out);
-    out.channels.insert(out.channels.end(), canvas_extra.begin(), canvas_extra.end());
+  be_.blend_patches(colour_jobs);
+  be_.blend_patches(extra_jobs);
+  out->channels = canvas;
+  out->width = ih_.width;
+  out->height = ih_.height;
+}
+
+// Saves the frame into the LF store or the reference slot it is saved to.
+void FramePlanner::record(const DecodedFrame& out) {
+  if (role_.lf_write >= 0) {
+    JXLB_CHECK(out.num_color == 3, kErrUnsupported, "grayscale LF frames are not supported");
+    StoredFrame lf;
+    lf.valid = true;
+    lf.channels.assign(out.channels.begin(), out.channels.begin() + 3);
+    for (const View& v : lf.channels) disown(v.plane);
+    stores_.replace(stores_.lf[role_.lf_write], std::move(lf), /*copy=*/false);
   }
-  if (is_ref_frame || (normal_frame && !fh_.is_keyframe())) out.internal = true;
-  // release everything not exported
+  if (role_.saved_to >= 0) {
+    StoredFrame ref;
+    ref.valid = true;
+    ref.ct_done = colour_.ct_target >= 0;
+    ref.width = out.width;
+    ref.height = out.height;
+    ref.channels = out.channels;
+    // a reference-only frame is never shown: the slot takes its planes over
+    const bool take = role_.kind == FrameType::kReferenceOnly;
+    if (take)
+      for (const View& v : ref.channels) disown(v.plane);
+    stores_.replace(stores_.ref[role_.saved_to], std::move(ref), /*copy=*/!take);
+  }
+}
+
+// Frees every plane of the frame that no store took and the caller does not get: a frame that is not shown comes back
+// without planes.
+void FramePlanner::release_planes(DecodedFrame* out) {
+  if (!role_.shown) {
+    out->internal = true;
+    out->channels.clear();
+  }
   for (int id : frame_planes_) {
     bool exported = false;
-    for (const View& v : out.channels) exported |= (v.plane == id);
+    for (const View& v : out->channels) exported |= (v.plane == id);
     if (!exported) be_.free_plane(id);
   }
   frame_planes_.clear();
   gm_coded_.clear();
-  be_.phase_mark("filters_colour");
-  return out;
 }
 
-void FramePlanner::render_vardct(DecodedFrame*) {
+void FramePlanner::render_vardct() {
   be_.vardct_coefficients(st_);
   // LF: dequant, chroma-from-luma, adaptive smoothing (vardct/mod.rs:163-201, util.rs:254-290)
   std::vector<LfDequantJob> jobs;
-  const uint32_t lfd = fh_.lf_group_dim();
   for (uint32_t g = 0; g < fh_.num_lf_groups(); ++g) {
     LfDequantJob j;
     j.rect = lf_rect_[g];
@@ -1132,8 +1170,8 @@ void FramePlanner::render_vardct(DecodedFrame*) {
   }
   if (st_.use_lf_frame) {
     // the LF image is the rendered LF frame, used as is (jxl-render/src/vardct/mod.rs:175-180)
-    const LfFrameStore& lf = (*lf_store_)[fh_.lf_level];
-    for (int c = 0; c < 3; ++c) be_.copy_rect(lf.planes[c], View{st_.lf[c], 0, 0, st_.bw, st_.bh});
+    const StoredFrame& lf = stores_.lf[fh_.lf_level];
+    for (int c = 0; c < 3; ++c) be_.copy_rect(lf.channels[c], View{st_.lf[c], 0, 0, st_.bw, st_.bh});
   } else {
     be_.lf_dequant(st_, jobs);
     if (!st_.subsampled) be_.lf_chroma_from_luma(st_);  // vardct/mod.rs:184-191
@@ -1272,27 +1310,32 @@ bool FramePlanner::colour_params(bool is_xyb, size_t num_colour, int output_colo
   return true;
 }
 
-void FramePlanner::ycbcr_to_rgb(std::vector<View>& colour) {  // jxl-render/src/lib.rs:950-954, util.rs:320-329
-  JXLB_CHECK(colour.size() == 3, kErrBitstream, "YCbCr needs three channels");
-  View v[3] = {colour[0], colour[1], colour[2]};
-  be_.ycbcr_to_rgb(v, Backend::YcbcrParams());
-  be_.stage_marker("rgb", v, 3);
-  if (ih_.colour_encoding.colour_space == ColourSpace::kGrey) colour.resize(1);
-}
-
-bool FramePlanner::finish_colour(std::vector<View>& colour, bool is_xyb, bool already_converted, int output_colour,
-                                 DecodedFrame* out) {
+// Brings the colour channels to encoding `target` (DecodeOptions::output_colour) unless they are there already
+// (`done`): YCbCr to RGB (jxl-render/src/lib.rs:950-954, util.rs:320-329), then XYB to (linear) sRGB. `out` gets the
+// colour channels, then `extra`. Returns true when it converted the planes.
+bool FramePlanner::colour_transform(std::vector<View> colour, const std::vector<View>& extra, bool done, int target,
+                                    DecodedFrame* out) {
+  bool converted = false;
+  if (fh_.do_ycbcr && !done) {
+    JXLB_CHECK(colour.size() == 3, kErrBitstream, "YCbCr needs three channels");
+    View v[3] = {colour[0], colour[1], colour[2]};
+    be_.ycbcr_to_rgb(v, Backend::YcbcrParams());
+    be_.stage_marker("rgb", v, 3);
+    if (ih_.colour_encoding.colour_space == ColourSpace::kGrey) colour.resize(1);
+    converted = true;
+  }
   ColorParams p;
-  const bool convert = !already_converted && colour_params(is_xyb, colour.size(), output_colour, &p);
-  if (convert) {
+  if (!done && colour_params(ih_.xyb_encoded, colour.size(), target, &p)) {
     View v[3] = {colour[0], colour[1], colour[2]};
     be_.xyb_to_rgb(v, p);
     if (p.to_luma) colour.resize(1);  // XyzToLuma leaves Y in the first channel (convert.rs:866-872)
     be_.stage_marker("rgb", colour.data(), int(colour.size()));
+    converted = true;
   }
   out->num_color = uint32_t(colour.size());
   out->channels = colour;
-  return convert;
+  out->channels.insert(out->channels.end(), extra.begin(), extra.end());
+  return converted;
 }
 
 }  // namespace
@@ -1365,28 +1408,15 @@ void Backend::add_noise_in_frame(const View v[3], uint32_t field_w, uint32_t fie
 void decode_frames(Backend& be, const uint8_t* cs, size_t size, const ImageHeader& ih, const DecodeOptions& opt, size_t pos,
                    uint64_t visible_frames, uint64_t invisible_frames, uint32_t max_shown,
                    const std::function<void(DecodedFrame&&)>& sink) {
-  LfFrameStore lf_store[4];
-  RefFrameStore ref_store[4];
-  auto drop_lf_frames = [&] {
-    for (LfFrameStore& s : lf_store)
-      if (s.valid)
-        for (const View& v : s.planes) be.free_plane(v.plane);
-    for (RefFrameStore& s : ref_store)
-      if (s.valid)
-        for (const View& v : s.channels) be.free_plane(v.plane);
-  };
+  FrameStores stores{be};
   uint32_t shown = 0;
   try {
     while (pos < size && shown < max_shown) {
-      FramePlanner planner(be, cs, size, ih, opt, &lf_store, &ref_store, visible_frames, invisible_frames);
+      FramePlanner planner(be, cs, size, ih, opt, stores, visible_frames, invisible_frames);
       size_t end = 0;
       DecodedFrame f = planner.decode_frame(pos, &end);
       bool last = f.header.is_last;
       if (f.internal) {  // an LF / reference / hidden frame: what later frames need lives in the stores
-        if (f.header.frame_type == FrameType::kLfFrame)
-          for (size_t c = 3; c < f.channels.size(); ++c) be.free_plane(f.channels[c].plane);
-        else if (f.header.frame_type != FrameType::kReferenceOnly)
-          for (const View& v : f.channels) be.free_plane(v.plane);
         ++invisible_frames;
       } else {
         ++shown;
@@ -1398,11 +1428,12 @@ void decode_frames(Backend& be, const uint8_t* cs, size_t size, const ImageHeade
       if (last) break;
     }
   } catch (...) {
-    drop_lf_frames();
+    stores.release_all();
     throw;
   }
-  drop_lf_frames();
+  stores.release_all();
 }
+
 
 DecodeResult decode_codestream(Backend& be, const uint8_t* cs, size_t size, const DecodeOptions& opt) {
   DecodeResult res;

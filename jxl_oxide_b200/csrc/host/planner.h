@@ -20,6 +20,31 @@ struct DecodeOptions {
   uint32_t max_frames = 0xffffffffu;
 };
 
+// What a frame is to the frames around it (jxl-render/src/lib.rs:294-330, jxl-frame/src/header.rs:221-225): the
+// decoder and the keyframe index (frame_index.h) both take it from here.
+struct FrameRole {
+  FrameType kind = FrameType::kRegular;
+  // blended onto the canvas: a regular frame that does not replace the whole canvas
+  bool composes = false;
+  int saved_to = -1;   // the reference slot the frame is saved to, -1 when it is not saved
+  bool shown = false;  // a keyframe: one of the frames of the decoded image
+  int lf_read = -1;    // the LF store the frame takes its LF image from (use_lf_frame), or -1
+  int lf_write = -1;   // the LF store an LF frame is kept in (lf_level - 1), or -1
+  bool regular() const { return kind != FrameType::kLfFrame && kind != FrameType::kReferenceOnly; }
+};
+
+inline FrameRole frame_role(const FrameHeader& fh, const ImageHeader& ih) {
+  FrameRole r;
+  r.kind = fh.frame_type;
+  r.composes = r.regular() && !(fh.resets_canvas && fh.width == ih.width && fh.height == ih.height);
+  const bool can_reference = !fh.is_last && (fh.duration == 0 || fh.save_as_reference != 0);
+  if (r.kind == FrameType::kReferenceOnly || (r.regular() && can_reference)) r.saved_to = int(fh.save_as_reference);
+  r.shown = fh.is_keyframe();
+  if (fh.use_lf_frame()) r.lf_read = int(fh.lf_level);
+  if (r.kind == FrameType::kLfFrame) r.lf_write = int(fh.lf_level) - 1;
+  return r;
+}
+
 struct DecodedFrame {
   bool internal = false;  // an LF frame: consumed by later frames, never shown (jxl-render/src/lib.rs:294-318)
   uint32_t width = 0, height = 0;
