@@ -761,10 +761,8 @@ void CudaBackend::decode_hf(VarDctState& st, std::vector<HfGroupJob>& jobs) {
   if (jobs.empty()) return;
   const uint32_t pass = jobs[0].pass_idx;
   const HfPassSyntax& hp = st.hfg->passes[pass];
-  // An LZ77 code runs the thread-per-stream kernel's LZ77 variant (hf_schedule), which has no chroma-subsampled form.
+  // An LZ77 code runs the thread-per-stream kernel's LZ77 variant (hf_schedule).
   const bool hf_lz77 = hp.code.lz77_enabled;
-  JXLB_CHECK(!(hf_lz77 && st.subsampled), kErrUnsupported,
-             "LZ77 in the HF coefficient streams of a chroma-subsampled frame is not supported on the device");
   const DevHfParams p = build_hf_params(st, pass, *this, d_natural_orders_, natural_order_offset_);
   const HfSchedule sched = hf_schedule(p, hf_streams_per_cta, hf_streams_per_warp);
   const std::vector<uint32_t> perm = hf_launch_order(jobs, sched.lanes);  // launch order -> `jobs`

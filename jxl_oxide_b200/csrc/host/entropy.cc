@@ -561,7 +561,7 @@ uint32_t EntropyReader::read_symbol(BitReader& br, uint32_t cluster) {
   return symbol;
 }
 
-uint32_t EntropyReader::read_varint_clustered(BitReader& br, uint32_t cluster, uint32_t dist_multiplier) {
+uint32_t EntropyReader::read_varint_clustered_untraced(BitReader& br, uint32_t cluster, uint32_t dist_multiplier) {
   const EntropyCode& c = *code_;
   if (!c.lz77_enabled) {
     uint32_t token = read_symbol(br, cluster);

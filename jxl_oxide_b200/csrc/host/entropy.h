@@ -13,6 +13,15 @@
 
 namespace jxlb {
 
+#ifdef JXLB_ENTROPY_TRACE
+// Built only into tools/hf_restream.cc: every stream start (the bit position before its ANS state), every value read
+// with its cluster and the bit position after it, and the bit span of each HF pass code (frame_syntax.cc).
+struct EntropyCode;
+void entropy_trace_begin(const void* reader, size_t pos_bits);
+void entropy_trace_value(const void* reader, uint32_t cluster, uint32_t value, size_t pos_bits);
+void entropy_trace_hf_code(uint32_t pass, size_t begin_bits, size_t end_bits, const EntropyCode& code);
+#endif
+
 // Hybrid-uint config, packed for the device: split_exponent | msb<<8 | lsb<<16.
 struct HybridUintConfig {
   uint32_t split_exponent = 0, msb_in_token = 0, lsb_in_token = 0;
@@ -79,6 +88,9 @@ class EntropyReader {
   explicit EntropyReader(const EntropyCode* code) : code_(code) {}
   // Decoder::begin (lib.rs:162-164): reads the 32-bit ANS state.
   void begin(BitReader& br) {
+#ifdef JXLB_ENTROPY_TRACE
+    entropy_trace_begin(this, br.pos());
+#endif
     if (!code_->use_prefix) {
       state_ = br.read(32);
       initial_ = false;
@@ -102,13 +114,20 @@ class EntropyReader {
     return uint32_t((((t << n) | rest) << c.lsb_in_token) | low);
   }
   // read_varint_with_multiplier_clustered (lib.rs:80-106), incl. LZ77 (lib.rs:476-569)
-  uint32_t read_varint_clustered(BitReader& br, uint32_t cluster, uint32_t dist_multiplier);
+  uint32_t read_varint_clustered(BitReader& br, uint32_t cluster, uint32_t dist_multiplier) {
+    const uint32_t v = read_varint_clustered_untraced(br, cluster, dist_multiplier);
+#ifdef JXLB_ENTROPY_TRACE
+    entropy_trace_value(this, cluster, v, br.pos());
+#endif
+    return v;
+  }
   uint32_t read_varint(BitReader& br, uint32_t ctx, uint32_t dist_multiplier = 0) {
     return read_varint_clustered(br, code_->cluster_map[ctx], dist_multiplier);
   }
   const EntropyCode& code() const { return *code_; }
 
  private:
+  uint32_t read_varint_clustered_untraced(BitReader& br, uint32_t cluster, uint32_t dist_multiplier);
   const EntropyCode* code_;
   uint32_t state_ = 0;
   bool initial_ = true;

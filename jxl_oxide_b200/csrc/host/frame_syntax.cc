@@ -687,7 +687,12 @@ HfGlobalSyntax parse_hf_global(BitReader& br, const ImageHeader& ih, const Frame
       }
       JXLB_CHECK(dec.finalize_ok(), kErrBitstream, "invalid ANS stream (coefficient orders)");
     }
+    const size_t code_begin = br.pos();
     hp.code = parse_entropy_code(br, 495 * g.num_hf_presets * lfg.hf_block_ctx.num_block_clusters);
+#ifdef JXLB_ENTROPY_TRACE
+    entropy_trace_hf_code(pass, code_begin, br.pos(), hp.code);
+#endif
+    (void)code_begin;
     g.passes.push_back(std::move(hp));
   }
   br.check();

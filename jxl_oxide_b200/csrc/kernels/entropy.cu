@@ -375,6 +375,7 @@ void launch_hf_lanes(const uint8_t* cs, DevFrame f, DevHfParams p, const uint2* 
     cudaFuncSetAttribute(decode_hf_lanes_kernel<false, true, false, THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
     cudaFuncSetAttribute(decode_hf_lanes_kernel<true, true, false, THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
     cudaFuncSetAttribute(decode_hf_lanes_kernel<false, false, true, THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    cudaFuncSetAttribute(decode_hf_lanes_kernel<true, false, true, THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
     return true;
   }();
   (void)attr_set;
@@ -383,8 +384,9 @@ void launch_hf_lanes(const uint8_t* cs, DevFrame f, DevHfParams p, const uint2* 
 #define JXLB_HF_LANES(SUB_, STAGED_, LZ77_)                                                                        \
   decode_hf_lanes_kernel<SUB_, STAGED_, LZ77_, THREADS><<<ctas, THREADS, L.total, stream>>>(                       \
       cs, f, p, list, counts, jobs, end_bits, status, num_jobs, first_pass, per_cta, lz_windows, lz_window_len)
-  if (p.code.lz77_enabled) {  // the caller rejects chroma-subsampled frames with an LZ77 code
-    JXLB_HF_LANES(false, false, true);
+  if (p.code.lz77_enabled) {
+    if (f.subsampled) JXLB_HF_LANES(true, false, true);
+    else JXLB_HF_LANES(false, false, true);
   } else if (hf_lane_staged(p, L)) {
     if (f.subsampled) JXLB_HF_LANES(true, true, false);
     else JXLB_HF_LANES(false, true, false);

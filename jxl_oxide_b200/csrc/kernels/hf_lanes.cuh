@@ -319,7 +319,9 @@ __device__ __forceinline__ bool hf_block_record(const DevFrame& f, const DevHfPa
 // LZ77 (general variant only): the code has LZ77 enabled, and every value -- non-zero count or coefficient -- goes
 // through lz77_read_value with distance multiplier 0 (hf_coeff.rs:181-222), keeping the stream's values in `*lz`'s
 // window (hf_lz77_window_entries of them). A copy still pending when the group ends is ignored, as in the reference.
-// Without LZ77, `lz` is unused (null).
+// With SUB, a channel slot skipped below (block not aligned to the channel's grid, or no block at the shifted position)
+// reads no value and leaves the LZ77 state alone, as the reference never reaches its read for such a slot; copies cross
+// channel and block boundaries freely. Without LZ77, `lz` is unused (null).
 // `list` / `count`: this stream's group's varblock records.
 template <bool SUB, bool STAGED, bool LZ77, class Mem>
 __device__ __forceinline__ void hf_lane_stream(const uint8_t* __restrict__ cs, const DevFrame& f, const DevHfParams& p,
@@ -553,17 +555,11 @@ struct HfLaneTables {
 // One stream on the host: `blk_ctx` holds hf_block_ctx_cell() of every cell of the frame (bw x bh); the stream's group
 // list is compacted from it in raster order, and the stream runs the variant the device launcher would pick for `p`.
 // An LZ77 code runs with a window of the device's size (hf_lz77_window_entries) and reports the number of values it
-// took from copies through JXLB_LANE_LZ77_COPIED; like CudaBackend::decode_hf, it is not supported in a chroma-subsampled
-// frame (status kDevUnsupported).
+// took from copies through JXLB_LANE_LZ77_COPIED.
 template <bool SUB>
 inline void hf_lane_decode(const uint8_t* cs, const DevFrame& f, const DevHfParams& p, const HfLaneTables& T,
                            const uint32_t* blk_ctx, const DevHfJob& job, uint8_t* nz, uint32_t nz_stride, int first_pass,
                            uint64_t* end_bit, int* status) {
-  if (p.code.lz77_enabled && f.subsampled) {
-    *end_bit = job.bit_pos;
-    *status = kDevUnsupported;
-    return;
-  }
   const HfGroupRect r = hf_group_rect(f, p, job.group_idx);
   std::vector<uint2> list;
   for (uint32_t y = 0; y < r.height; ++y)

@@ -179,7 +179,7 @@ void launch_decode_hf(const uint8_t* codestream, DevFrame f, DevHfParams p, cons
 // streams_per_warp of each warp only help stage the tables.
 // `list` / `counts` come from launch_hf_block_list: per group (hf_block_list_count of them), its varblock origins in
 // raster order with their transform type and context offset, group_dim_blocks^2 records apart, and their number.
-// A code with LZ77 (not in chroma-subsampled frames) needs `lz_windows`: num_jobs windows of `lz_window_len` entries
+// A code with LZ77 needs `lz_windows`: num_jobs windows of `lz_window_len` entries
 // (hf_lz77_window_entries in launch_tables.h), stream i's at lz_windows + i * lz_window_len.
 size_t hf_block_list_count(DevFrame f, DevHfParams p);
 void launch_hf_block_list(DevFrame f, DevHfParams p, uint2* list, uint32_t* counts, cudaStream_t stream);

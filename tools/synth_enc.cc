@@ -20,7 +20,10 @@
 // --hf-lz77 rle|match codes the HF passes with LZ77 (HfLz77 below); everything else is written as without it, and the
 // number of values the decoder takes from copies goes to stderr. --extra TYPE:BITS:DIM_SHIFT:EC_UPSAMPLING (repeatable)
 // adds extra channels at their coded sizes to a VarDCT or --modular frame; --ycbcr and --upsampling make --modular frames
-// with chroma-subsampled Cb, Y, Cr or a reduced colour resolution (encode_channels). --upsampling K also codes a VarDCT
+// with chroma-subsampled Cb, Y, Cr or a reduced colour resolution (encode_channels). --ycbcr also makes a VarDCT frame
+// laid out like a JPEG transcode: Cb, Y, Cr with jpeg_upsampling, DCT8 in every cell, no chroma from luma,
+// skip_adaptive_lf_smoothing, each channel's LF and HF at its shifted grid; it combines with --hf-lz77, and
+// --dump-coeffs FILE writes the HF coefficients of any VarDCT frame. --upsampling K also codes a VarDCT
 // frame at ceil(W / K) x ceil(H / K), and --noise / --noise-zero, --splines N and --dangling-patch give a VarDCT frame
 // those LfGlobal features (write_features).
 //
@@ -787,7 +790,10 @@ struct Args {
   HfLz77 hf_lz77;          // --hf-lz77 rle | match | bad-first | bad-length: LZ77 in the HF pass codes (see HfLz77)
   // Channels coded below the frame's resolution: a --modular frame with any of these is written without transforms,
   // from seeded integer samples at each channel's coded size (encode_channels); --extra also goes with VarDCT frames
-  std::string ycbcr;       // --ycbcr 444 | 420 | 422 | 440: Cb, Y, Cr colour channels with that chroma subsampling
+  std::string ycbcr;       // --ycbcr 444 | 420 | 422 | 440: Cb, Y, Cr colour channels with that chroma subsampling; a
+                           // VarDCT frame is then laid out like a JPEG transcode (ycbcr_shifts)
+  std::string dump_coeffs; // --dump-coeffs FILE: a VarDCT frame's HF coefficients as the decoder accumulates them over
+                           // the passes: per channel (X / Cb, Y, B / Cr) a plane of its blocks * 8 samples, int32
   uint32_t upsampling = 1; // --upsampling 1 | 2 | 4 | 8: the frame's colour upsampling (a VarDCT frame is coded at
                            // ceil(W / k) x ceil(H / k))
   // LfGlobal features of a VarDCT frame, drawn from generators of their own (the frame's other draws stay as without them)
@@ -1022,6 +1028,18 @@ int write_modular_frame(const Args& a, const std::vector<MChan>& ch, uint32_t cw
 std::array<uint32_t, 3> jpeg_upsampling(const Args& a) {
   const uint32_t y = a.ycbcr == "420" ? 1 : a.ycbcr == "422" ? 2 : a.ycbcr == "440" ? 3 : 0;
   return {0, y, 0};
+}
+
+// The channel shifts of --ycbcr (ChannelShift::from_jpeg_upsampling, as host/planner.cc derives them): channel c (Cb, Y,
+// Cr) keeps one sample (or 8x8 block) per (1 << hs[c]) x (1 << vs[c]) luma ones. All zero without --ycbcr.
+void ycbcr_shifts(const Args& a, uint32_t hs[3], uint32_t vs[3]) {
+  const std::array<uint32_t, 3> ju = jpeg_upsampling(a);
+  bool h_any = false, v_any = false;
+  for (uint32_t j : ju) h_any |= j == 1 || j == 2, v_any |= j == 1 || j == 3;
+  for (int c = 0; c < 3; ++c) {
+    hs[c] = h_any && (ju[c] == 0 || ju[c] == 3);
+    vs[c] = v_any && (ju[c] == 0 || ju[c] == 2);
+  }
 }
 
 // num_extra and one ExtraChannelInfo per --extra (jxl-image/src/lib.rs:303-345)
@@ -1376,6 +1394,7 @@ int write_modular_frame(const Args& a, const std::vector<MChan>& ch, uint32_t cw
 
 }  // namespace
 
+#ifndef SYNTH_ENC_NO_MAIN  // tools/hf_restream.cc includes this file for its entropy writer
 int main(int argc, char** argv) {
   Args a;
   for (int i = 1; i < argc; ++i) {
@@ -1402,6 +1421,7 @@ int main(int argc, char** argv) {
     else if (s == "--hf-lz77") a.hf_lz77.mode = next();
     else if (s == "-o") a.out = next();
     else if (s == "--ycbcr") a.ycbcr = next();
+    else if (s == "--dump-coeffs") a.dump_coeffs = next();
     else if (s == "--upsampling") a.upsampling = uint32_t(atoi(next().c_str()));
     else if (s == "--noise") a.noise = Args::kSeededNoise;
     else if (s == "--dangling-patch") a.dangling_patch = true;
@@ -1424,7 +1444,12 @@ int main(int argc, char** argv) {
     fprintf(stderr, "--ycbcr takes 444, 420, 422 or 440\n"), exit(2);
   if (a.upsampling != 1 && a.upsampling != 2 && a.upsampling != 4 && a.upsampling != 8)
     fprintf(stderr, "--upsampling takes 1, 2, 4 or 8\n"), exit(2);
-  if (!a.ycbcr.empty() && !a.modular) fprintf(stderr, "--ycbcr makes --modular frames\n"), exit(2);
+  if (!a.ycbcr.empty() && !a.modular &&
+      (a.lf_frame || a.all_types || a.only_type >= 0 || !a.colour.empty() || a.upsampling != 1 || !a.extras.empty() ||
+       a.noise != Args::kNoNoise || a.splines || a.dangling_patch))
+    fprintf(stderr, "--ycbcr of a VarDCT frame is not written with --lf-frame, --all-types, --only-type, --colour, "
+                    "--upsampling, --extra or LfGlobal features\n"), exit(2);
+  if (!a.dump_coeffs.empty() && a.modular) fprintf(stderr, "--dump-coeffs goes with VarDCT frames\n"), exit(2);
   if ((a.noise != Args::kNoNoise || a.splines || a.dangling_patch) && a.modular)
     fprintf(stderr, "--noise, --splines and --dangling-patch go with VarDCT frames\n"), exit(2);
   if (a.upsampling != 1 && !a.modular && (a.lf_frame || !a.extras.empty()))
@@ -1437,11 +1462,18 @@ int main(int argc, char** argv) {
   if (a.modular) return encode_modular(a);
   if (a.only_type >= int(kNumTransformTypes) || (a.only_type >= 0 && a.all_types))
     fprintf(stderr, "--only-type takes a transform type 0..26 (not with --all-types)\n"), exit(2);
+  const bool ycbcr = !a.ycbcr.empty();
+  if (ycbcr) a.only_type = kDct8;  // a JPEG transcode codes DCT8 in every cell
+  uint32_t hs[3], vs[3];
+  ycbcr_shifts(a, hs, vs);
   std::mt19937 rng(a.seed);
   auto uni = [&](double lo, double hi) { return lo + (hi - lo) * (double(rng()) / 4294967296.0); };
   // the frame's content at its coded size; the image (and frame) size is width x height
   const uint32_t up = a.upsampling, W = (a.width + up - 1) / up, H = (a.height + up - 1) / up;
-  const uint32_t bw = (W + 7) / 8, bh = (H + 7) / 8;
+  // in a subsampled direction the block grid is rounded up to an even size (whole chroma blocks), as the decoder lays
+  // it out (blocks_w in host/planner.cc); the rounding never adds a group
+  const bool h_sub = hs[0] | hs[1] | hs[2], v_sub = vs[0] | vs[1] | vs[2];
+  const uint32_t bw = h_sub ? ((W + 7) / 8 + 1) / 2 * 2 : (W + 7) / 8, bh = v_sub ? ((H + 7) / 8 + 1) / 2 * 2 : (H + 7) / 8;
   const uint32_t gcols = (W + 255) / 256, grows = (H + 255) / 256, num_groups = gcols * grows;
   const uint32_t lcols = (W + 2047) / 2048, lrows = (H + 2047) / 2048, num_lf = lcols * lrows;
   if (a.passes < 1 || a.passes > 3 || (a.passes > 1 && a.lf_frame)) fprintf(stderr, "--passes takes 1..3 (not with --lf-frame)\n"), exit(2);
@@ -1532,11 +1564,14 @@ int main(int argc, char** argv) {
     uint32_t lw = std::min(256u, bw - lx0), lh = std::min(256u, bh - ly0);
     std::vector<Plane2D> ch(3);
     const int order[3] = {1, 0, 2};  // modular channels are Y, X, B
-    for (int k = 0; k < 3; ++k) {
-      ch[k].w = lw, ch[k].h = lh;
-      ch[k].v.resize(size_t(lw) * lh);
-      for (uint32_t y = 0; y < lh; ++y)
-        for (uint32_t x = 0; x < lw; ++x) ch[k].v[size_t(y) * lw + x] = lfq[order[k]][size_t(ly0 + y) * bw + lx0 + x];
+    for (int k = 0; k < 3; ++k) {  // each channel at its shifted grid, taken from the top-left part of lfq
+      const int c = order[k];
+      const uint32_t sw = (lw + (1u << hs[c]) - 1) >> hs[c], sh = (lh + (1u << vs[c]) - 1) >> vs[c];
+      const uint32_t sx0 = lx0 >> hs[c], sy0 = ly0 >> vs[c];
+      ch[k].w = sw, ch[k].h = sh;
+      ch[k].v.resize(size_t(sw) * sh);
+      for (uint32_t y = 0; y < sh; ++y)
+        for (uint32_t x = 0; x < sw; ++x) ch[k].v[size_t(y) * sw + x] = lfq[c][size_t(sy0 + y) * bw + sx0 + x];
     }
     modular_tokens(tree, ch, int32_t(1 + lg), &lfcoeff_tokens[lg]);
     // HfMetadata: x_from_y, b_from_y (lw/8 x lh/8), block info (nb x 2), sharpness (lw x lh)
@@ -1545,7 +1580,7 @@ int main(int argc, char** argv) {
     for (int k = 0; k < 2; ++k) {
       hm[k].w = w64, hm[k].h = h64;
       hm[k].v.resize(size_t(w64) * h64);
-      for (auto& v : hm[k].v) v = int32_t(rng() % 33) - 16;
+      for (auto& v : hm[k].v) v = ycbcr ? 0 : int32_t(rng() % 33) - 16;  // no chroma from luma in a JPEG transcode
     }
     const auto& blocks = lf_blocks[lg];
     nb_blocks[lg] = uint32_t(blocks.size());
@@ -1598,6 +1633,12 @@ int main(int argc, char** argv) {
   // part_p = remainder / 2^shift_p truncated toward zero
   std::vector<std::vector<Token>> hf_tokens(size_t(P) * num_groups);
   std::exponential_distribution<double> expo(1.0);
+  std::vector<int32_t> dump[3];  // --dump-coeffs: channel c's plane is dump_w[c] samples wide
+  uint32_t dump_w[3];
+  for (int c = 0; c < 3; ++c) {
+    dump_w[c] = ((bw + (1u << hs[c]) - 1) >> hs[c]) * 8;
+    if (!a.dump_coeffs.empty()) dump[c].assign(size_t(dump_w[c]) * (((bh + (1u << vs[c]) - 1) >> vs[c]) * 8), 0);
+  }
   for (uint32_t g = 0; g < num_groups; ++g) {
     uint32_t bx0 = (g % gcols) * 32, by0 = (g / gcols) * 32;
     uint32_t gw = std::min(32u, bw - bx0), gh = std::min(32u, bh - by0);
@@ -1613,6 +1654,9 @@ int main(int argc, char** argv) {
         uint32_t num_blocks = uint32_t(ti.w8) * ti.h8, nb_log = ceil_log2_nonzero(num_blocks), size = num_blocks * 64;
         for (int ci = 0; ci < 3; ++ci) {
           int c = ci == 0 ? 1 : (ci == 1 ? 0 : 2);
+          // a subsampled channel codes only the blocks aligned to its grid, at the shifted position (hf_coeff.rs:143-155)
+          const uint32_t sx = x >> hs[c], sy = y >> vs[c];
+          if ((sx << hs[c]) != x || (sy << vs[c]) != y) continue;
           uint32_t block_ctx = kDefaultBlockCtxMap[ci * 13 + ti.order_id];
           // synthesise coefficients along the scan order: Laplacian with decaying scale
           full.assign(size, 0);
@@ -1624,6 +1668,13 @@ int main(int argc, char** argv) {
             int32_t q = int32_t(mag + 0.35);
             if (q) full[k] = (rng() & 1) ? q : -q;
           }
+          if (!a.dump_coeffs.empty())
+            for (uint32_t k = num_blocks; k < size; ++k) {
+              uint32_t dx = orders[ti.order_id][k] & 0xffff, dy = orders[ti.order_id][k] >> 16;
+              if (ti.transpose) std::swap(dx, dy);
+              const size_t px = size_t((bx0 >> hs[c]) + sx) * 8 + dx, py = size_t((by0 >> vs[c]) + sy) * 8 + dy;
+              dump[c][py * dump_w[c] + px] = full[k];
+            }
           for (uint32_t pass = 0; pass < P; ++pass) {
           const uint32_t shift = P - 1 - pass;
           std::vector<Token>& toks = hf_tokens[size_t(pass) * num_groups + g];
@@ -1636,13 +1687,13 @@ int main(int argc, char** argv) {
             if (coeffs[k]) ++non_zeros;
           }
           uint32_t predicted;
-          if (y == 0) predicted = x == 0 ? 32 : nz_row[c][x - 1];
-          else if (x == 0) predicted = nz_row[c][x];
-          else predicted = (nz_row[c][x] + nz_row[c][x - 1] + 1) >> 1;
+          if (sy == 0) predicted = sx == 0 ? 32 : nz_row[c][sx - 1];
+          else if (sx == 0) predicted = nz_row[c][sx];
+          else predicted = (nz_row[c][sx] + nz_row[c][sx - 1] + 1) >> 1;
           uint32_t pidx = predicted >= 8 ? 4 + predicted / 2 : predicted;
           toks.push_back({block_ctx + pidx * nbc, non_zeros});
           uint32_t nz_val = (non_zeros + num_blocks - 1) >> nb_log;
-          for (uint32_t dx = 0; dx < ti.w8; ++dx) nz_row[c][x + dx] = nz_val;
+          for (uint32_t dx = 0; dx < ti.w8; ++dx) nz_row[c][sx + dx] = nz_val;
           if (!non_zeros) continue;
           uint32_t prev = non_zeros <= num_blocks * 4 ? 1 : 0;
           uint32_t base = block_ctx * 458 + 37 * nbc;
@@ -1662,6 +1713,12 @@ int main(int argc, char** argv) {
           }
         }
       }
+  }
+  if (!a.dump_coeffs.empty()) {
+    FILE* df = fopen(a.dump_coeffs.c_str(), "wb");
+    if (!df) return perror("fopen"), 1;
+    for (const auto& d : dump) fwrite(d.data(), 4, d.size(), df);
+    fclose(df);
   }
   // context clustering for the HF code (495 * nbc contexts -> 28 clusters)
   std::vector<uint8_t> hf_map(495 * nbc, 0);
@@ -1731,7 +1788,16 @@ int main(int argc, char** argv) {
     else write_u32(w, 3, 16, global_scale - 8193);
     write_u32(w, 1, 5, quant_lf - 1);
     w.write(1, 1);  // HfBlockContext default
-    w.write(1, 1);  // LfChannelCorrelation all_default
+    if (ycbcr) {    // LfChannelCorrelation of a JPEG transcode: no chroma from luma (base correlations 0)
+      w.write(1, 0);
+      write_u32(w, 0, 0, 0);  // colour_factor 84
+      w.write(16, 0);         // base_correlation_x = 0.0 (f16)
+      w.write(16, 0);         // base_correlation_b = 0.0 (f16)
+      w.write(8, 128);        // x_factor_lf
+      w.write(8, 128);        // b_factor_lf
+    } else {
+      w.write(1, 1);  // LfChannelCorrelation all_default
+    }
     w.write(1, 1);  // global MA tree present
     write_tree(w, tree);
     std::vector<uint8_t> map(size_t(tree.num_leaves()));
@@ -1802,7 +1868,7 @@ int main(int argc, char** argv) {
   write_dim(a.height);
   cs.write(3, 0);  // ratio
   write_dim(a.width);
-  if (a.colour.empty() && a.extras.empty()) {
+  if (a.colour.empty() && a.extras.empty() && !ycbcr) {
     cs.write(1, 1);  // ImageMetadata all_default
   } else {  // ImageMetadata with extra channels and / or an enum ColourEncoding (jxl-image/src/lib.rs:229-287, color.rs:21-58)
     const bool pq = a.colour == "pq";
@@ -1818,7 +1884,7 @@ int main(int argc, char** argv) {
     cs.write(2, 0);  // 8 bits
     cs.write(1, a.wide_samples() ? 0 : 1);  // modular_16bit_buffers
     write_extra_channels(cs, a);
-    cs.write(1, 1);  // xyb_encoded
+    cs.write(1, ycbcr ? 0 : 1);  // xyb_encoded
     cs.write(1, a.colour.empty() ? 1 : 0);  // ColourEncoding all_default (sRGB)
   }
   if (!a.colour.empty()) {
@@ -1866,7 +1932,7 @@ int main(int argc, char** argv) {
       cs.write(16, 0);       // linear_below
     }
   }
-  if (!a.colour.empty() || !a.extras.empty()) cs.write(2, 0);  // extensions
+  if (!a.colour.empty() || !a.extras.empty() || ycbcr) cs.write(2, 0);  // extensions
   cs.write(1, 1);  // default_m
   cs.pad();
   auto write_u64_small = [&](uint32_t v) {  // U64 (jxl-bitstream): 0 | 1 + u(4) | 17 + u(8)
@@ -1941,15 +2007,23 @@ int main(int argc, char** argv) {
     cs.write(2, 0);         // name: empty
     cs.write(1, 1);         // restoration filter all_default
     write_u64_small(0);     // frame extensions
-  } else if (P > 1 || a.epf_iters != 2 || !a.gaborish || !a.extras.empty() || up != 1 || a.noise != Args::kNoNoise || a.splines || a.dangling_patch) {
+  } else if (P > 1 || a.epf_iters != 2 || !a.gaborish || !a.extras.empty() || up != 1 || a.noise != Args::kNoNoise || a.splines || a.dangling_patch ||
+             ycbcr) {
     cs.write(1, 0);         // all_default
     cs.write(2, 0);         // Regular
     cs.write(1, 0);         // VarDCT
-    write_u64_small((a.noise != Args::kNoNoise ? 0x1 : 0) | (a.dangling_patch ? 0x2 : 0) | (a.splines ? 0x10 : 0));  // flags: noise, patches, splines
+    // flags: noise, patches, splines, skip_adaptive_lf_smoothing (set in every JPEG transcode)
+    write_u64_small((a.noise != Args::kNoNoise ? 0x1 : 0) | (a.dangling_patch ? 0x2 : 0) | (a.splines ? 0x10 : 0) | (ycbcr ? 0x80 : 0));
+    if (ycbcr) {
+      cs.write(1, 1);  // do_ycbcr
+      for (uint32_t j : jpeg_upsampling(a)) cs.write(2, j);
+    }
     cs.write(2, ceil_log2_nonzero(up));  // upsampling: U32 selector k is 2^k
     for (const Args::Extra& e : a.extras) cs.write(2, ceil_log2_nonzero(e.ec_upsampling));  // U32 selector k is 2^k
-    cs.write(3, 3);         // x_qm_scale
-    cs.write(3, 2);         // b_qm_scale
+    if (!ycbcr) {
+      cs.write(3, 3);       // x_qm_scale
+      cs.write(3, 2);       // b_qm_scale
+    }
     cs.write(2, P - 1);     // num_passes (1, 2 or 3)
     if (P > 1) {
       cs.write(2, 0);       // num_ds = 0
@@ -2008,3 +2082,4 @@ int main(int argc, char** argv) {
           H, cs.bytes.size(), 8.0 * cs.bytes.size() / (double(W) * H), lf_bytes, hf_bytes, num_groups, num_lf);
   return 0;
 }
+#endif
