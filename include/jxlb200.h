@@ -114,6 +114,39 @@ int32_t jxlb_frame_write_to_buffer(jxlb_decoder* dec, int32_t frame, int32_t sam
  * returns after the packing kernel has finished, so the buffer may be used on any stream. */
 int32_t jxlb_frame_write_to_device(jxlb_decoder* dec, int32_t frame, int32_t sample_type, int32_t orientation,
                                    void* device_dst, size_t dst_bytes);
+/* ---- Every output layout of jxl-oxide's Render (crates/jxl-oxide/src/lib.rs:1133-1198, fb.rs:184-410) from one packer ----
+ * The frame's resident planes are converted on the device in one kernel (kernels/pack.cu), whatever the layout:
+ *   JXLB_LAYOUT_STREAM           Render::stream(): colour, the black channel of a CMYK image, the first alpha channel,
+ *                                spot colours mixed into RGB; interleaved (channel fastest). jxlb_frame_write_to_buffer's output.
+ *   JXLB_LAYOUT_STREAM_NO_ALPHA  Render::stream_no_alpha(): the same without the alpha channel.
+ *   JXLB_LAYOUT_ALL_INTERLEAVED  Render::image_all_channels(): colour, then every extra channel in header order, interleaved.
+ *   JXLB_LAYOUT_ALL_PLANAR       Render::image_planar(): the same channels, one oriented (height, width) plane per channel,
+ *                                channel-major. (jxlb_frame_channel_to_host copies the stored planes, not oriented.)
+ * All layouts apply the orientation. render_spot_colour = 0 is JxlImage::set_render_spot_color(false): the stream
+ * layouts then leave the spot colours unmixed. The all-channel layouts never mix spot colours and ignore the setting;
+ * spot colours are never mixed into grayscale images. */
+enum {
+  JXLB_LAYOUT_STREAM = 0,
+  JXLB_LAYOUT_STREAM_NO_ALPHA = 1,
+  JXLB_LAYOUT_ALL_INTERLEAVED = 2,
+  JXLB_LAYOUT_ALL_PLANAR = 3
+};
+typedef struct {
+  int32_t layout;             /* JXLB_LAYOUT_* */
+  int32_t sample_type;        /* 0 = u8, 1 = u16, 2 = f32 (u8 / u16: round(v * max) clamped, NaN -> 0, fb.rs:436-520) */
+  int32_t orientation;        /* 1..8, or 0 for the image header's */
+  int32_t render_spot_colour; /* nonzero: mix spot colours into RGB (the reference's default) */
+} jxlb_write_spec;
+/* The number of channels and the byte count a write of `frame` with `spec` produces (either pointer may be NULL).
+ * The output is width x height samples per channel, height x width for orientations 5..8. JXLB_ERR_INVALID_ARG for a
+ * spec out of range. */
+int32_t jxlb_frame_write_size(jxlb_decoder* dec, int32_t frame, const jxlb_write_spec* spec, uint32_t* num_channels,
+                              uint64_t* bytes);
+/* Writes `frame` as `spec` asks into `dst`: host memory, or with dst_on_device = 1 memory of this decoder's GPU (e.g. a
+ * torch tensor), which then never touches the host. JXLB_ERR_INVALID_ARG when `dst_bytes` is smaller than
+ * jxlb_frame_write_size's count. Returns after the samples are in `dst`, so the buffer may be used on any stream. */
+int32_t jxlb_frame_write_ex(jxlb_decoder* dec, int32_t frame, const jxlb_write_spec* spec, void* dst, size_t dst_bytes,
+                            int32_t dst_on_device);
 /* Device-resident access: pointer to the channel's top-left sample and its row stride (floats). */
 int32_t jxlb_frame_channel_device(jxlb_decoder* dec, int32_t frame, int32_t channel, float** dptr, uint32_t* stride);
 int32_t jxlb_release_frames(jxlb_decoder* dec);
@@ -297,6 +330,15 @@ int32_t jxlb_pipeline_wait(jxlb_pipeline* p, uint64_t* tag, int32_t* status, voi
  * otherwise a segment with more keyframes than the ring has buffers never finishes. */
 int32_t jxlb_pipeline_submit_keyframes(jxlb_pipeline* p, const uint8_t* data, size_t size, int32_t slot, int32_t out_mode,
                                        void* dst, size_t dst_bytes, uint64_t tag);
+/* jxlb_pipeline_submit / _submit_keyframes with the output described by a jxlb_write_spec, copied: any layout, sample
+ * type, orientation and spot-colour setting, instead of an out_mode. The samples go to host `dst`, to device `dst` (of the
+ * pipeline's GPU) with dst_on_device = 1, or with dst = NULL to a buffer of the pipeline's host ring sized for the spec.
+ * For keyframes, keyframe k goes at k * (dst_bytes / num_keyframes) as before. */
+int32_t jxlb_pipeline_submit_ex(jxlb_pipeline* p, const uint8_t* data, size_t size, int32_t slot, const jxlb_write_spec* spec,
+                                void* dst, size_t dst_bytes, int32_t dst_on_device, uint64_t tag);
+int32_t jxlb_pipeline_submit_keyframes_ex(jxlb_pipeline* p, const uint8_t* data, size_t size, int32_t slot,
+                                          const jxlb_write_spec* spec, void* dst, size_t dst_bytes, int32_t dst_on_device,
+                                          uint64_t tag);
 /* jxlb_pipeline_wait plus the keyframe index of the report (-1 for a frame of jxlb_pipeline_submit). */
 int32_t jxlb_pipeline_wait_keyframe(jxlb_pipeline* p, uint64_t* tag, int32_t* keyframe, int32_t* status, void** out,
                                     size_t* out_bytes, char* err, size_t err_cap);

@@ -36,7 +36,15 @@ EXPORTED_SYMBOLS = [
     "jxlb_pipeline_wait", "jxlb_pipeline_release_output", "jxlb_pipeline_launch_count", "jxlb_pipeline_workers", "jxlb_pipeline_decoder",
     "jxlb_jpeg_reconstruction_status", "jxlb_reconstruct_jpeg", "jxlb_jpeg_copy",
     "jxlb_image_keyframes", "jxlb_decode_keyframe", "jxlb_pipeline_submit_keyframes", "jxlb_pipeline_wait_keyframe",
+    "jxlb_frame_write_size", "jxlb_frame_write_ex", "jxlb_pipeline_submit_ex", "jxlb_pipeline_submit_keyframes_ex",
 ]
+
+# Output layouts of Decoder.frame_write / jxlb_write_spec: Render::stream(), stream_no_alpha(), image_all_channels(),
+# image_planar() (oriented)
+LAYOUT_STREAM, LAYOUT_STREAM_NO_ALPHA, LAYOUT_ALL_INTERLEAVED, LAYOUT_ALL_PLANAR = range(4)
+_LAYOUT_NAMES = {"stream": LAYOUT_STREAM, "stream_no_alpha": LAYOUT_STREAM_NO_ALPHA, "all_channels": LAYOUT_ALL_INTERLEAVED,
+                 "planar": LAYOUT_ALL_PLANAR}
+_SAMPLE_TYPES = {np.dtype(np.uint8): 0, np.dtype(np.uint16): 1, np.dtype(np.float32): 2}
 
 
 class JxlError(RuntimeError):
@@ -67,6 +75,18 @@ class _ImageInfo(ctypes.Structure):
 
 class _Section(ctypes.Structure):
     _fields_ = [("data", ctypes.c_char_p), ("size", ctypes.c_size_t)]
+
+
+class WriteSpec(ctypes.Structure):
+    """jxlb_write_spec: what Decoder.frame_write and Pipeline.submit(spec=...) write."""
+    _fields_ = [(n, ctypes.c_int32) for n in ("layout", "sample_type", "orientation", "render_spot_colour")]
+
+
+def write_spec(layout=LAYOUT_STREAM, dtype=np.uint8, orientation=0, spot_colours=True):
+    """A WriteSpec: `layout` a LAYOUT_* value or its name ("stream", "stream_no_alpha", "all_channels", "planar"), `dtype`
+    uint8 / uint16 / float32, `orientation` 1..8 or 0 for the image's, `spot_colours` False to leave spot colours unmixed."""
+    layout = _LAYOUT_NAMES.get(layout, layout)
+    return WriteSpec(int(layout), _SAMPLE_TYPES[np.dtype(dtype)], int(orientation), int(bool(spot_colours)))
 
 
 class _PipelineConfig(ctypes.Structure):
@@ -169,6 +189,13 @@ def load_library():
     L.jxlb_image_keyframes.argtypes = [ctypes.c_char_p, ctypes.c_size_t, ctypes.POINTER(i32), ctypes.POINTER(i32)]
     L.jxlb_image_keyframes.restype = i32
     L.jxlb_decode_keyframe.argtypes = [vp, ctypes.c_char_p, ctypes.c_size_t, ctypes.POINTER(_Options), i32]
+    L.jxlb_frame_write_size.argtypes = [vp, i32, ctypes.POINTER(WriteSpec), ctypes.POINTER(u32), ctypes.POINTER(ctypes.c_uint64)]
+    L.jxlb_frame_write_size.restype = i32
+    L.jxlb_frame_write_ex.argtypes = [vp, i32, ctypes.POINTER(WriteSpec), vp, ctypes.c_size_t, i32]
+    L.jxlb_frame_write_ex.restype = i32
+    L.jxlb_pipeline_submit_ex.argtypes = [vp, vp, ctypes.c_size_t, i32, ctypes.POINTER(WriteSpec), vp, ctypes.c_size_t, i32, ctypes.c_uint64]
+    L.jxlb_pipeline_submit_keyframes_ex.argtypes = [vp, vp, ctypes.c_size_t, i32, ctypes.POINTER(WriteSpec), vp, ctypes.c_size_t, i32,
+                                                    ctypes.c_uint64]
     _lib = L
     return L
 
@@ -357,6 +384,38 @@ class Decoder:
         self._check(self._L.jxlb_frame_write_to_device(self._h, frame, st, orientation, out.data_ptr(), out.numel() * out.element_size()))
         return out
 
+    def frame_write_shape(self, frame, spec: WriteSpec):
+        """(shape, nbytes) of frame_write's output: (height, width, channels) interleaved or (channels, height, width)
+        planar, oriented."""
+        n, nbytes = ctypes.c_uint32(), ctypes.c_uint64()
+        self._check(self._L.jxlb_frame_write_size(self._h, frame, ctypes.byref(spec), ctypes.byref(n), ctypes.byref(nbytes)))
+        info = self.frame_info(frame)
+        orient = spec.orientation or self.image_info().orientation
+        w, h = (info.height, info.width) if orient >= 5 else (info.width, info.height)
+        shape = (n.value, h, w) if spec.layout == LAYOUT_ALL_PLANAR else (h, w, n.value)
+        return shape, nbytes.value
+
+    def frame_write(self, frame, layout=LAYOUT_STREAM, dtype=np.uint8, orientation=0, spot_colours=True, out=None):
+        """One of the Render layouts (jxlb_frame_write_ex), packed on the device: `layout` as for write_spec(). Returns a
+        numpy array, or fills `out`: a C-contiguous numpy array, or a contiguous torch CUDA tensor of this decoder's GPU
+        (the samples then stay in HBM), of frame_write_shape()'s shape and `dtype`."""
+        spec = write_spec(layout, dtype, orientation, spot_colours)
+        shape, nbytes = self.frame_write_shape(frame, spec)
+        if out is None:
+            out = np.empty(shape, dtype=dtype)
+        if hasattr(out, "data_ptr"):
+            import torch
+            tdt = {0: torch.uint8, 1: torch.uint16, 2: torch.float32}[spec.sample_type]
+            if tuple(out.shape) != shape or out.dtype != tdt or not out.is_contiguous() or not out.is_cuda:
+                raise ValueError(f"out must be a contiguous CUDA {tdt} tensor of shape {shape}")
+            dst, on_device = out.data_ptr(), 1
+        else:
+            if out.shape != shape or out.dtype != np.dtype(dtype) or not out.flags.c_contiguous:
+                raise ValueError(f"out must be a C-contiguous {np.dtype(dtype)} array of shape {shape}")
+            dst, on_device = out.ctypes.data, 0
+        self._check(self._L.jxlb_frame_write_ex(self._h, frame, ctypes.byref(spec), dst, nbytes, on_device))
+        return out
+
     def set_capture(self, on=True):
         self._L.jxlb_set_capture(self._h, int(on))
 
@@ -499,18 +558,34 @@ class Pipeline:
             dst, nbytes = (out.ctypes.data, out.nbytes) if out is not None else (None, 0)
         return mode, dst, nbytes
 
-    def submit(self, data=None, slot=-1, out=None, mode=None, tag=None):
+    @staticmethod
+    def _spec_dst(out):
+        """(dst, nbytes, on_device) of a spec submission: a torch CUDA tensor, a numpy array, or None for the ring."""
+        if out is None:
+            return None, 0, 0
+        if hasattr(out, "data_ptr"):
+            return int(out.data_ptr()), out.numel() * out.element_size(), 1
+        return out.ctypes.data, out.nbytes, 0
+
+    def submit(self, data=None, slot=-1, out=None, mode=None, tag=None, spec=None):
         """Queues one frame: `data` (bytes) or a preloaded `slot`. `out`: None (decode only), a float32 (c, h, w) array
-        (planar) or a uint8 / uint16 (h, w, c) array (interleaved); it must stay untouched until wait() reports the tag."""
+        (planar) or a uint8 / uint16 (h, w, c) array (interleaved); it must stay untouched until wait() reports the tag.
+        With `spec` (a WriteSpec, see write_spec()) the frame is written as it describes, into `out` (a numpy array, or a
+        torch CUDA tensor that is filled on the device) or, with out=None, into a buffer of the pipeline's ring."""
         if tag is None:
             tag = self._next_tag
             self._next_tag += 1
-        mode, dst, nbytes = self._dst(out, mode)
         buf = None
         if data is not None:
             buf = ctypes.c_char_p(data)
-        rc = self._L.jxlb_pipeline_submit(self._h, ctypes.cast(buf, ctypes.c_void_p) if buf is not None else None,
-                                          len(data) if data is not None else 0, slot, mode, dst, nbytes, tag)
+        src = ctypes.cast(buf, ctypes.c_void_p) if buf is not None else None
+        if spec is not None:
+            dst, nbytes, on_device = self._spec_dst(out)
+            rc = self._L.jxlb_pipeline_submit_ex(self._h, src, len(data) if data is not None else 0, slot, ctypes.byref(spec), dst,
+                                                 nbytes, on_device, tag)
+        else:
+            mode, dst, nbytes = self._dst(out, mode)
+            rc = self._L.jxlb_pipeline_submit(self._h, src, len(data) if data is not None else 0, slot, mode, dst, nbytes, tag)
         if rc != OK:
             self._err(rc)
         self._keep[tag] = (data, buf, out)
@@ -540,19 +615,24 @@ class Pipeline:
             self._L.jxlb_pipeline_release_output(self._h, out)
         return tag.value
 
-    def submit_keyframes(self, data=None, slot=-1, out=None, mode=None, tag=None):
+    def submit_keyframes(self, data=None, slot=-1, out=None, mode=None, tag=None, spec=None):
         """Queues every keyframe of `data` (bytes) or of a preloaded `slot`, one task per independent segment
         (jxlb_pipeline_submit_keyframes). `out` as for submit() with a leading keyframe axis: (num_keyframes, ...);
-        keyframe k lands in out[k]. Collect the reports with wait_keyframe(); with out=None and a mode, release each
-        output as it is consumed. Returns the tag."""
+        keyframe k lands in out[k]. Collect the reports with wait_keyframe(); with out=None and a mode or a spec, release
+        each output as it is consumed. `spec` as for submit(). Returns the tag."""
         if tag is None:
             tag = self._next_tag
             self._next_tag += 1
-        mode, dst, nbytes = self._dst(out, mode)
         reports = _keyframe_reports(data) if data is not None else self._slot_reports.get(slot, 1)
         buf = ctypes.c_char_p(data) if data is not None else None
-        rc = self._L.jxlb_pipeline_submit_keyframes(self._h, ctypes.cast(buf, ctypes.c_void_p) if buf is not None else None,
-                                                    len(data) if data is not None else 0, slot, mode, dst, nbytes, tag)
+        src = ctypes.cast(buf, ctypes.c_void_p) if buf is not None else None
+        if spec is not None:
+            dst, nbytes, on_device = self._spec_dst(out)
+            rc = self._L.jxlb_pipeline_submit_keyframes_ex(self._h, src, len(data) if data is not None else 0, slot, ctypes.byref(spec),
+                                                           dst, nbytes, on_device, tag)
+        else:
+            mode, dst, nbytes = self._dst(out, mode)
+            rc = self._L.jxlb_pipeline_submit_keyframes(self._h, src, len(data) if data is not None else 0, slot, mode, dst, nbytes, tag)
         if rc != OK:
             self._err(rc)
         if reports:
@@ -630,15 +710,33 @@ class Pipeline:
 
 
 class Render:
-    """Result of JxlImage.render_frame(): planar f32 channels (crates/jxl-oxide/src/lib.rs:1080-1216)."""
+    """Result of JxlImage.render_frame(): planar f32 channels (crates/jxl-oxide/src/lib.rs:1080-1216). The layouts with
+    the orientation applied are packed on the device from the frame still resident in `decoder`."""
 
-    def __init__(self, planar, num_color, is_vardct):
+    def __init__(self, planar, num_color, is_vardct, decoder=None, frame=0, spot_colours=True):
         self._planar = planar
         self.num_color = num_color
         self.is_vardct = is_vardct
+        self._dec = decoder
+        self._frame = frame
+        self._spot_colours = spot_colours
 
-    def image_planar(self):
-        return self._planar
+    def image_planar(self, oriented=False):
+        """The stored planes (channels, height, width) float32; oriented=True: Render::image_planar(), every channel with
+        the image's orientation applied."""
+        if not oriented:
+            return self._planar
+        return self._dec.frame_write(self._frame, LAYOUT_ALL_PLANAR, np.float32)
+
+    def stream(self, no_alpha=False, dtype=np.float32, out=None):
+        """Render::stream() / stream_no_alpha() written out: colour, black and alpha channels (h, w, c), spot colours
+        mixed in unless JxlImage.set_render_spot_color(False), oriented. `out` as for Decoder.frame_write()."""
+        layout = LAYOUT_STREAM_NO_ALPHA if no_alpha else LAYOUT_STREAM
+        return self._dec.frame_write(self._frame, layout, dtype, spot_colours=self._spot_colours, out=out)
+
+    def image_all_channels(self, dtype=np.float32, out=None):
+        """Render::image_all_channels(): every channel interleaved (h, w, c), oriented."""
+        return self._dec.frame_write(self._frame, LAYOUT_ALL_INTERLEAVED, dtype, out=out)
 
     def color_channels(self):
         return self._planar[: self.num_color]
@@ -660,6 +758,8 @@ class JxlImage:
         self.bits_per_sample = info.bits_per_sample
         self.num_extra_channels = info.num_extra_channels
         self.xyb_encoded = bool(info.xyb_encoded)
+        self._grayscale = bool(info.grayscale)
+        self._render_spot_color = True
 
     @classmethod
     def read(cls, data: bytes, **kw):
@@ -675,7 +775,19 @@ class JxlImage:
 
     def render_frame(self, keyframe_index=0):
         info = self._dec.frame_info(keyframe_index)
-        return Render(self._dec.frame_planar(keyframe_index), info.num_color, bool(info.is_vardct))
+        return Render(self._dec.frame_planar(keyframe_index), info.num_color, bool(info.is_vardct), self._dec, keyframe_index,
+                      self._render_spot_color)
+
+    def render_spot_color(self):
+        return self._render_spot_color
+
+    def set_render_spot_color(self, render_spot_color: bool):
+        """JxlImage::set_render_spot_color (lib.rs:599-610): whether Render.stream() mixes the spot colours in. Turning it on
+        for a grayscale image is ignored, as the reference does."""
+        if render_spot_color and self._grayscale:
+            return self
+        self._render_spot_color = bool(render_spot_color)
+        return self
 
     @property
     def decoder(self):

@@ -14,7 +14,7 @@ OUT = os.path.join(HERE, "libjxlb200.so")
 
 SOURCES = [
     "capi.cu", "cuda_backend.cu", "launch_tables.cc", "pipeline.cu",
-    "kernels/modular.cu", "kernels/modular_stream.cu", "kernels/entropy.cu", "kernels/blockinfo.cu", "kernels/vardct.cu", "kernels/filters.cu", "kernels/filters_fused.cu", "kernels/jpeg.cu",
+    "kernels/modular.cu", "kernels/modular_stream.cu", "kernels/entropy.cu", "kernels/blockinfo.cu", "kernels/vardct.cu", "kernels/filters.cu", "kernels/filters_fused.cu", "kernels/jpeg.cu", "kernels/pack.cu",
     "host/entropy.cc", "host/headers.cc", "host/modular_syntax.cc", "host/frame_syntax.cc", "host/planner.cc", "host/icc.cc", "host/jbrd.cc", "host/frame_index.cc",
 ]
 

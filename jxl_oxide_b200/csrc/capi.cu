@@ -485,6 +485,57 @@ int32_t write_frame(jxlb_decoder* dec, int32_t frame, int32_t sample_type, int32
 }
 }  // namespace
 
+static_assert(int(JXLB_LAYOUT_STREAM) == kWriteStream && int(JXLB_LAYOUT_STREAM_NO_ALPHA) == kWriteStreamNoAlpha &&
+                  int(JXLB_LAYOUT_ALL_INTERLEAVED) == kWriteAllInterleaved && int(JXLB_LAYOUT_ALL_PLANAR) == kWriteAllPlanar,
+              "the ABI's layout numbers are the planner's");
+
+namespace {
+WritePlan frame_write_plan(const jxlb_decoder* dec, int32_t frame, const jxlb_write_spec& spec) {
+  JXLB_CHECK(dec->have_result && frame >= 0 && size_t(frame) < dec->res.frames.size(), kErrInvalidArg, "no such frame");
+  return plan_write(dec->res.image_header, dec->res.frames[size_t(frame)], spec.layout, spec.sample_type, spec.orientation,
+                    spec.render_spot_colour != 0);
+}
+}  // namespace
+
+int32_t jxlb_frame_write_size(jxlb_decoder* dec, int32_t frame, const jxlb_write_spec* spec, uint32_t* num_channels,
+                              uint64_t* bytes) {
+  if (!dec || !spec) return JXLB_ERR_INVALID_ARG;
+  return guarded(dec, [&] {
+    const WritePlan w = frame_write_plan(dec, frame, *spec);
+    if (num_channels) *num_channels = uint32_t(w.layout.channels.size());
+    if (bytes) *bytes = w.bytes;
+  });
+}
+
+int32_t jxlb_frame_write_ex(jxlb_decoder* dec, int32_t frame, const jxlb_write_spec* spec, void* dst, size_t dst_bytes,
+                            int32_t dst_on_device) {
+  if (!dec || !spec || !dst) return JXLB_ERR_INVALID_ARG;
+  return guarded(dec, [&] {
+    const WritePlan w = frame_write_plan(dec, frame, *spec);
+    JXLB_CHECK(dst_bytes >= w.bytes, kErrInvalidArg, "destination buffer too small");
+    const DecodedFrame& f = dec->res.frames[size_t(frame)];
+    DevPackSpec p;
+    p.num_channels = uint32_t(w.layout.channels.size());
+    p.num_spots = uint32_t(w.layout.spots.size());
+    p.width = w.width;
+    p.height = w.height;
+    p.orientation = w.orientation;
+    p.sample_type = w.sample_type;
+    p.planar = w.planar ? 1 : 0;
+    std::vector<DevPackChannel> channels;
+    for (size_t c : w.layout.channels) {
+      const DevView d = dec->be->dev_view(f.channels[c]);
+      channels.push_back(DevPackChannel{static_cast<const float*>(d.ptr), d.stride});
+    }
+    std::vector<DevPackSpot> spots;
+    for (const StreamSpot& s : w.layout.spots) {
+      const DevView d = dec->be->dev_view(f.channels[s.channel]);
+      spots.push_back(DevPackSpot{static_cast<const float*>(d.ptr), d.stride, {s.rgb[0], s.rgb[1], s.rgb[2]}, s.solidity});
+    }
+    dec->be->pack(p, channels, spots, dst, w.bytes, dst_on_device != 0);
+  });
+}
+
 int32_t jxlb_frame_stream_channels(const jxlb_decoder* dec, int32_t frame) {
   if (!dec || !dec->have_result || frame < 0 || size_t(frame) >= dec->res.frames.size()) return -1;
   return int32_t(stream_layout(dec->res.image_header, dec->res.frames[frame]).channels.size());

@@ -1112,6 +1112,26 @@ void CudaBackend::pack_to_device(const DevPackParams& p, void* d_dst) {
   sync();  // the caller may hand the buffer to any stream (NCCL's, torch's) afterwards
 }
 
+void CudaBackend::pack(const DevPackSpec& p, const std::vector<DevPackChannel>& channels, const std::vector<DevPackSpot>& spots,
+                       void* dst, size_t bytes, bool dst_on_device) {
+  if (dst_on_device) {
+    cudaPointerAttributes attr;
+    if (cudaPointerGetAttributes(&attr, dst) != cudaSuccess || attr.type != cudaMemoryTypeDevice || attr.device != device_) {
+      cudaGetLastError();
+      fail(kErrInvalidArg, "destination is not device memory of this decoder's GPU");
+    }
+  }
+  const auto* d_channels = static_cast<const DevPackChannel*>(upload_temp(channels.data(), channels.size() * sizeof(DevPackChannel)));
+  const auto* d_spots = spots.empty() ? nullptr : static_cast<const DevPackSpot*>(upload_temp(spots.data(), spots.size() * sizeof(DevPackSpot)));
+  void* out = dst_on_device ? dst : dmalloc(bytes);
+  begin_k("pack");
+  launch_pack(p, d_channels, d_spots, out, S());
+  end_k();
+  if (!dst_on_device) CUDA_CHECK(cudaMemcpyAsync(dst, out, bytes, cudaMemcpyDeviceToHost, S()));
+  sync();  // a device destination may go to any stream (NCCL's, torch's) afterwards
+  if (!dst_on_device) dfree(out);
+}
+
 int CudaBackend::upsample(const View& v, uint32_t factor_log2, const ImageHeader& ih) {
   DevView cur = dev_view(v);
   void* cur_owned = nullptr;

@@ -142,6 +142,10 @@ class CudaBackend : public Backend, private TableSink {
   void pack_to_host(const DevPackParams& p, void* dst, size_t bytes);
   // Same, straight into the caller's device buffer (no host copy): the packed frame stays in HBM for an NCCL gather.
   void pack_to_device(const DevPackParams& p, void* d_dst);
+  // Any layout (launch_pack): the tables go up with the launch; `dst` is host memory of `bytes`, or device memory of this
+  // decoder's GPU. Returns after the samples are in `dst`.
+  void pack(const DevPackSpec& p, const std::vector<DevPackChannel>& channels, const std::vector<DevPackSpot>& spots, void* dst,
+            size_t bytes, bool dst_on_device);
   bool fuse_filters = true;  // single-kernel Gaborish+EPF+colour (off: stage-by-stage, for stage parity tests)
   // HF coefficient streams per CTA (jxlb_set_hf_streams_per_cta, hf_schedule). Initialised from JXLB_HF_LANES.
   int hf_streams_per_cta = 0;

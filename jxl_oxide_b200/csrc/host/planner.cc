@@ -1340,7 +1340,7 @@ bool FramePlanner::colour_transform(std::vector<View> colour, const std::vector<
 
 }  // namespace
 
-StreamLayout stream_layout(const ImageHeader& ih, const DecodedFrame& f) {
+StreamLayout stream_layout(const ImageHeader& ih, const DecodedFrame& f, bool skip_alpha, bool render_spot_colour) {
   StreamLayout l;
   for (size_t c = 0; c < f.num_color && c < f.channels.size(); ++c) l.channels.push_back(c);
   if (ih.icc_is_cmyk)  // fb.rs:211-226
@@ -1349,18 +1349,49 @@ StreamLayout stream_layout(const ImageHeader& ih, const DecodedFrame& f) {
         l.channels.push_back(f.num_color + e);
         break;
       }
-  for (size_t e = 0; e < ih.ec_info.size() && f.num_color + e < f.channels.size(); ++e)
-    if (ih.ec_info[e].type == ExtraChannelType::kAlpha) {
-      l.channels.push_back(f.num_color + e);
-      break;
-    }
-  if (f.num_color == 3 && !ih.grayscale())
+  if (!skip_alpha)  // fb.rs:228-243
+    for (size_t e = 0; e < ih.ec_info.size() && f.num_color + e < f.channels.size(); ++e)
+      if (ih.ec_info[e].type == ExtraChannelType::kAlpha) {
+        l.channels.push_back(f.num_color + e);
+        break;
+      }
+  if (render_spot_colour && f.num_color == 3 && !ih.grayscale())
     for (size_t e = 0; e < ih.ec_info.size() && f.num_color + e < f.channels.size(); ++e)
       if (ih.ec_info[e].type == ExtraChannelType::kSpotColour) {
         const float* s = ih.ec_info[e].spot;
         l.spots.push_back(StreamSpot{f.num_color + e, {s[0], s[1], s[2]}, s[3]});
       }
   return l;
+}
+
+StreamLayout all_channels_layout(const DecodedFrame& f) {
+  StreamLayout l;
+  for (size_t c = 0; c < f.channels.size(); ++c) l.channels.push_back(c);
+  return l;
+}
+
+WritePlan plan_write(const ImageHeader& ih, const DecodedFrame& f, int32_t layout, int32_t sample_type, int32_t orientation,
+                     bool render_spot_colour) {
+  JXLB_CHECK(layout >= kWriteStream && layout <= kWriteAllPlanar, kErrInvalidArg,
+             "layout must be 0 (stream), 1 (stream without alpha), 2 (all channels interleaved) or 3 (all channels planar)");
+  JXLB_CHECK(sample_type >= 0 && sample_type <= 2, kErrInvalidArg, "sample_type must be 0 (u8), 1 (u16) or 2 (f32)");
+  JXLB_CHECK(orientation >= 0 && orientation <= 8, kErrInvalidArg, "orientation must be 1..8 (0 = the image's)");
+  JXLB_CHECK(!f.channels.empty(), kErrInvalidArg, "frame without channels");
+  WritePlan w;
+  w.layout = layout <= kWriteStreamNoAlpha ? stream_layout(ih, f, layout == kWriteStreamNoAlpha, render_spot_colour)
+                                           : all_channels_layout(f);
+  w.orientation = orientation == 0 ? ih.orientation : uint32_t(orientation);
+  JXLB_CHECK(w.orientation >= 1 && w.orientation <= 8, kErrInvalidArg, "orientation must be 1..8 (0 = the image's)");
+  w.sample_type = uint32_t(sample_type);
+  w.planar = layout == kWriteAllPlanar;
+  w.width = f.channels[0].w;
+  w.height = f.channels[0].h;
+  for (size_t c : w.layout.channels)
+    JXLB_CHECK(f.channels[c].w == w.width && f.channels[c].h == w.height, kErrUnsupported, "channels of different sizes");
+  for (const StreamSpot& s : w.layout.spots)
+    JXLB_CHECK(f.channels[s.channel].w == w.width && f.channels[s.channel].h == w.height, kErrUnsupported, "channels of different sizes");
+  w.bytes = size_t(w.width) * w.height * w.layout.channels.size() * (sample_type == 0 ? 1 : (sample_type == 1 ? 2 : 4));
+  return w;
 }
 
 size_t parse_codestream_header(const uint8_t* cs, size_t size, ImageHeader* out) {

@@ -66,7 +66,27 @@ struct StreamLayout {
   std::vector<size_t> channels;  // indices into DecodedFrame::channels, in output order
   std::vector<StreamSpot> spots;
 };
-StreamLayout stream_layout(const ImageHeader& ih, const DecodedFrame& f);
+// `skip_alpha` leaves the alpha channel out (Render::stream_no_alpha); `render_spot_colour` off leaves the spot colours
+// unmixed (JxlImage::set_render_spot_color(false), fb.rs:247).
+StreamLayout stream_layout(const ImageHeader& ih, const DecodedFrame& f, bool skip_alpha = false, bool render_spot_colour = true);
+// Render::image_all_channels / image_planar (lib.rs:1150-1198): the colour channels, then every extra channel in header
+// order; nothing is mixed.
+StreamLayout all_channels_layout(const DecodedFrame& f);
+
+// One write of a frame's samples (jxlb_write_spec, include/jxlb200.h): which planes go where, and the output's size.
+enum WriteLayout : int32_t { kWriteStream = 0, kWriteStreamNoAlpha = 1, kWriteAllInterleaved = 2, kWriteAllPlanar = 3 };
+struct WritePlan {
+  StreamLayout layout;
+  uint32_t orientation = 1;  // 1..8
+  uint32_t sample_type = 0;  // 0: u8, 1: u16, 2: f32
+  bool planar = false;
+  uint32_t width = 0, height = 0;  // of the stored planes; the output is height x width for orientations 5..8
+  size_t bytes = 0;
+};
+// Throws kErrInvalidArg for a layout, sample type or orientation (0 = the image's, else 1..8) out of range, and
+// kErrUnsupported when the selected planes differ in size. `render_spot_colour` matters to the stream layouts only.
+WritePlan plan_write(const ImageHeader& ih, const DecodedFrame& f, int32_t layout, int32_t sample_type, int32_t orientation,
+                     bool render_spot_colour);
 
 struct DecodeResult {
   ImageHeader image_header;

@@ -255,6 +255,27 @@ struct DevPackParams {
   float spot_solidity[8];
 };
 void launch_pack_interleaved(DevPackParams p, void* out, cudaStream_t stream);
+// Every output layout of a frame (pack.cu, per-sample rules in pack.cuh): any number of f32 planes, read through channel
+// and spot tables in device memory, to u8 / u16 / f32 samples interleaved (channel fastest) or planar (channel-major), with
+// the orientation applied.
+struct DevPackChannel {
+  const float* plane;
+  uint32_t stride;
+};
+struct DevPackSpot {
+  const float* plane;
+  uint32_t stride;
+  float rgb[3];
+  float solidity;
+};
+struct DevPackSpec {
+  uint32_t num_channels, num_spots;
+  uint32_t width, height;  // of the stored (un-oriented) planes
+  uint32_t orientation;    // 1..8
+  uint32_t sample_type;    // 0: u8, 1: u16, 2: f32
+  uint32_t planar;         // 0: interleaved, 1: one plane per channel
+};
+void launch_pack(const DevPackSpec& p, const DevPackChannel* channels, const DevPackSpot* spots, void* out, cudaStream_t stream);
 // Rectangle blending (jxl-render/src/blend.rs:550-727), one CTA per job; modes 1 Replace, 2 Add, 3 Mul,
 // 4 Blend, 5 MulAdd, 6 MixAlpha.
 struct DevPatchJob {

@@ -49,6 +49,9 @@ struct Job {
   size_t size = 0;
   int32_t slot = -1;              // a preloaded slot
   int32_t out_mode = 0;
+  bool has_spec = false;  // jxlb_pipeline_submit_ex: `spec` replaces out_mode
+  jxlb_write_spec spec{};
+  bool dst_on_device = false;
   void* dst = nullptr;
   size_t dst_bytes = 0;
   uint64_t tag = 0;
@@ -532,7 +535,7 @@ struct jxlb_pipeline {
           rc = decode_resident(dec, r->codestream.data(), r->codestream.size(), r->dptr, nullptr);
         }
       }
-      if (rc == JXLB_OK) rc = deliver(dec, job.out_mode, job.dst, job.dst_bytes, d);
+      if (rc == JXLB_OK) rc = deliver(dec, job, job.dst, job.dst_bytes, d);
       if (rc != JXLB_OK) {
         d.status = rc;
         d.error = dec->error;
@@ -551,25 +554,33 @@ struct jxlb_pipeline {
     cv_done.notify_all();
   }
 
-  // Packs frame 0 of `dec` as `out_mode` asks into `dst` (NULL: a buffer of the ring) and records in `d` where it went.
-  int32_t deliver(jxlb_decoder* dec, int32_t out_mode, void* dst, size_t dst_bytes, Done& d) {
+  // Packs frame 0 of `dec` as the job's spec or, without one, its `out_mode` asks into `dst` (NULL: a buffer of the ring)
+  // and records in `d` where it went.
+  int32_t deliver(jxlb_decoder* dec, const Job& job, void* dst, size_t dst_bytes, Done& d) {
+    const jxlb_write_spec* spec = job.has_spec ? &job.spec : nullptr;
+    const int32_t out_mode = job.out_mode;
     int32_t rc = JXLB_OK;
     const bool own = !dst;
-    if (out_mode == 4 || out_mode == 5) {
+    if (spec ? job.dst_on_device : (out_mode == 4 || out_mode == 5)) {
       // packed straight into the caller's device buffer (input of an NCCL gather): no host link involved
-      rc = jxlb_frame_write_to_device(dec, 0, out_mode - 4, 0, dst, dst_bytes);
+      rc = spec ? jxlb_frame_write_ex(dec, 0, spec, dst, dst_bytes, 1) : jxlb_frame_write_to_device(dec, 0, out_mode - 4, 0, dst, dst_bytes);
       d.out = dst;
       d.out_bytes = dst_bytes;
-    } else if (out_mode != 0) {
+    } else if (spec || out_mode != 0) {
       if (!dst) {  // library-owned pinned staging, sized from the decoded frame
         jxlb_frame_info fi;
         jxlb_frame_get_info(dec, 0, &fi);
-        if (out_mode == 1) {
+        if (spec) {
+          uint64_t bytes = 0;
+          rc = jxlb_frame_write_size(dec, 0, spec, nullptr, &bytes);
+          dst_bytes = size_t(bytes);
+        } else if (out_mode == 1) {
           dst_bytes = 0;
           for (const View& v : dec->res.frames[0].channels) dst_bytes += size_t(v.w) * v.h * 4;
         } else {
           dst_bytes = size_t(fi.width) * fi.height * size_t(jxlb_frame_stream_channels(dec, 0)) * (out_mode == 2 ? 1 : 2);
         }
+        if (rc != JXLB_OK) return rc;
         dst = acquire_host(dst_bytes);
         if (!dst) {
           rc = JXLB_ERR_CUDA;
@@ -583,7 +594,8 @@ struct jxlb_pipeline {
         rc = jxlb_sync(dec);
         std::lock_guard<std::mutex> copy_lock(copy_mu);
         if (rc != JXLB_OK) {
-        } else if (out_mode == 1) rc = frame_planar_to_host(dec, 0, static_cast<float*>(dst), dst_bytes);
+        } else if (spec) rc = jxlb_frame_write_ex(dec, 0, spec, dst, dst_bytes, 0);
+        else if (out_mode == 1) rc = frame_planar_to_host(dec, 0, static_cast<float*>(dst), dst_bytes);
         else rc = jxlb_frame_write_to_buffer(dec, 0, out_mode - 2, 0, dst, dst_bytes);
         d.out = dst;
         d.out_bytes = dst_bytes;
@@ -612,7 +624,7 @@ struct jxlb_pipeline {
           Done d{job.tag, JXLB_OK, std::string()};
           d.keyframe = int32_t(k);
           void* dst = job.dst ? static_cast<uint8_t*>(job.dst) + size_t(k) * per_keyframe : nullptr;
-          const int32_t r = deliver(dec, job.out_mode, dst, per_keyframe, d);
+          const int32_t r = deliver(dec, job, dst, per_keyframe, d);
           if (r == JXLB_OK) {
             report(std::move(d));
             next = k + 1;
@@ -710,17 +722,15 @@ int32_t jxlb_pipeline_preload(jxlb_pipeline* p, int32_t slot, const uint8_t* dat
   }
 }
 
-int32_t jxlb_pipeline_submit(jxlb_pipeline* p, const uint8_t* data, size_t size, int32_t slot, int32_t out_mode, void* dst,
-                             size_t dst_bytes, uint64_t tag) {
-  if (!p || out_mode < 0 || out_mode > 5 || (!data && slot < 0) || (out_mode >= 4 && !dst)) return JXLB_ERR_INVALID_ARG;
-  Job j;
+}  // extern "C"
+
+namespace {
+// Queues one frame; `out` carries the output fields of the Job (out_mode or spec, destination).
+int32_t submit_frame(jxlb_pipeline* p, const uint8_t* data, size_t size, int32_t slot, const Job& out) {
+  Job j = out;
   j.data = data;
   j.size = size;
   j.slot = slot;
-  j.out_mode = out_mode;
-  j.dst = dst;
-  j.dst_bytes = dst_bytes;
-  j.tag = tag;
   {
     std::lock_guard<std::mutex> lk(p->mu);
     if (p->stopping) return JXLB_ERR_INVALID_ARG;
@@ -731,11 +741,10 @@ int32_t jxlb_pipeline_submit(jxlb_pipeline* p, const uint8_t* data, size_t size,
   return JXLB_OK;
 }
 
-int32_t jxlb_pipeline_submit_keyframes(jxlb_pipeline* p, const uint8_t* data, size_t size, int32_t slot, int32_t out_mode,
-                                       void* dst, size_t dst_bytes, uint64_t tag) {
-  if (!p || out_mode < 0 || out_mode > 5 || (!data && slot < 0) || (out_mode >= 4 && !dst)) return JXLB_ERR_INVALID_ARG;
+// Queues one task per segment of the image; `out` as for submit_frame.
+int32_t submit_keyframes(jxlb_pipeline* p, const uint8_t* data, size_t size, int32_t slot, const Job& out) {
   auto ks = std::make_shared<KeyframeSubmission>();
-  Done fail_all{tag, JXLB_OK, std::string()};
+  Done fail_all{out.tag, JXLB_OK, std::string()};
   try {
     if (data) {
       ks->codestream = extract_codestream(data, size);
@@ -760,13 +769,9 @@ int32_t jxlb_pipeline_submit_keyframes(jxlb_pipeline* p, const uint8_t* data, si
       ++p->submitted;
     } else {
       for (size_t s = 0; s < ks->index.segments.size(); ++s) {
-        Job j;
+        Job j = out;
         j.keyframes = ks;
         j.segment = s;
-        j.out_mode = out_mode;
-        j.dst = dst;
-        j.dst_bytes = dst_bytes;
-        j.tag = tag;
         p->queue.push_back(j);
       }
       p->submitted += ks->index.num_keyframes;
@@ -775,6 +780,60 @@ int32_t jxlb_pipeline_submit_keyframes(jxlb_pipeline* p, const uint8_t* data, si
   if (fail_all.status != JXLB_OK) p->cv_done.notify_all();
   else p->cv_job.notify_all();
   return JXLB_OK;
+}
+
+Job mode_output(int32_t out_mode, void* dst, size_t dst_bytes, uint64_t tag) {
+  Job j;
+  j.out_mode = out_mode;
+  j.dst = dst;
+  j.dst_bytes = dst_bytes;
+  j.tag = tag;
+  return j;
+}
+
+Job spec_output(const jxlb_write_spec& spec, void* dst, size_t dst_bytes, int32_t dst_on_device, uint64_t tag) {
+  Job j;
+  j.has_spec = true;
+  j.spec = spec;
+  j.dst_on_device = dst_on_device != 0;
+  j.dst = dst;
+  j.dst_bytes = dst_bytes;
+  j.tag = tag;
+  return j;
+}
+
+// The checks a spec can take before a frame is decoded (the rest, e.g. the buffer size, needs the frame's header).
+bool spec_ok(const jxlb_write_spec* spec, const void* dst, int32_t dst_on_device) {
+  return spec && spec->layout >= JXLB_LAYOUT_STREAM && spec->layout <= JXLB_LAYOUT_ALL_PLANAR && spec->sample_type >= 0 &&
+         spec->sample_type <= 2 && spec->orientation >= 0 && spec->orientation <= 8 && (dst || !dst_on_device);
+}
+}  // namespace
+
+extern "C" {
+
+int32_t jxlb_pipeline_submit(jxlb_pipeline* p, const uint8_t* data, size_t size, int32_t slot, int32_t out_mode, void* dst,
+                             size_t dst_bytes, uint64_t tag) {
+  if (!p || out_mode < 0 || out_mode > 5 || (!data && slot < 0) || (out_mode >= 4 && !dst)) return JXLB_ERR_INVALID_ARG;
+  return submit_frame(p, data, size, slot, mode_output(out_mode, dst, dst_bytes, tag));
+}
+
+int32_t jxlb_pipeline_submit_keyframes(jxlb_pipeline* p, const uint8_t* data, size_t size, int32_t slot, int32_t out_mode,
+                                       void* dst, size_t dst_bytes, uint64_t tag) {
+  if (!p || out_mode < 0 || out_mode > 5 || (!data && slot < 0) || (out_mode >= 4 && !dst)) return JXLB_ERR_INVALID_ARG;
+  return submit_keyframes(p, data, size, slot, mode_output(out_mode, dst, dst_bytes, tag));
+}
+
+int32_t jxlb_pipeline_submit_ex(jxlb_pipeline* p, const uint8_t* data, size_t size, int32_t slot, const jxlb_write_spec* spec,
+                                void* dst, size_t dst_bytes, int32_t dst_on_device, uint64_t tag) {
+  if (!p || (!data && slot < 0) || !spec_ok(spec, dst, dst_on_device)) return JXLB_ERR_INVALID_ARG;
+  return submit_frame(p, data, size, slot, spec_output(*spec, dst, dst_bytes, dst_on_device, tag));
+}
+
+int32_t jxlb_pipeline_submit_keyframes_ex(jxlb_pipeline* p, const uint8_t* data, size_t size, int32_t slot,
+                                          const jxlb_write_spec* spec, void* dst, size_t dst_bytes, int32_t dst_on_device,
+                                          uint64_t tag) {
+  if (!p || (!data && slot < 0) || !spec_ok(spec, dst, dst_on_device)) return JXLB_ERR_INVALID_ARG;
+  return submit_keyframes(p, data, size, slot, spec_output(*spec, dst, dst_bytes, dst_on_device, tag));
 }
 
 int32_t jxlb_pipeline_wait_keyframe(jxlb_pipeline* p, uint64_t* tag, int32_t* keyframe, int32_t* status, void** out,
