@@ -1,6 +1,7 @@
-// tools/hf_restream — rewrites the HF passes of an existing VarDCT file with LZ77 codes, keeping everything else.
+// tools/hf_restream — rewrites the HF passes of an existing VarDCT file with LZ77 codes, or in one of synth_enc's
+// entropy-code forms (--code), keeping everything else.
 //
-//   hf_restream IN.jxl OUT.jxl rle|match
+//   hf_restream IN.jxl OUT.jxl rle|match|prefix|ans-forms|configs
 //
 // The container boxes (jbrd included), the image and frame headers, LfGlobal, the LF groups, HfGlobal's dequant
 // matrices and coefficient orders, and each pass group's HF preset and coefficient values stay bit for bit. Only the HF
@@ -8,6 +9,8 @@
 // sections and the TOC change. The values and their clusters come from one decode by the project's CPU oracle, traced
 // through EntropyReader (JXLB_ENTROPY_TRACE in host/entropy.h); the new streams are written by synth_enc's LZ77 parser
 // and ANS writer (lz77_parse, EntropyEncoder). The number of values the decoder takes from copies goes to stderr.
+// The form modes keep the context-to-cluster map too (the traced values carry their cluster, not their context) and
+// write the codes and streams in that form without LZ77; the writer's "code-form:" report goes to stderr.
 //
 // Not part of the product: test infrastructure (built with oracle/'s sources, see tools/hf_restream.py).
 #define SYNTH_ENC_NO_MAIN
@@ -77,10 +80,12 @@ void copy_bits(BitWriter& w, const std::vector<uint8_t>& src, size_t from, size_
 }  // namespace
 
 int main(int argc, char** argv) {
-  if (argc != 4) die("usage: hf_restream IN OUT rle|match");
+  if (argc != 4) die("usage: hf_restream IN OUT rle|match|prefix|ans-forms|configs");
   HfLz77 opt;
   opt.mode = argv[3];
-  if (opt.mode != "rle" && opt.mode != "match") die("mode is rle or match");
+  const bool form = opt.mode == "prefix" || opt.mode == "ans-forms" || opt.mode == "configs";
+  if (opt.mode != "rle" && opt.mode != "match" && !form) die("mode is rle, match, prefix, ans-forms or configs");
+  if (form) g_code = opt.mode, atexit([] { g_report.print(); });
   std::vector<uint8_t> file;
   {
     FILE* f = fopen(argv[1], "rb");
@@ -139,6 +144,7 @@ int main(int argc, char** argv) {
   std::vector<BitWriter> sections(toc.entries.size());
   std::vector<EntropyEncoder> enc(P);
   std::vector<std::vector<Sym>> syms(size_t(P) * num_groups);
+  std::vector<std::vector<Token>> tokens(size_t(P) * num_groups);  // form modes
   std::vector<const jxlb::TracedStream*> streams(size_t(P) * num_groups);
   std::vector<std::vector<uint8_t>> maps(P);
   for (uint32_t p = 0; p < P; ++p) {
@@ -155,10 +161,15 @@ int main(int argc, char** argv) {
       streams[size_t(p) * num_groups + g] = &it->second;
       std::vector<Token> toks;
       for (const auto& [cl, v] : it->second.values) toks.push_back({rep[cl], v});
+      if (form) {
+        tokens[size_t(p) * num_groups + g] = toks;
+        continue;
+      }
       syms[size_t(p) * num_groups + g] = lz77_parse(toks, opt, dist_ctx, false, &lzc);
       all.insert(all.end(), syms[size_t(p) * num_groups + g].begin(), syms[size_t(p) * num_groups + g].end());
     }
     maps[p] = code.cluster_map;
+    if (form) continue;
     maps[p].push_back(uint8_t(code.num_clusters));  // the distance context gets a cluster of its own
     if (code.num_clusters >= 255) die("too many clusters for a distance cluster of its own");
     static Lz77Header header;
@@ -174,10 +185,16 @@ int main(int argc, char** argv) {
     for (uint32_t p = 0; p < P; ++p) {
       const jxlb::TracedCode& code = jxlb::g_codes[p];
       copy_bits(w, cs, at, code.begin);
+      at = code.end;
+      if (form) {
+        std::vector<Token> all;
+        for (uint32_t g = 0; g < num_groups; ++g) all.insert(all.end(), tokens[size_t(p) * num_groups + g].begin(), tokens[size_t(p) * num_groups + g].end());
+        enc[p].write_header(w, all, uint32_t(maps[p].size()), maps[p]);
+        continue;
+      }
       std::vector<Sym> all;
       for (uint32_t g = 0; g < num_groups; ++g) all.insert(all.end(), syms[size_t(p) * num_groups + g].begin(), syms[size_t(p) * num_groups + g].end());
       enc[p].write_header_syms(w, all, uint32_t(maps[p].size()), maps[p]);
-      at = code.end;
     }
     w.pad();  // nothing follows the last pass code but padding
   }
@@ -189,7 +206,8 @@ int main(int argc, char** argv) {
       const jxlb::TracedStream& s = *streams[size_t(p) * num_groups + g];
       BitWriter& w = sections[i];
       copy_bits(w, cs, b, s.begin);
-      enc[p].write_syms(w, syms[size_t(p) * num_groups + g]);
+      if (form) enc[p].write_tokens(w, tokens[size_t(p) * num_groups + g]);
+      else enc[p].write_syms(w, syms[size_t(p) * num_groups + g]);
       bool rest = false;  // anything but zero padding after the HF data
       for (size_t k = s.end; k < e && !rest; ++k) rest = (cs[k / 8] >> (k % 8)) & 1;
       if (rest) copy_bits(w, cs, s.end, e);

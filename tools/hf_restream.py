@@ -1,8 +1,8 @@
 """Builds and runs tools/hf_restream.cc: an existing VarDCT file with its HF passes rewritten with LZ77 codes (rle or
-match), everything else kept. Test infrastructure; the binary goes to a per-user temporary directory keyed by its
+match) or in an entropy-code form of synth_enc's --code (prefix, ans-forms or configs), everything else kept. Test infrastructure; the binary goes to a per-user temporary directory keyed by its
 sources, since the source tree may be read-only.
 
-    python tools/hf_restream.py IN.jxl OUT.jxl rle|match
+    python tools/hf_restream.py IN.jxl OUT.jxl rle|match|prefix|ans-forms|configs
 """
 import glob
 import hashlib
@@ -40,15 +40,18 @@ def tool():
 
 
 def restream(data: bytes, mode: str):
-    """(restreamed file, values the decoder takes from LZ77 copies as the restreamer counted them)."""
+    """(restreamed file, values the decoder takes from LZ77 copies as the restreamer counted them); for the
+    entropy-code forms, (restreamed file, the restreamer's stderr with its "code-form:" report)."""
     with tempfile.TemporaryDirectory() as d:
         src, dst = os.path.join(d, "in.jxl"), os.path.join(d, "out.jxl")
         with open(src, "wb") as f:
             f.write(data)
         r = subprocess.run([tool(), src, dst, mode], capture_output=True, text=True, check=True)
-        copied = int(r.stderr.split("values copied")[0].split(":")[-1])
         with open(dst, "rb") as f:
-            return f.read(), copied
+            out = f.read()
+        if mode not in ("rle", "match"):
+            return out, r.stderr
+        return out, int(r.stderr.split("values copied")[0].split(":")[-1])
 
 
 if __name__ == "__main__":
@@ -58,4 +61,4 @@ if __name__ == "__main__":
         out, n = restream(f.read(), sys.argv[3])
     with open(sys.argv[2], "wb") as f:
         f.write(out)
-    print(f"{len(out)} bytes, {n} values copied")
+    print(f"{len(out)} bytes", f"{n} values copied" if sys.argv[3] in ("rle", "match") else n.strip())

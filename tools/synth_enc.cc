@@ -25,7 +25,8 @@
 // skip_adaptive_lf_smoothing, each channel's LF and HF at its shifted grid; it combines with --hf-lz77, and
 // --dump-coeffs FILE writes the HF coefficients of any VarDCT frame. --upsampling K also codes a VarDCT
 // frame at ceil(W / K) x ceil(H / K), and --noise / --noise-zero, --splines N and --dangling-patch give a VarDCT frame
-// those LfGlobal features (write_features).
+// those LfGlobal features (write_features). --code FORM writes every entropy code of the file in one form of the
+// entropy-code syntax (prefix, ans-forms, configs, clusters; see g_code) and reports the branches it reached.
 //
 // Not part of the product; not a general-purpose encoder (it does not transform an input image).
 #include <algorithm>
@@ -247,6 +248,230 @@ void write_ans_histogram(BitWriter& w, const std::vector<uint32_t>& counts) {
   }
 }
 
+// ---- --code FORM: every entropy code of the file (MA tree, cluster maps, Modular channels, LF and HF) is written in
+// one form of the entropy-code syntax, from the spec semantics of jxl-coding (ans.rs, prefix.rs, lib.rs):
+//   prefix     prefix codes: length-limited (15) Huffman; clusters with at most 4 symbols in the simple form (NSYM 1-4,
+//              both tree_select values), the others in the complex form (hskip 0, 2 and 3 in turn, repeat codes 16 and
+//              17); in each code the cluster with the most symbols (16 or more) gets a chain-shaped code up to 15 bits.
+//   ans-forms  ANS at log alphabet 6, 7, 8 in turn; clusters of one or two symbols in the simple forms, the others
+//              flat, RLE-coded (logcount 13) or in the general form with shift 0..13 in turn.
+//   configs    ANS at log alphabet 8; each cluster takes the next hybrid-uint config of kFormConfigs that can code its
+//              values within the alphabet.
+//   clusters   ANS at log alphabet 8; context i goes to cluster i mod K: K of 65 to 256 in a complex cluster map (with
+//              and without move-to-front) where there are that many contexts, otherwise a simple map with nbits 0..3.
+// The writer builds its own tables and checks that parse_entropy_code reads back exactly what was written (exit 1
+// otherwise); FormReport lists the branches reached and goes to stderr as one "code-form:" line.
+std::string g_code;
+// --corrupt KIND: one invalid stream or code in the file, the rest as without it (tests of rejected streams):
+//   ans-state        the last Modular group's stream, or the first HF group's, is encoded from end state 0x130001: every
+//                    value decodes as written, but the stream does not end in state 0x130000 (lib.rs:176-180)
+//   truncate         the last section is cut to half its size, the TOC saying so: its stream ends early (with --code
+//                    prefix, nothing but the end of the data tells)
+//   oversub-clcl     the first complex prefix code's code-length code has its last length one shorter: over-subscribed
+//                    (prefix.rs:246-258)
+//   oversub-lengths  the first complex prefix code's last code length is one shorter: over-subscribed (prefix.rs:317-329)
+//   ans-sum          the first ANS histogram of a --code form is written with explicit counts summing past 4096
+//                    (ans.rs:172-175)
+std::string g_corrupt;
+bool g_corrupt_done = false;  // applied (once per file)
+bool g_flip_state = false;    // ans-state: set just before the stream to corrupt is written
+uint32_t g_code_seed = 0;  // --seed
+uint32_t g_code_turn = 0;  // advances with every choice the forms cycle through
+
+const UintConfig kFormConfigs[] = {{0, 0, 0}, {1, 0, 1}, {2, 1, 1}, {3, 0, 3}, {4, 2, 2}, {5, 1, 3}, {6, 3, 3},
+                                   {7, 0, 7}, {8, 0, 0}, {1, 1, 0}, {4, 2, 0}, {5, 0, 0}, {3, 1, 0}, {6, 0, 1}};
+
+struct FormReport {
+  uint64_t codes = 0, prefix_codes = 0, prefix_clusters = 0, single_symbol = 0, nsym[5] = {}, tree_select[2] = {},
+           hskip[4] = {}, repeat16 = 0, repeat17 = 0, long_codes = 0;
+  uint32_t max_prefix_len = 0, max_clusters = 0, max_ans_table_bytes = 0;
+  uint64_t ans_forms[5] = {};  // unary, binary, flat, general, rle
+  uint32_t shifts = 0, log_alphas = 0, map_nbits = 0, map_mtf = 0, configs = 0;  // bit sets
+  uint32_t rejected_by_parser = 0;  // codes made invalid by --corrupt that parse_entropy_code refused
+  void print() const {
+    fprintf(stderr,
+            "code-form: codes=%llu prefix_codes=%llu prefix_clusters=%llu single_symbol=%llu nsym=%llu,%llu,%llu,%llu "
+            "tree_select=%llu,%llu hskip0=%llu hskip2=%llu hskip3=%llu repeat16=%llu repeat17=%llu max_prefix_len=%u "
+            "root_bits=%u long_codes=%llu ans_unary=%llu ans_binary=%llu ans_flat=%llu ans_general=%llu ans_rle=%llu "
+            "shifts=0x%x log_alphas=0x%x max_clusters=%u map_nbits=0x%x map_mtf=0x%x configs=0x%x "
+            "max_ans_table_bytes=%u rejected_by_parser=%u\n",
+            (unsigned long long)codes, (unsigned long long)prefix_codes, (unsigned long long)prefix_clusters,
+            (unsigned long long)single_symbol, (unsigned long long)nsym[1], (unsigned long long)nsym[2],
+            (unsigned long long)nsym[3], (unsigned long long)nsym[4], (unsigned long long)tree_select[0],
+            (unsigned long long)tree_select[1], (unsigned long long)hskip[0], (unsigned long long)hskip[2],
+            (unsigned long long)hskip[3], (unsigned long long)repeat16, (unsigned long long)repeat17, max_prefix_len,
+            kPrefixRootBits, (unsigned long long)long_codes, (unsigned long long)ans_forms[0], (unsigned long long)ans_forms[1],
+            (unsigned long long)ans_forms[2], (unsigned long long)ans_forms[3], (unsigned long long)ans_forms[4], shifts,
+            log_alphas, max_clusters, map_nbits, map_mtf, configs, max_ans_table_bytes, rejected_by_parser);
+  }
+} g_report;
+
+[[noreturn]] void form_fail(const char* what, uint32_t cluster) {
+  fprintf(stderr, "--code %s: %s (cluster %u)\n", g_code.c_str(), what, cluster);
+  exit(1);
+}
+
+// Code lengths of min_len to max_len bits for the symbols with freq > 0 (a complete code when at least two symbols are
+// used and 2^min_len at most): Huffman, then lengths clamped and the Kraft sum brought back to exactly 1.
+std::vector<uint8_t> limited_lengths(const std::vector<double>& freq, uint32_t max_len, uint32_t min_len = 1) {
+  std::vector<uint8_t> len(freq.size(), 0);
+  struct Node {
+    double w;
+    int a, b;
+  };
+  std::vector<Node> nodes;
+  std::vector<std::pair<double, int>> heap;
+  for (size_t i = 0; i < freq.size(); ++i)
+    if (freq[i] > 0) nodes.push_back({freq[i], -1 - int(i), 0}), heap.push_back({-freq[i], int(nodes.size()) - 1});
+  if (nodes.size() < 2) {
+    for (const Node& n : nodes) len[size_t(-1 - n.a)] = 1;
+    return len;
+  }
+  std::make_heap(heap.begin(), heap.end());
+  while (heap.size() > 1) {
+    std::pop_heap(heap.begin(), heap.end());
+    const auto x = heap.back();
+    heap.pop_back();
+    std::pop_heap(heap.begin(), heap.end());
+    const auto y = heap.back();
+    heap.pop_back();
+    nodes.push_back({-x.first - y.first, x.second, y.second});
+    heap.push_back({x.first + y.first, int(nodes.size()) - 1});
+    std::push_heap(heap.begin(), heap.end());
+  }
+  std::function<void(int, uint32_t)> walk = [&](int n, uint32_t d) {
+    if (nodes[size_t(n)].a < 0) {
+      len[size_t(-1 - nodes[size_t(n)].a)] = uint8_t(std::min(std::max(d, min_len), max_len));
+      return;
+    }
+    walk(nodes[size_t(n)].a, d + 1);
+    walk(nodes[size_t(n)].b, d + 1);
+  };
+  walk(heap[0].second, 0);
+  const uint64_t full = 1ull << max_len;
+  auto kraft = [&]() {
+    uint64_t k = 0;
+    for (uint8_t l : len)
+      if (l) k += full >> l;
+    return k;
+  };
+  for (uint64_t k = kraft(); k != full; k = kraft()) {
+    int pick = -1;  // over-full: lengthen the longest code below max_len; short: shorten the longest code
+    for (size_t i = 0; i < len.size(); ++i)
+      if (len[i] && (k > full ? len[i] < max_len : len[i] > min_len) && (pick < 0 || len[i] > len[size_t(pick)])) pick = int(i);
+    if (pick < 0) form_fail("no complete code", 0);
+    len[size_t(pick)] = uint8_t(len[size_t(pick)] + (k > full ? 1 : -1));
+  }
+  return len;
+}
+
+// Canonical (Brotli) codes of `len`, bit-reversed because the stream is read LSB first.
+std::vector<uint32_t> canonical_codes(const std::vector<uint8_t>& len) {
+  uint32_t count[17] = {}, next[17] = {};
+  for (uint8_t l : len)
+    if (l) ++count[l];
+  for (uint32_t l = 1, code = 0; l <= 16; ++l) next[l] = code = (code + count[l - 1]) << 1;
+  std::vector<uint32_t> out(len.size(), 0);
+  for (size_t s = 0; s < len.size(); ++s) {
+    if (!len[s]) continue;
+    const uint32_t c = next[len[s]]++;
+    for (uint32_t i = 0; i < len[s]; ++i) out[s] |= ((c >> i) & 1) << (len[s] - 1 - i);
+  }
+  return out;
+}
+
+// ans.rs:180-254: the alias table of `dist`, packed as parse_entropy_code packs it (pack_ans_bucket).
+std::vector<uint64_t> alias_table(const std::vector<uint32_t>& dist, uint32_t log_alpha, uint32_t alphabet_size) {
+  const uint32_t table_size = 1u << log_alpha, bucket_size = 1u << (12 - log_alpha);
+  std::vector<uint64_t> out;
+  for (uint32_t s = 0; s < table_size; ++s)
+    if (dist[s] == 4096) {
+      for (uint32_t i = 0; i < table_size; ++i) out.push_back(pack_ans_bucket(s, 0, dist[i], bucket_size * i, dist[i] ^ 4096));
+      return out;
+    }
+  struct B {
+    uint32_t dist, sym, offset, cutoff;
+  };
+  std::vector<B> b(table_size);
+  std::vector<uint32_t> under, over;
+  for (uint32_t i = 0; i < table_size; ++i) {
+    b[i] = {dist[i], i < alphabet_size ? i : 0, 0, dist[i]};
+    if (dist[i] < bucket_size) under.push_back(i);
+    else if (dist[i] > bucket_size) over.push_back(i);
+  }
+  while (!over.empty() && !under.empty()) {
+    const uint32_t o = over.back(), u = under.back();
+    over.pop_back(), under.pop_back();
+    b[o].cutoff -= bucket_size - b[u].cutoff;
+    b[u].sym = o;
+    b[u].offset = b[o].cutoff;
+    if (b[o].cutoff < bucket_size) under.push_back(o);
+    else if (b[o].cutoff > bucket_size) over.push_back(o);
+  }
+  for (uint32_t i = 0; i < table_size; ++i)
+    out.push_back(b[i].cutoff == bucket_size ? pack_ans_bucket(i, 0, b[i].dist, 0, 0)
+                                             : pack_ans_bucket(b[i].sym, b[i].cutoff, b[i].dist, b[i].offset - b[i].cutoff,
+                                                               b[i].dist ^ b[b[i].sym].dist));
+  return out;
+}
+
+void write_shift(BitWriter& w, uint32_t shift) {  // inverse of ans.rs:87-95
+  uint32_t len = 0;
+  while (len < 3 && (1u << (len + 1)) - 1 <= shift) ++len;
+  for (uint32_t i = 0; i < len; ++i) w.write(1, 1);
+  if (len < 3) w.write(1, 0);
+  w.write(int(len), shift + 1 - (1u << len));
+}
+
+// Counts (summing to 4096) in the general form with `shift`: each count but the omitted one (the first of the largest
+// logcount) rounded down to what the shift can represent, the omitted one taking the rest. Writes the histogram.
+std::vector<uint32_t> write_general(BitWriter& w, std::vector<uint32_t> c, uint32_t shift, bool rle) {
+  c.resize(std::max<size_t>(c.size(), 3), 0);
+  auto logc = [](uint32_t v) { return v ? 32 - uint32_t(__builtin_clz(v)) : 0u; };
+  uint32_t omit = 0;
+  for (uint32_t i = 0; i < c.size(); ++i)
+    if (logc(c[i]) > logc(c[omit])) omit = i;
+  uint32_t sum = 0;
+  for (uint32_t i = 0; i < c.size(); ++i) {
+    if (i == omit || c[i] <= 1) {
+      sum += i == omit ? 0 : c[i];
+      continue;
+    }
+    const int zeros = int(logc(c[i])) - 1, bitcount = std::min(std::max(int(shift) - ((12 - zeros) >> 1), 0), zeros);
+    c[i] &= ~((1u << (zeros - bitcount)) - 1);
+    sum += c[i];
+  }
+  c[omit] = 4096 - sum;
+  w.write(1, 0);
+  w.write(1, 0);
+  write_shift(w, shift);
+  write_u8(w, uint32_t(c.size()) - 3);
+  // logcounts; with `rle`, runs of four or more counts equal to the one before as logcount 13 and a repeat count
+  // (ans.rs:107-116, 138-155: not right after the omitted count, whose place repeats as 0, nor over it)
+  std::vector<bool> repeated(c.size(), false);
+  for (uint32_t i = 0; i < c.size();) {
+    uint32_t r = 0;
+    if (rle && i > 0 && i - 1 != omit)
+      while (i + r < c.size() && i + r != omit && c[i + r] == c[i - 1]) ++r;
+    if (r >= 4) {
+      write_logcount(w, 13);
+      write_u8(w, std::min<uint32_t>(r, 259) - 4);
+      for (uint32_t k = i; k < i + std::min<uint32_t>(r, 259); ++k) repeated[k] = true;
+      i += std::min<uint32_t>(r, 259);
+      ++g_report.ans_forms[4];
+      continue;
+    }
+    write_logcount(w, logc(c[i]));
+    ++i;
+  }
+  for (uint32_t i = 0; i < c.size(); ++i) {
+    if (repeated[i] || i == omit || c[i] <= 1) continue;
+    const int zeros = int(logc(c[i])) - 1, bitcount = std::min(std::max(int(shift) - ((12 - zeros) >> 1), 0), zeros);
+    w.write(bitcount, (c[i] - (1u << zeros)) >> (zeros - bitcount));
+  }
+  return c;
+}
+
 // Writes the entropy-code header for `tokens` (clustered by `cluster_of_ctx`) and then the ANS
 // stream itself (32-bit initial state first). With `lz` set the code has LZ77 enabled: the symbols then hold
 // literals, length tokens (min_symbol and up) and distances, and the last context of the map is the distance context.
@@ -256,10 +481,423 @@ struct EntropyEncoder {
   std::vector<std::vector<uint32_t>> counts;     // per cluster, normalised
   std::vector<std::vector<std::vector<uint16_t>>> inv;  // cluster -> symbol -> offset -> idx
   const Lz77Header* lz = nullptr;
+  // --code only: per-cluster hybrid-uint configs, and the prefix code (lengths and bit-reversed codes) of each cluster
+  std::vector<UintConfig> cfg;
+  std::vector<std::vector<uint8_t>> plen;
+  std::vector<std::vector<uint32_t>> pcode;
+  std::vector<int32_t> psingle;  // the symbol of a 0-bit prefix code, -1 otherwise
+  bool broken = false;           // --corrupt made this code invalid: its streams are not written
 
+  std::vector<Sym> syms_of(const std::vector<Token>& tokens) const {
+    if (cfg.empty()) return to_syms(tokens);
+    std::vector<Sym> s(tokens.size());
+    for (size_t i = 0; i < tokens.size(); ++i) {
+      s[i].ctx = tokens[i].ctx;
+      tokenize_with(cfg[cluster_of_ctx[tokens[i].ctx]], tokens[i].value, &s[i].tok, &s[i].nbits, &s[i].bits);
+    }
+    return s;
+  }
   void write_header(BitWriter& w, const std::vector<Token>& tokens, uint32_t num_ctx_, const std::vector<uint8_t>& map) {
+    if (!g_code.empty() && g_code != "lz77" && !lz) return write_header_form(w, tokens, num_ctx_, map);
     write_header_syms(w, to_syms(tokens), num_ctx_, map);
   }
+
+  // --code: the cluster map, the configs and the tokens are chosen here (see the comment above g_code).
+  void write_header_form(BitWriter& w, const std::vector<Token>& tokens, uint32_t num_ctx_, std::vector<uint8_t> map) {
+    const std::string& f = g_code;
+    num_ctx = num_ctx_;
+    const uint32_t turn = g_code_turn++;
+    BitWriter hw;
+    hw.write(1, 0);  // no LZ77
+    // ---- cluster map ----
+    bool simple_map = true, mtf = false;
+    uint32_t nbits = 0;
+    if (f == "clusters" && num_ctx > 1) {
+      uint32_t K;
+      if (num_ctx >= 65) {
+        static uint32_t complex_maps = 0;  // K and move-to-front in turn
+        const uint32_t ks[3] = {65, 256, 131};
+        K = std::min(ks[complex_maps % 3], num_ctx);
+        simple_map = false;
+        mtf = complex_maps++ % 2;
+      } else {
+        static uint32_t simple_maps = 0;  // nbits 0..3 in turn, starting from the frame's seed
+        nbits = (simple_maps++ + g_code_seed) % 4;
+        K = std::min(1u << nbits, num_ctx);
+      }
+      map.resize(num_ctx);
+      for (uint32_t i = 0; i < num_ctx; ++i) map[i] = uint8_t(i % K);
+    } else if (num_ctx > 1) {
+      uint32_t n = 0;
+      for (uint8_t c : map) n = std::max<uint32_t>(n, c + 1u);
+      if (n > 8) simple_map = false;
+      else nbits = n <= 1 ? 0 : ceil_log2_nonzero(n);
+    }
+    cluster_of_ctx = map;
+    num_clusters = 0;
+    for (uint8_t c : map) num_clusters = std::max<uint32_t>(num_clusters, c + 1u);
+    if (num_ctx > 1) {
+      if (simple_map) {
+        hw.write(1, 1);
+        hw.write(2, nbits);
+        for (uint32_t i = 0; i < num_ctx; ++i) hw.write(int(nbits), map[i]);
+        g_report.map_nbits |= 1u << nbits;
+      } else {
+        hw.write(1, 0);
+        hw.write(1, mtf ? 1 : 0);
+        std::vector<Token> mt;
+        uint8_t order[256];
+        for (int i = 0; i < 256; ++i) order[i] = uint8_t(i);
+        for (uint32_t i = 0; i < num_ctx; ++i) {
+          uint32_t v = map[i];
+          if (mtf) {  // lib.rs:714-725 inverted: the position of the cluster in the list, which then moves to the front
+            uint32_t k = 0;
+            while (order[k] != map[i]) ++k;
+            std::memmove(order + 1, order, k);
+            order[0] = map[i];
+            v = k;
+          }
+          mt.push_back({0, v});
+        }
+        EntropyEncoder nested;
+        nested.write_header(hw, mt, 1, std::vector<uint8_t>(1, 0));
+        nested.write_tokens(hw, mt);
+        g_report.map_mtf |= 1u << (mtf ? 1 : 0);
+      }
+    }
+    // ---- configs and tokens ----
+    const bool prefix = f == "prefix";
+    cfg.assign(num_clusters, UintConfig{kSplitExp, kMsb, kLsb});
+    if (f == "ans-forms") log_alpha = 6 + turn % 3;
+    else log_alpha = 8;
+    if (f == "configs") {
+      std::vector<uint32_t> maxv(num_clusters, 0);
+      for (const Token& t : tokens) maxv[map[t.ctx]] = std::max(maxv[map[t.ctx]], t.value);
+      const uint32_t ncfg = sizeof(kFormConfigs) / sizeof(kFormConfigs[0]);
+      for (uint32_t c = 0; c < num_clusters; ++c)
+        for (uint32_t k = 0; k < ncfg; ++k) {
+          const uint32_t i = (g_code_turn + k) % ncfg;
+          uint32_t tok, nb, bits;
+          tokenize_with(kFormConfigs[i], maxv[c], &tok, &nb, &bits);
+          if (tok < (1u << log_alpha)) {
+            cfg[c] = kFormConfigs[i];
+            g_report.configs |= 1u << i;
+            ++g_code_turn;
+            break;
+          }
+        }
+    }
+    const std::vector<Sym> syms = syms_of(tokens);
+    std::vector<std::vector<uint64_t>> freq(num_clusters);
+    for (const Sym& s : syms) {
+      auto& fr = freq[map[s.ctx]];
+      if (fr.size() <= s.tok) fr.resize(s.tok + 1, 0);
+      ++fr[s.tok];
+    }
+    for (uint32_t c = 0; c < num_clusters; ++c)
+      if (!prefix && freq[c].size() > (1u << log_alpha)) form_fail("token alphabet too large", c);
+    hw.write(1, prefix ? 1 : 0);
+    if (!prefix) hw.write(2, log_alpha - 5);
+    const uint32_t la = prefix ? 15 : log_alpha;
+    for (uint32_t c = 0; c < num_clusters; ++c) {  // lib.rs:378-412
+      hw.write(int(add_log2_ceil(la)), cfg[c].split_exp);
+      if (cfg[c].split_exp != la) {
+        hw.write(int(add_log2_ceil(cfg[c].split_exp)), cfg[c].msb);
+        hw.write(int(add_log2_ceil(cfg[c].split_exp - cfg[c].msb)), cfg[c].lsb);
+      }
+    }
+    std::vector<std::vector<uint64_t>> tables;  // ANS: the alias table of each cluster
+    if (prefix) write_prefix_codes(hw, freq);
+    else tables = write_ans_codes(hw, freq, f == "ans-forms");
+    // ---- read back with the product's parser; everything must be what was written ----
+    const size_t written_bits = hw.total_bits;
+    hw.pad();
+    if (g_corrupt_done && (g_corrupt == "oversub-clcl" || g_corrupt == "oversub-lengths" || g_corrupt == "ans-sum") &&
+        !g_report.rejected_by_parser) {
+      try {
+        BitReader br(hw.bytes.data(), hw.bytes.size());
+        parse_entropy_code(br, num_ctx);
+      } catch (const Error&) {
+        ++g_report.rejected_by_parser;
+      }
+      BitReader cp(hw.bytes.data(), hw.bytes.size());
+      for (size_t b = written_bits; b;) {
+        const uint32_t n = uint32_t(std::min<size_t>(b, 32));
+        w.write(int(n), cp.read(n));
+        b -= n;
+      }
+      broken = true;  // the streams that follow are never read
+      return;
+    }
+    BitReader br(hw.bytes.data(), hw.bytes.size());
+    EntropyCode code = parse_entropy_code(br, num_ctx);
+    if (code.num_clusters != num_clusters || code.cluster_map != map || code.use_prefix != prefix ||
+        (!prefix && code.log_alphabet_size != log_alpha))
+      form_fail("cluster map or code kind read back differently", 0);
+    for (uint32_t c = 0; c < num_clusters; ++c) {
+      const HybridUintConfig& h = code.configs[c];
+      if (h.split_exponent != cfg[c].split_exp || h.msb_in_token != cfg[c].msb || h.lsb_in_token != cfg[c].lsb)
+        form_fail("hybrid-uint config read back differently", c);
+      if (prefix) check_prefix_table(code, c);
+      else
+        for (size_t i = 0; i < tables[c].size(); ++i)
+          if (code.ans_table[(size_t(c) << log_alpha) + i] != tables[c][i]) form_fail("ANS alias table differs", c);
+    }
+    if (!prefix) build_inverse(tables);
+    ++g_report.codes;
+    g_report.max_clusters = std::max(g_report.max_clusters, num_clusters);
+    if (!prefix) {
+      g_report.log_alphas |= 1u << log_alpha;
+      g_report.max_ans_table_bytes = std::max(g_report.max_ans_table_bytes, (num_clusters << log_alpha) * 8);
+    }
+    size_t hbits = br.pos();
+    BitReader cp(hw.bytes.data(), hw.bytes.size());
+    for (; hbits;) {
+      const uint32_t n = uint32_t(std::min<size_t>(hbits, 32));
+      w.write(int(n), cp.read(n));
+      hbits -= n;
+    }
+  }
+
+  // lib.rs:433-452 and prefix.rs: the alphabet size of each cluster, then its code.
+  void write_prefix_codes(BitWriter& hw, const std::vector<std::vector<uint64_t>>& freq) {
+    ++g_report.prefix_codes;
+    plen.assign(num_clusters, {});
+    pcode.assign(num_clusters, {});
+    psingle.assign(num_clusters, -1);
+    uint32_t deep = 0, deep_n = 0;  // the cluster with the most symbols gets the chain-shaped code
+    for (uint32_t c = 0; c < num_clusters; ++c) {
+      uint32_t n = 0;
+      for (uint64_t x : freq[c]) n += x != 0;
+      if (n > deep_n) deep = c, deep_n = n;
+    }
+    for (uint32_t c = 0; c < num_clusters; ++c) {
+      const uint32_t count = std::max<uint32_t>(1, uint32_t(freq[c].size()));
+      if (count == 1) {
+        hw.write(1, 0);
+      } else {
+        hw.write(1, 1);
+        const uint32_t n = 31 - uint32_t(__builtin_clz(count - 1));
+        hw.write(4, n);
+        hw.write(int(n), count - 1 - (1u << n));
+      }
+    }
+    for (uint32_t c = 0; c < num_clusters; ++c) {
+      ++g_report.prefix_clusters;
+      const uint32_t count = std::max<uint32_t>(1, uint32_t(freq[c].size()));
+      std::vector<uint32_t> used;  // by falling frequency
+      for (uint32_t s = 0; s < freq[c].size(); ++s)
+        if (freq[c][s]) used.push_back(s);
+      std::stable_sort(used.begin(), used.end(), [&](uint32_t a, uint32_t b) { return freq[c][a] > freq[c][b]; });
+      std::vector<uint8_t>& len = plen[c];
+      len.assign(count, 0);
+      if (used.size() <= 1) {  // 0 bits per symbol
+        ++g_report.single_symbol;
+        psingle[c] = used.empty() ? 0 : int32_t(used[0]);
+        if (count > 1) {
+          hw.write(2, 1), hw.write(2, 0), hw.write(int(ceil_log2_nonzero(count)), used[0]);
+          ++g_report.nsym[1];
+        }
+        pcode[c].assign(count, 0);
+        continue;
+      }
+      if (used.size() <= 4) {  // prefix.rs:149-207
+        const uint32_t abits = ceil_log2_nonzero(count), n = uint32_t(used.size());
+        hw.write(2, 1);
+        hw.write(2, n - 1);
+        bool tree_select = false;
+        if (n == 4) tree_select = (g_code_turn++ % 2) == 1, ++g_report.tree_select[tree_select];
+        const uint8_t lens[5][4] = {{}, {}, {1, 1}, {1, 2, 2}, {2, 2, 2, 2}};
+        for (uint32_t i = 0; i < n; ++i) {
+          hw.write(int(abits), used[i]);
+          len[used[i]] = tree_select ? uint8_t(std::min<uint32_t>(i + 1, 3)) : lens[n][i];
+        }
+        if (n == 4) hw.write(1, tree_select);
+        ++g_report.nsym[n];
+      } else {
+        // hskip 2 and 3 leave out the code-length symbols 1, 2 (and 3): codes of at least 3 (4) bits where they fit
+        const uint32_t kSkips[3] = {0, 2, 3};
+        const bool chain = c == deep && used.size() >= 16;
+        const uint32_t hskip = chain ? 0 : kSkips[g_code_turn++ % 3];
+        const uint32_t min_len = hskip == 3 && used.size() >= 16 ? 4 : hskip && used.size() >= 8 ? 3 : 1;
+        std::vector<double> wt(count, 0.0);
+        for (uint32_t i = 0; i < used.size(); ++i) wt[used[i]] = chain ? std::ldexp(1.0, -int(i)) : double(freq[c][used[i]]);
+        len = limited_lengths(wt, 15, min_len);
+        write_complex(hw, len, hskip);
+      }
+      pcode[c] = canonical_codes(len);
+      for (uint8_t l : len) {
+        g_report.max_prefix_len = std::max<uint32_t>(g_report.max_prefix_len, l);
+        g_report.long_codes += l > kPrefixRootBits;
+      }
+    }
+  }
+
+  // prefix.rs:209-332: the code-length code, then the code lengths with repeat codes 16 and 17.
+  void write_complex(BitWriter& hw, const std::vector<uint8_t>& len, uint32_t hskip) {
+    struct Item {
+      uint32_t sym, nbits, bits;
+    };
+    std::vector<Item> items;
+    size_t last = len.size();
+    while (last > 0 && !len[last - 1]) --last;
+    uint32_t last_nz = 8, prev = 0xff;
+    for (size_t i = 0; i < last;) {
+      size_t r = 0;
+      while (i + r < last && len[i + r] == len[i]) ++r;
+      if (len[i] == 0 && r >= 3 && prev != 17) {
+        const uint32_t k = uint32_t(std::min<size_t>(r, 10));
+        items.push_back({17, 3, k - 3}), prev = 17, i += k;
+        ++g_report.repeat17;
+      } else if (len[i] != 0 && len[i] == last_nz && r >= 3 && prev != 16) {
+        const uint32_t k = uint32_t(std::min<size_t>(r, 6));
+        items.push_back({16, 2, k - 3}), prev = 16, i += k;
+        ++g_report.repeat16;
+      } else {
+        items.push_back({len[i], 0, 0}), prev = len[i];
+        if (len[i]) last_nz = len[i];
+        ++i;
+      }
+    }
+    if (g_corrupt == "oversub-lengths" && !g_corrupt_done && items.back().sym >= 2 && items.back().sym <= 15)
+      --items.back().sym, g_corrupt_done = true;
+    std::vector<double> cf(18, 0.0);
+    for (const Item& it : items) cf[it.sym] += 1.0;
+    std::vector<uint8_t> cl = limited_lengths(cf, 5);
+    uint32_t nz = 0;
+    for (uint8_t l : cl) nz += l != 0;
+    static const uint32_t kOrder[18] = {1, 2, 3, 4, 0, 5, 17, 6, 16, 7, 8, 9, 10, 11, 12, 13, 14, 15};
+    while (hskip && (cl[1] || cl[2] || (hskip == 3 && cl[3]))) hskip = hskip == 3 ? 2 : 0;
+    ++g_report.hskip[hskip];
+    hw.write(2, hskip);
+    uint32_t acc = 0, last_k = 0;
+    for (uint32_t k = hskip; k < 18 && (nz == 1 || acc < 32); ++k) {
+      if (cl[kOrder[k]]) acc += 32u >> cl[kOrder[k]], last_k = k;
+    }
+    const bool bad_clcl = g_corrupt == "oversub-clcl" && !g_corrupt_done && nz > 1 && cl[kOrder[last_k]] >= 2;
+    if (bad_clcl) g_corrupt_done = true;
+    acc = 0;
+    for (uint32_t k = hskip; k < 18 && (nz == 1 || acc < 32); ++k) {
+      const uint32_t l = cl[kOrder[k]] - (bad_clcl && k == last_k ? 1 : 0);
+      if (l == 0) hw.write(2, 0);
+      else if (l == 4) hw.write(2, 1);
+      else if (l == 3) hw.write(2, 2);
+      else if (l == 2) hw.write(2, 3), hw.write(1, 0);
+      else if (l == 1) hw.write(2, 3), hw.write(1, 1), hw.write(1, 0);
+      else hw.write(2, 3), hw.write(1, 1), hw.write(1, 1);
+      if (l) acc += 32u >> l;
+      if (bad_clcl && k == last_k) return;  // the parser stops here
+    }
+    const std::vector<uint32_t> cc = canonical_codes(cl);
+    for (const Item& it : items) {
+      if (nz > 1) hw.write(cl[it.sym], cc[it.sym]);
+      if (it.nbits) hw.write(int(it.nbits), it.bits);
+    }
+  }
+
+  // Every symbol's code looked up in the parser's table (entropy.h: kPrefixNested, kPrefixRootBits) gives it back.
+  void check_prefix_table(const EntropyCode& code, uint32_t c) const {
+    const PrefixMeta& m = code.prefix_meta[c];
+    const uint32_t* t = code.prefix_table.data() + m.table_offset;
+    uint32_t nused = 0;
+    for (uint32_t s = 0; s < plen[c].size(); ++s) {
+      if (!plen[c][s]) continue;
+      ++nused;
+      uint32_t e = t[pcode[c][s] & ((1u << m.root_bits) - 1)];
+      if (e & kPrefixNested) {
+        if (m.root_bits != kPrefixRootBits) form_fail("nested entry below the root bits", c);
+        const uint32_t sb = (e >> 16) & 0xff;
+        e = t[(1u << m.root_bits) + (e & 0xffff) + ((pcode[c][s] >> m.root_bits) & ((1u << sb) - 1))];
+      }
+      if ((e & 0xffff) != s || ((e >> 16) & 0xff) != plen[c][s]) form_fail("prefix code read back differently", c);
+    }
+    if (nused == 0 && code.single_symbol[c] != psingle[c]) form_fail("single-symbol prefix code read back differently", c);
+  }
+
+  // ANS histograms (ans.rs:31-178) in the form chosen for each cluster; returns each cluster's alias table.
+  std::vector<std::vector<uint64_t>> write_ans_codes(BitWriter& hw, const std::vector<std::vector<uint64_t>>& freq,
+                                                     bool forms) {
+    std::vector<std::vector<uint64_t>> tables;
+    counts.clear();
+    for (uint32_t c = 0; c < num_clusters; ++c) {
+      std::vector<uint64_t> fr = freq[c].empty() ? std::vector<uint64_t>(1, 0) : freq[c];
+      std::vector<uint32_t> used;
+      for (uint32_t s = 0; s < fr.size(); ++s)
+        if (fr[s]) used.push_back(s);
+      std::vector<uint32_t> dist(size_t(1) << log_alpha, 0);
+      uint32_t alphabet;  // the alphabet size the histogram declares (ans.rs:46-102)
+      if (g_corrupt == "ans-sum" && !g_corrupt_done) {  // counts 2048 (omitted), 4095, 4095: explicit ones sum to 8190
+        g_corrupt_done = true;
+        hw.write(1, 0), hw.write(1, 0), write_shift(hw, 13), write_u8(hw, 0);
+        for (int i = 0; i < 3; ++i) write_logcount(hw, 12);
+        hw.write(11, 2047), hw.write(11, 2047);
+        counts.push_back(dist);
+        tables.push_back({});
+        continue;
+      }
+      if (used.size() > 2 || (!forms && used.size() == 2)) {
+        const uint32_t kind = forms ? g_code_turn++ % 4 : 3;  // 0 flat, 1 rle, 2-3 general
+        std::vector<uint32_t> nc = normalize(fr);
+        if (kind == 0) {  // evenly distributed over [0, last]
+          const uint32_t n = uint32_t(fr.size());
+          hw.write(1, 0), hw.write(1, 1), write_u8(hw, n - 1);
+          for (uint32_t i = 0; i < n; ++i) nc[i] = 4096 / n + (i < 4096 % n ? 1 : 0);
+          ++g_report.ans_forms[2];
+        } else if (kind == 1) {  // equal counts, the rest on symbol 0
+          const uint32_t n = uint32_t(fr.size()), base = std::max<uint32_t>(1, 2048 / n);
+          for (uint32_t i = 0; i < n; ++i) nc[i] = base;
+          nc[0] = 4096 - (n - 1) * base;
+          nc = write_general(hw, nc, 13, true);
+        } else {
+          const uint32_t shift = forms ? g_report.ans_forms[3] % 14 : 13;
+          nc = write_general(hw, nc, shift, false);
+          g_report.shifts |= 1u << shift;
+          ++g_report.ans_forms[3];
+        }
+        for (uint32_t i = 0; i < nc.size(); ++i) dist[i] = nc[i];
+        alphabet = kind == 0 ? uint32_t(fr.size()) : uint32_t(nc.size());
+      } else if (used.size() == 2) {
+        std::vector<uint32_t> nc = normalize(fr);
+        hw.write(1, 1), hw.write(1, 1);
+        write_u8(hw, used[0]), write_u8(hw, used[1]);
+        hw.write(12, nc[used[0]]);
+        dist[used[0]] = nc[used[0]], dist[used[1]] = 4096 - nc[used[0]];
+        alphabet = used[1] + 1;
+        ++g_report.ans_forms[1];
+      } else {
+        const uint32_t s = used.empty() ? 0 : used[0];
+        hw.write(1, 1), hw.write(1, 0), write_u8(hw, s);
+        dist[s] = 4096;
+        alphabet = s + 1;
+        ++g_report.ans_forms[0];
+      }
+      for (uint32_t s : used)
+        if (!dist[s]) form_fail("a used symbol has no probability", c);
+      counts.push_back(dist);
+      tables.push_back(alias_table(dist, log_alpha, alphabet));
+    }
+    return tables;
+  }
+
+  // The encoder's inverse of the alias tables: symbol and offset -> table index (ans.rs:264-290, read_symbol).
+  void build_inverse(const std::vector<std::vector<uint64_t>>& tables) {
+    inv.assign(num_clusters, {});
+    const uint32_t log_bucket = 12 - log_alpha;
+    for (uint32_t c = 0; c < num_clusters; ++c) {
+      inv[c].resize(size_t(1) << log_alpha);
+      for (size_t s = 0; s < counts[c].size(); ++s) inv[c][s].assign(counts[c][s], 0xffff);
+      for (uint32_t idx = 0; idx < 4096; ++idx) {
+        const uint32_t i = idx >> log_bucket, pos = idx & ((1u << log_bucket) - 1);
+        const uint64_t b = tables[c][i];
+        const uint32_t alias_symbol = uint32_t(b & 0xff), cutoff = uint32_t((b >> 8) & 0xff);
+        const bool alias = pos >= cutoff;
+        const uint32_t offset = (alias ? uint32_t((b >> 32) & 0xffff) : 0) + pos, sym = alias ? alias_symbol : i;
+        if (sym >= inv[c].size() || offset >= inv[c][sym].size()) form_fail("alias table inconsistent", c);
+        inv[c][sym][offset] = uint16_t(idx);
+      }
+    }
+  }
+
   // `num_ctx_` counts the distance context of an LZ77 code.
   void write_header_syms(BitWriter& w, const std::vector<Sym>& syms, uint32_t num_ctx_, const std::vector<uint8_t>& map) {
     num_ctx = num_ctx_;
@@ -355,8 +993,17 @@ struct EntropyEncoder {
     }
   }
 
-  void write_tokens(BitWriter& w, const std::vector<Token>& tokens) const { write_syms(w, to_syms(tokens)); }
+  void write_tokens(BitWriter& w, const std::vector<Token>& tokens) const { write_syms(w, syms_of(tokens)); }
   void write_syms(BitWriter& w, const std::vector<Sym>& syms) const {
+    if (broken) return;
+    if (!plen.empty()) {  // prefix codes: no state, each symbol's code and then its extra bits
+      for (const Sym& s : syms) {
+        const uint32_t c = cluster_of_ctx[s.ctx];
+        if (plen[c][s.tok]) w.write(plen[c][s.tok], pcode[c][s.tok]);
+        if (s.nbits) w.write(int(s.nbits), s.bits);
+      }
+      return;
+    }
     struct Out {
       uint16_t ans_bits;
       uint8_t has_ans;
@@ -364,7 +1011,7 @@ struct EntropyEncoder {
       uint32_t bits;
     };
     std::vector<Out> outs(syms.size());
-    uint32_t state = 0x130000;
+    uint32_t state = g_flip_state ? 0x130001 : 0x130000;  // ans-state: every value decodes, the end state is wrong
     for (size_t k = syms.size(); k-- > 0;) {
       const uint32_t tok = syms[k].tok;
       uint32_t c = cluster_of_ctx[syms[k].ctx];
@@ -381,6 +1028,7 @@ struct EntropyEncoder {
       state = ((state / f) << 12) + inv[c][tok][state % f];
     }
     w.write(32, state);
+    g_flip_state = false;
     for (const Out& o : outs) {
       if (o.has_ans) w.write(16, o.ans_bits);
       if (o.nbits) w.write(o.nbits, o.bits);
@@ -400,21 +1048,35 @@ struct EntropyEncoder {
 //          pending when the stream ends is ignored).
 //   bad-first / bad-length: `match`, with group 0's stream made invalid -- it starts with a copy, or its first copy has
 //          a length whose value plus min_length does not fit 32 bits.
+//   modular (--code lz77): `match` over a Modular stream, with the U32 selectors of min_symbol (224 or 8 + u(15) = 128)
+//          and min_length (3, 4, 5 + u(2) = 6, 9 + u(8) = 10) taken from `sel`. The decoder scales the special distance
+//          codes 0..119 by the stream's widest channel (image.rs:460, lib.rs:530-545): a copy from dy rows up and dx
+//          columns over is written with such a code where one fits, any other distance as 120 + distance - 1.
+//          Matches stay within the 2^20-value window; copies run across channel boundaries, and none is pending at
+//          the end of the stream.
 struct HfLz77 {
   std::string mode;  // empty: no LZ77
+  uint32_t sel = 0;  // modular: min_length selector in bits 0-1, min_symbol 8 + u(15) in bit 2
   Lz77Header header() const {
     if (mode == "rle") return {224, 3, 0, 0, {0, 0, 0}};
+    if (mode == "modular") {
+      const uint32_t len_min[4] = {3, 4, 6, 10};
+      if (sel & 4) return {128, len_min[sel & 3], 3, int(sel & 3), {kSplitExp, kMsb, kLsb}};
+      return {224, len_min[sel & 3], 0, int(sel & 3), {0, 0, 0}};
+    }
     return {128, 4, 3, 1, {kSplitExp, kMsb, kLsb}};
   }
 };
 struct Lz77Counts {
   uint64_t copied = 0, from_start = 0;
+  uint64_t special = 0, far = 0, cross_channel = 0, past_window = 0;  // modular: copies of each kind
 };
 
+// `mult`: the stream's distance multiplier (0 in HF streams); `chan_start`: where each channel's values begin.
 std::vector<Sym> lz77_parse(const std::vector<Token>& toks, const HfLz77& opt, uint32_t dist_ctx, bool corrupt,
-                            Lz77Counts* counts) {
+                            Lz77Counts* counts, uint32_t mult = 0, const std::vector<size_t>& chan_start = {}) {
   const Lz77Header h = opt.header();
-  const size_t n = toks.size();
+  const size_t n = toks.size(), kWindow = size_t(1) << 20;
   struct Item {
     size_t pos;
     bool copy;
@@ -455,20 +1117,42 @@ std::vector<Sym> lz77_parse(const std::vector<Token>& toks, const HfLz77& opt, u
       while (i + l < n && l < 65536 && v(j + l) == v(i + l)) ++l;
       return l;
     };
+    auto special = [&](size_t dist) {  // the special distance code of `dist`, or -1
+      for (int k = 0; k < 120; ++k)
+        if (int64_t(kLz77SpecialDistances[k][0]) + int64_t(mult) * kLz77SpecialDistances[k][1] == int64_t(dist)) return k;
+      return -1;
+    };
+    auto chan_of = [&](size_t i) { return std::upper_bound(chan_start.begin(), chan_start.end(), i) - chan_start.begin(); };
     for (size_t i = 0; i < n;) {
       size_t best = 0, best_j = 0;
       if (i > 0 && i + 4 <= n) {
+        if (mult)
+          for (int k = 0; k < 120; ++k) {
+            const int64_t dd = int64_t(kLz77SpecialDistances[k][0]) + int64_t(mult) * kLz77SpecialDistances[k][1];
+            if (dd < 1 || dd > int64_t(i)) continue;
+            const size_t l = match_len(i - size_t(dd), i);
+            if (l > best) best = l, best_j = i - size_t(dd);
+          }
         int tries = 0;
         for (int32_t j = head[hash(i)]; j >= 0 && tries < 32; j = prev[size_t(j)], ++tries) {
+          if (i - size_t(j) > kWindow) break;
           const size_t l = match_len(size_t(j), i);
           if (l > best) best = l, best_j = size_t(j);
         }
-        const size_t l0 = match_len(0, i);  // ties go to the stream's first value
+        const size_t l0 = i < kWindow ? match_len(0, i) : 0;  // ties go to the stream's first value
         if (l0 >= best && l0 > 0) best = l0, best_j = 0;
       }
       if (best >= h.min_length) {
         uint32_t d = uint32_t(i - best_j - 1);
+        const int k = mult && best_j ? special(i - best_j) : -1;
         if (best_j == 0) d = (from_start++ & 1) ? uint32_t(i) + 1000 : (1u << 20) + 17;  // clamped to i by the decoder
+        if (mult) {
+          d = k >= 0 ? uint32_t(k) : d + 120;
+          counts->special += k >= 0;
+          counts->far += k < 0;
+          counts->past_window += i >= kWindow;
+          if (!chan_start.empty()) counts->cross_channel += chan_of(best_j) != chan_of(i) || chan_of(i + best - 1) != chan_of(i);
+        }
         items.push_back({i, true, uint32_t(best - h.min_length), d});
         copied += best;
         for (size_t k = i; k < i + best; ++k) insert(k);
@@ -480,7 +1164,8 @@ std::vector<Sym> lz77_parse(const std::vector<Token>& toks, const HfLz77& opt, u
       }
     }
     // the last copy runs past the end of the stream
-    if (!items.empty() && items.back().copy) {
+    if (mult) {
+    } else if (!items.empty() && items.back().copy) {
       items.back().len_value += 5;
     } else if (n >= 2) {
       for (size_t j = n - 1; j-- > 0;)
@@ -499,6 +1184,7 @@ std::vector<Sym> lz77_parse(const std::vector<Token>& toks, const HfLz77& opt, u
     Sym s{toks[it.pos].ctx, 0, 0, 0};
     if (!it.copy) {
       tokenize(v(it.pos), &s.tok, &s.nbits, &s.bits);
+      if (s.tok >= h.min_symbol) fprintf(stderr, "a literal token reaches min_symbol\n"), exit(1);
       out.push_back(s);
       continue;
     }
@@ -1274,9 +1960,39 @@ int write_modular_frame(const Args& a, const std::vector<MChan>& ch, uint32_t cw
     modular_tokens(tree, pg_streams[g], int32_t(1 + 3 * num_lf + 17 + g), &pg_tokens[g]);
     all.insert(all.end(), pg_tokens[g].begin(), pg_tokens[g].end());
   }
+  // ---- --code lz77: each stream's values parsed into literals and copies (HfLz77 "modular") ----
+  const bool lz77 = g_code == "lz77";
+  HfLz77 lzopt{"modular", a.seed % 8};
+  const Lz77Header lzh = lzopt.header();
+  Lz77Counts lzc;
+  std::vector<Sym> lz_global;
+  std::vector<std::vector<Sym>> lz_lf(num_lf), lz_pg(num_groups);
+  if (lz77) {
+    const uint32_t dist_ctx = uint32_t(tree.num_leaves());
+    auto parse = [&](const std::vector<Plane2D>& planes, const std::vector<Token>& toks, std::vector<Sym>* out) {
+      uint32_t mult = 0;  // the widest channel of the stream
+      std::vector<size_t> starts;
+      size_t at = 0;
+      for (const Plane2D& p : planes) {
+        mult = std::max(mult, p.w);
+        starts.push_back(at);
+        at += size_t(p.w) * p.h;
+      }
+      *out = lz77_parse(toks, lzopt, dist_ctx, false, &lzc, mult, starts);
+    };
+    std::vector<Plane2D> g;
+    for (size_t i = 0; i < nglobal; ++i) g.push_back(ch[i].p);
+    parse(g, global_tokens, &lz_global);
+    for (uint32_t i = 0; i < num_lf; ++i) parse(lf_streams[i], lf_tokens[i], &lz_lf[i]);
+    for (uint32_t i = 0; i < num_groups; ++i) parse(pg_streams[i], pg_tokens[i], &lz_pg[i]);
+  }
   // ---- sections ----
   std::vector<BitWriter> sections(1 + num_lf + 1 + num_groups);
   EntropyEncoder enc;
+  auto write_stream = [&](BitWriter& w, const std::vector<Token>& toks, const std::vector<Sym>& syms) {
+    if (lz77) enc.write_syms(w, syms);
+    else enc.write_tokens(w, toks);
+  };
   {
     BitWriter& w = sections[0];
     w.write(1, 1);  // LfChannelDequantization all_default
@@ -1284,7 +2000,21 @@ int write_modular_frame(const Args& a, const std::vector<MChan>& ch, uint32_t cw
     write_tree(w, tree);
     std::vector<uint8_t> map(size_t(tree.num_leaves()));
     for (size_t i = 0; i < map.size(); ++i) map[i] = uint8_t(i);
-    enc.write_header(w, all, uint32_t(map.size()), map);
+    if (lz77) {
+      std::vector<Sym> syms = lz_global;
+      for (const auto& v : lz_lf) syms.insert(syms.end(), v.begin(), v.end());
+      for (const auto& v : lz_pg) syms.insert(syms.end(), v.begin(), v.end());
+      map.push_back(uint8_t(map.size()));  // the distance context gets a cluster of its own
+      enc.lz = &lzh;
+      enc.write_header_syms(w, syms, uint32_t(map.size()), map);
+      fprintf(stderr, "lz77-modular: min_symbol=%u min_length=%u symbol_sel=%d length_sel=%d copies_values=%llu "
+                      "special=%llu far=%llu from_start=%llu cross_channel=%llu past_window=%llu\n",
+              lzh.min_symbol, lzh.min_length, lzh.symbol_sel, lzh.length_sel, (unsigned long long)lzc.copied,
+              (unsigned long long)lzc.special, (unsigned long long)lzc.far, (unsigned long long)lzc.from_start,
+              (unsigned long long)lzc.cross_channel, (unsigned long long)lzc.past_window);
+    } else {
+      enc.write_header(w, all, uint32_t(map.size()), map);
+    }
     if (a.shifted()) {
       write_modular_header(w);
     } else {  // GlobalModular header (lib.rs:117-125): global tree, default WP, two transforms
@@ -1297,21 +2027,22 @@ int write_modular_frame(const Args& a, const std::vector<MChan>& ch, uint32_t cw
       w.write(2, 2);          // Squeeze
       write_u32(w, 0, 0, 0);  //   num_sq = 0: default parameters
     }
-    enc.write_tokens(w, global_tokens);
+    write_stream(w, global_tokens, lz_global);
     w.pad();
   }
   for (uint32_t g = 0; g < num_lf; ++g) {
     if (lf_streams[g].empty()) continue;
     BitWriter& w = sections[1 + g];
     write_modular_header(w);
-    enc.write_tokens(w, lf_tokens[g]);
+    write_stream(w, lf_tokens[g], lz_lf[g]);
     w.pad();
   }
   for (uint32_t g = 0; g < num_groups; ++g) {
     if (pg_streams[g].empty()) continue;
     BitWriter& w = sections[2 + num_lf + g];
     write_modular_header(w);
-    enc.write_tokens(w, pg_tokens[g]);
+    g_flip_state = g_corrupt == "ans-state" && g + 1 == num_groups;
+    write_stream(w, pg_tokens[g], lz_pg[g]);
     w.pad();
   }
   // ---- codestream ----
@@ -1374,6 +2105,7 @@ int write_modular_frame(const Args& a, const std::vector<MChan>& ch, uint32_t cw
   cs.pad();
   // one group: a single TOC entry; every channel fits the global stream, so LfGlobal is all there is
   if (num_groups == 1) sections.resize(1);
+  if (g_corrupt == "truncate") sections.back().bytes.resize(sections.back().bytes.size() / 2);
   for (const BitWriter& sct : sections) {
     const uint32_t sz = uint32_t(sct.bytes.size());
     if (sz < 1024) write_u32(cs, 0, 10, sz);
@@ -1419,6 +2151,8 @@ int main(int argc, char** argv) {
     else if (s == "--only-type") a.only_type = atoi(next().c_str());
     else if (s == "--dump-blocks") a.dump_blocks = next();
     else if (s == "--hf-lz77") a.hf_lz77.mode = next();
+    else if (s == "--code") g_code = next();
+    else if (s == "--corrupt") g_corrupt = next();
     else if (s == "-o") a.out = next();
     else if (s == "--ycbcr") a.ycbcr = next();
     else if (s == "--dump-coeffs") a.dump_coeffs = next();
@@ -1455,6 +2189,20 @@ int main(int argc, char** argv) {
   if (a.upsampling != 1 && !a.modular && (a.lf_frame || !a.extras.empty()))
     fprintf(stderr, "--upsampling of a VarDCT frame is not written with --lf-frame or --extra\n"), exit(2);
   if (!a.extras.empty() && a.lf_frame) fprintf(stderr, "--extra is not written with --lf-frame\n"), exit(2);
+  if (!g_code.empty() && g_code != "prefix" && g_code != "ans-forms" && g_code != "configs" && g_code != "clusters" &&
+      g_code != "lz77")
+    fprintf(stderr, "--code takes prefix, ans-forms, configs, clusters or lz77 (--modular)\n"), exit(2);
+  if (g_code == "lz77" && !a.modular) fprintf(stderr, "--code lz77 goes with --modular frames\n"), exit(2);
+  if (!g_corrupt.empty() && g_corrupt != "ans-state" && g_corrupt != "truncate" && g_corrupt != "oversub-clcl" &&
+      g_corrupt != "oversub-lengths" && g_corrupt != "ans-sum")
+    fprintf(stderr, "--corrupt takes ans-state, truncate, oversub-clcl, oversub-lengths or ans-sum\n"), exit(2);
+  if ((g_corrupt == "oversub-clcl" || g_corrupt == "oversub-lengths") && g_code != "prefix")
+    fprintf(stderr, "--corrupt %s goes with --code prefix\n", g_corrupt.c_str()), exit(2);
+  if (g_corrupt == "ans-sum" && (g_code.empty() || g_code == "prefix" || g_code == "lz77"))
+    fprintf(stderr, "--corrupt ans-sum goes with --code ans-forms, configs or clusters\n"), exit(2);
+  if (!g_code.empty() && !a.hf_lz77.mode.empty()) fprintf(stderr, "--code is not written with --hf-lz77\n"), exit(2);
+  if (!g_code.empty()) atexit([] { g_report.print(); });
+  g_code_seed = a.seed;
   if (a.modular && a.shifted()) return encode_channels(a);
   const std::string& lzm = a.hf_lz77.mode;
   if (!lzm.empty() && (a.modular || (lzm != "rle" && lzm != "match" && lzm != "bad-first" && lzm != "bad-length")))
@@ -1846,6 +2594,7 @@ int main(int argc, char** argv) {
     for (uint32_t g = 0; g < num_groups; ++g) {
       BitWriter& w = sections[2 + num_lf + size_t(pass) * num_groups + g];
       w.write(int(ceil_log2_nonzero(NP)), g % NP);  // hfp: 0 bits with a single preset
+      g_flip_state = g_corrupt == "ans-state" && pass == 0 && g == 0;
       if (a.hf_lz77.mode.empty()) hf_enc[pass].write_tokens(w, hf_tokens[size_t(pass) * num_groups + g]);
       else hf_enc[pass].write_syms(w, hf_syms[size_t(pass) * num_groups + g]);
       if (pass + 1 == P && !ex_pg_tokens[g].empty()) {  // Modular pass-group channels, after the HF data
