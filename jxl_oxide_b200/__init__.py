@@ -354,34 +354,17 @@ class Decoder:
     def frame_to_buffer(self, frame, dtype=np.uint8, orientation=0, out=None):
         """ImageStream::write_to_buffer: (height, width, channels) interleaved u8 / u16 / f32 samples with the
         orientation applied (0 = the image header's). `out`: a C-contiguous array of that shape to fill (e.g. pinned)."""
-        info = self.frame_info(frame)
-        img = self.image_info()
-        orient = orientation or img.orientation
-        w, h = (info.height, info.width) if orient >= 5 else (info.width, info.height)
-        st = {np.dtype(np.uint8): 0, np.dtype(np.uint16): 1, np.dtype(np.float32): 2}[np.dtype(dtype)]
-        shape = (h, w, self._L.jxlb_frame_stream_channels(self._h, frame))
-        if out is None:
-            out = np.empty(shape, dtype=dtype)
-        elif out.shape != shape or out.dtype != np.dtype(dtype) or not out.flags.c_contiguous:
-            raise ValueError(f"out must be a C-contiguous {np.dtype(dtype)} array of shape {shape}")
-        self._check(self._L.jxlb_frame_write_to_buffer(self._h, frame, st, orientation, out.ctypes.data, out.nbytes))
+        spec = write_spec(LAYOUT_STREAM, dtype, orientation)
+        out, dst, nbytes = self._write_target(frame, spec, out, on_device=False)
+        self._check(self._L.jxlb_frame_write_to_buffer(self._h, frame, spec.sample_type, spec.orientation, dst, nbytes))
         return out
 
     def frame_to_torch(self, frame, dtype=np.uint8, orientation=0, out=None):
         """frame_to_buffer() with the packed (height, width, channels) samples left in HBM as a torch tensor on this
         decoder's GPU (jxlb_frame_write_to_device); torch only owns the memory."""
-        import torch
-        info = self.frame_info(frame)
-        orient = orientation or self.image_info().orientation
-        w, h = (info.height, info.width) if orient >= 5 else (info.width, info.height)
-        st = {np.dtype(np.uint8): 0, np.dtype(np.uint16): 1, np.dtype(np.float32): 2}[np.dtype(dtype)]
-        tdt = {0: torch.uint8, 1: torch.uint16, 2: torch.float32}[st]
-        shape = (h, w, self._L.jxlb_frame_stream_channels(self._h, frame))
-        if out is None:
-            out = torch.empty(shape, dtype=tdt, device=f"cuda:{self.device}")
-        if tuple(out.shape) != shape or out.dtype != tdt or not out.is_contiguous() or not out.is_cuda:
-            raise ValueError(f"out must be a contiguous CUDA {tdt} tensor of shape {shape}")
-        self._check(self._L.jxlb_frame_write_to_device(self._h, frame, st, orientation, out.data_ptr(), out.numel() * out.element_size()))
+        spec = write_spec(LAYOUT_STREAM, dtype, orientation)
+        out, dst, nbytes = self._write_target(frame, spec, out, on_device=True)
+        self._check(self._L.jxlb_frame_write_to_device(self._h, frame, spec.sample_type, spec.orientation, dst, nbytes))
         return out
 
     def frame_write_shape(self, frame, spec: WriteSpec):
@@ -395,25 +378,33 @@ class Decoder:
         shape = (n.value, h, w) if spec.layout == LAYOUT_ALL_PLANAR else (h, w, n.value)
         return shape, nbytes.value
 
+    def _write_target(self, frame, spec: WriteSpec, out, on_device):
+        """(out, pointer, nbytes) of a write of `frame` as `spec` asks: `out` checked against frame_write_shape(), or
+        allocated when None: a numpy array, or with on_device a torch tensor on this decoder's GPU."""
+        shape, nbytes = self.frame_write_shape(frame, spec)
+        if on_device:
+            import torch
+            tdt = {0: torch.uint8, 1: torch.uint16, 2: torch.float32}[spec.sample_type]
+            if out is None:
+                out = torch.empty(shape, dtype=tdt, device=f"cuda:{self.device}")
+            if tuple(out.shape) != shape or out.dtype != tdt or not out.is_contiguous() or not out.is_cuda:
+                raise ValueError(f"out must be a contiguous CUDA {tdt} tensor of shape {shape}")
+            return out, out.data_ptr(), nbytes
+        dtype = {0: np.uint8, 1: np.uint16, 2: np.float32}[spec.sample_type]
+        if out is None:
+            out = np.empty(shape, dtype=dtype)
+        if out.shape != shape or out.dtype != np.dtype(dtype) or not out.flags.c_contiguous:
+            raise ValueError(f"out must be a C-contiguous {np.dtype(dtype)} array of shape {shape}")
+        return out, out.ctypes.data, nbytes
+
     def frame_write(self, frame, layout=LAYOUT_STREAM, dtype=np.uint8, orientation=0, spot_colours=True, out=None):
         """One of the Render layouts (jxlb_frame_write_ex), packed on the device: `layout` as for write_spec(). Returns a
         numpy array, or fills `out`: a C-contiguous numpy array, or a contiguous torch CUDA tensor of this decoder's GPU
         (the samples then stay in HBM), of frame_write_shape()'s shape and `dtype`."""
         spec = write_spec(layout, dtype, orientation, spot_colours)
-        shape, nbytes = self.frame_write_shape(frame, spec)
-        if out is None:
-            out = np.empty(shape, dtype=dtype)
-        if hasattr(out, "data_ptr"):
-            import torch
-            tdt = {0: torch.uint8, 1: torch.uint16, 2: torch.float32}[spec.sample_type]
-            if tuple(out.shape) != shape or out.dtype != tdt or not out.is_contiguous() or not out.is_cuda:
-                raise ValueError(f"out must be a contiguous CUDA {tdt} tensor of shape {shape}")
-            dst, on_device = out.data_ptr(), 1
-        else:
-            if out.shape != shape or out.dtype != np.dtype(dtype) or not out.flags.c_contiguous:
-                raise ValueError(f"out must be a C-contiguous {np.dtype(dtype)} array of shape {shape}")
-            dst, on_device = out.ctypes.data, 0
-        self._check(self._L.jxlb_frame_write_ex(self._h, frame, ctypes.byref(spec), dst, nbytes, on_device))
+        on_device = hasattr(out, "data_ptr")
+        out, dst, nbytes = self._write_target(frame, spec, out, on_device)
+        self._check(self._L.jxlb_frame_write_ex(self._h, frame, ctypes.byref(spec), dst, nbytes, int(on_device)))
         return out
 
     def set_capture(self, on=True):

@@ -42,6 +42,18 @@ DevView raw_view(void* p, uint32_t w, uint32_t h, uint32_t stride) {
   return v;
 }
 
+// Queues the copy of plane `v` to host `dst`, whose rows are `dst_stride` floats apart: one linear copy when both sides
+// are contiguous, else a 2-D copy.
+void plane_to_host(jxlb_decoder* dec, const View& v, float* dst, size_t dst_stride) {
+  const DevView d = dec->be->dev_view(v);
+  const cudaError_t e =
+      d.stride == v.w && dst_stride == v.w
+          ? cudaMemcpyAsync(dst, d.ptr, size_t(v.w) * v.h * 4, cudaMemcpyDeviceToHost, dec->be->stream())
+          : cudaMemcpy2DAsync(dst, dst_stride * 4, d.ptr, size_t(d.stride) * 4, size_t(v.w) * 4, v.h, cudaMemcpyDeviceToHost,
+                              dec->be->stream());
+  JXLB_CHECK(e == cudaSuccess, kErrCuda, cudaGetErrorString(e));
+}
+
 }  // namespace
 
 namespace jxlb {
@@ -110,19 +122,12 @@ int32_t frame_planar_to_host(jxlb_decoder* dec, int32_t frame, float* dst, size_
   if (!dec || !dst || !dec->have_result || frame < 0 || size_t(frame) >= dec->res.frames.size()) return JXLB_ERR_INVALID_ARG;
   return guarded(dec, [&] {
     const DecodedFrame& f = dec->res.frames[frame];
-    size_t off = 0;
+    size_t off = 0;  // in floats
     for (const View& v : f.channels) {
-      const size_t bytes = size_t(v.w) * v.h * 4;
-      JXLB_CHECK(off + bytes <= dst_bytes, kErrInvalidArg, "destination buffer too small");
-      DevView d = dec->be->dev_view(v);
-      cudaError_t e;
-      if (d.stride == v.w)
-        e = cudaMemcpyAsync(reinterpret_cast<uint8_t*>(dst) + off, d.ptr, bytes, cudaMemcpyDeviceToHost, dec->be->stream());
-      else
-        e = cudaMemcpy2DAsync(reinterpret_cast<uint8_t*>(dst) + off, size_t(v.w) * 4, d.ptr, size_t(d.stride) * 4, size_t(v.w) * 4, v.h,
-                              cudaMemcpyDeviceToHost, dec->be->stream());
-      JXLB_CHECK(e == cudaSuccess, kErrCuda, cudaGetErrorString(e));
-      off += bytes;
+      const size_t n = size_t(v.w) * v.h;
+      JXLB_CHECK((off + n) * 4 <= dst_bytes, kErrInvalidArg, "destination buffer too small");
+      plane_to_host(dec, v, dst + off, v.w);
+      off += n;
     }
     dec->be->sync();
   });
@@ -414,76 +419,10 @@ int32_t jxlb_frame_channel_to_host(jxlb_decoder* dec, int32_t frame, int32_t cha
     JXLB_CHECK(channel >= 0 && size_t(channel) < f.channels.size(), kErrInvalidArg, "channel out of range");
     const View& v = f.channels[channel];
     JXLB_CHECK(dst_stride >= v.w, kErrInvalidArg, "dst_stride too small");
-    DevView d = dec->be->dev_view(v);
-    cudaError_t e;
-    if (d.stride == v.w && dst_stride == v.w)  // contiguous on both sides: one linear DMA
-      e = cudaMemcpyAsync(dst, d.ptr, size_t(v.w) * v.h * 4, cudaMemcpyDeviceToHost, dec->be->stream());
-    else
-      e = cudaMemcpy2DAsync(dst, dst_stride * 4, d.ptr, size_t(d.stride) * 4, size_t(v.w) * 4, v.h, cudaMemcpyDeviceToHost,
-                            dec->be->stream());
-    JXLB_CHECK(e == cudaSuccess, kErrCuda, cudaGetErrorString(e));
+    plane_to_host(dec, v, dst, dst_stride);
     dec->be->sync();
   });
 }
-
-namespace {
-int32_t write_frame(jxlb_decoder* dec, int32_t frame, int32_t sample_type, int32_t orientation, void* dst, size_t dst_bytes,
-                    bool dst_on_device);
-}
-
-int32_t jxlb_frame_write_to_buffer(jxlb_decoder* dec, int32_t frame, int32_t sample_type, int32_t orientation, void* dst,
-                                   size_t dst_bytes) {
-  return write_frame(dec, frame, sample_type, orientation, dst, dst_bytes, false);
-}
-
-int32_t jxlb_frame_write_to_device(jxlb_decoder* dec, int32_t frame, int32_t sample_type, int32_t orientation, void* device_dst,
-                                   size_t dst_bytes) {
-  return write_frame(dec, frame, sample_type, orientation, device_dst, dst_bytes, true);
-}
-
-namespace {
-int32_t write_frame(jxlb_decoder* dec, int32_t frame, int32_t sample_type, int32_t orientation, void* dst, size_t dst_bytes,
-                    bool dst_on_device) {
-  if (!dec || !dst || !dec->have_result || frame < 0 || size_t(frame) >= dec->res.frames.size()) return JXLB_ERR_INVALID_ARG;
-  return guarded(dec, [&] {
-    const DecodedFrame& f = dec->res.frames[frame];
-    JXLB_CHECK(sample_type >= 0 && sample_type <= 2, kErrInvalidArg, "sample_type must be 0 (u8), 1 (u16) or 2 (f32)");
-    JXLB_CHECK(!f.channels.empty(), kErrInvalidArg, "frame without channels");
-    const StreamLayout layout = stream_layout(dec->res.image_header, f);
-    JXLB_CHECK(layout.spots.size() <= 8, kErrUnsupported, "more than 8 spot colour channels");
-    const uint32_t orient = orientation == 0 ? dec->res.image_header.orientation : uint32_t(orientation);
-    JXLB_CHECK(orient >= 1 && orient <= 8, kErrInvalidArg, "orientation must be 1..8 (0 = the image's)");
-    DevPackParams p;
-    std::memset(&p, 0, sizeof(p));
-    p.num_channels = uint32_t(layout.channels.size());
-    p.width = f.channels[0].w;
-    p.height = f.channels[0].h;
-    for (size_t c = 0; c < layout.channels.size(); ++c) {
-      const View& v = f.channels[layout.channels[c]];
-      JXLB_CHECK(v.w == p.width && v.h == p.height, kErrUnsupported, "channels of different sizes");
-      DevView d = dec->be->dev_view(v);
-      p.planes[c] = static_cast<const float*>(d.ptr);
-      p.strides[c] = d.stride;
-    }
-    p.num_spots = uint32_t(layout.spots.size());
-    for (size_t s = 0; s < layout.spots.size(); ++s) {
-      const View& v = f.channels[layout.spots[s].channel];
-      JXLB_CHECK(v.w == p.width && v.h == p.height, kErrUnsupported, "channels of different sizes");
-      DevView d = dec->be->dev_view(v);
-      p.spot_planes[s] = static_cast<const float*>(d.ptr);
-      p.spot_strides[s] = d.stride;
-      for (int k = 0; k < 3; ++k) p.spot_rgb[s][k] = layout.spots[s].rgb[k];
-      p.spot_solidity[s] = layout.spots[s].solidity;
-    }
-    p.orientation = orient;
-    p.sample_type = uint32_t(sample_type);
-    const size_t bytes = size_t(p.width) * p.height * p.num_channels * (sample_type == 0 ? 1 : (sample_type == 1 ? 2 : 4));
-    JXLB_CHECK(dst_bytes >= bytes, kErrInvalidArg, "destination buffer too small");
-    if (dst_on_device) dec->be->pack_to_device(p, dst);
-    else dec->be->pack_to_host(p, dst, bytes);
-  });
-}
-}  // namespace
 
 static_assert(int(JXLB_LAYOUT_STREAM) == kWriteStream && int(JXLB_LAYOUT_STREAM_NO_ALPHA) == kWriteStreamNoAlpha &&
                   int(JXLB_LAYOUT_ALL_INTERLEAVED) == kWriteAllInterleaved && int(JXLB_LAYOUT_ALL_PLANAR) == kWriteAllPlanar,
@@ -534,6 +473,19 @@ int32_t jxlb_frame_write_ex(jxlb_decoder* dec, int32_t frame, const jxlb_write_s
     }
     dec->be->pack(p, channels, spots, dst, w.bytes, dst_on_device != 0);
   });
+}
+
+// ImageStream::write_to_buffer is the stream layout with spot colours mixed.
+int32_t jxlb_frame_write_to_buffer(jxlb_decoder* dec, int32_t frame, int32_t sample_type, int32_t orientation, void* dst,
+                                   size_t dst_bytes) {
+  const jxlb_write_spec spec{JXLB_LAYOUT_STREAM, sample_type, orientation, 1};
+  return jxlb_frame_write_ex(dec, frame, &spec, dst, dst_bytes, 0);
+}
+
+int32_t jxlb_frame_write_to_device(jxlb_decoder* dec, int32_t frame, int32_t sample_type, int32_t orientation, void* device_dst,
+                                   size_t dst_bytes) {
+  const jxlb_write_spec spec{JXLB_LAYOUT_STREAM, sample_type, orientation, 1};
+  return jxlb_frame_write_ex(dec, frame, &spec, device_dst, dst_bytes, 1);
 }
 
 int32_t jxlb_frame_stream_channels(const jxlb_decoder* dec, int32_t frame) {

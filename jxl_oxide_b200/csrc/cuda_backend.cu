@@ -1090,28 +1090,6 @@ void CudaBackend::add_noise_in_frame(const View v[3], uint32_t field_w, uint32_t
   for (int c = 0; c < 3; ++c) dfree(field[c]);
 }
 
-void CudaBackend::pack_to_host(const DevPackParams& p, void* dst, size_t bytes) {
-  void* d = dmalloc(bytes);
-  begin_k("pack_interleaved");
-  launch_pack_interleaved(p, d, S());
-  end_k();
-  CUDA_CHECK(cudaMemcpyAsync(dst, d, bytes, cudaMemcpyDeviceToHost, S()));
-  sync();
-  dfree(d);
-}
-
-void CudaBackend::pack_to_device(const DevPackParams& p, void* d_dst) {
-  cudaPointerAttributes attr;
-  if (cudaPointerGetAttributes(&attr, d_dst) != cudaSuccess || attr.type != cudaMemoryTypeDevice || attr.device != device_) {
-    cudaGetLastError();
-    fail(kErrInvalidArg, "destination is not device memory of this decoder's GPU");
-  }
-  begin_k("pack_interleaved");
-  launch_pack_interleaved(p, d_dst, S());
-  end_k();
-  sync();  // the caller may hand the buffer to any stream (NCCL's, torch's) afterwards
-}
-
 void CudaBackend::pack(const DevPackSpec& p, const std::vector<DevPackChannel>& channels, const std::vector<DevPackSpot>& spots,
                        void* dst, size_t bytes, bool dst_on_device) {
   if (dst_on_device) {
@@ -1121,11 +1099,15 @@ void CudaBackend::pack(const DevPackSpec& p, const std::vector<DevPackChannel>& 
       fail(kErrInvalidArg, "destination is not device memory of this decoder's GPU");
     }
   }
-  const auto* d_channels = static_cast<const DevPackChannel*>(upload_temp(channels.data(), channels.size() * sizeof(DevPackChannel)));
-  const auto* d_spots = spots.empty() ? nullptr : static_cast<const DevPackSpot*>(upload_temp(spots.data(), spots.size() * sizeof(DevPackSpot)));
+  const DevPackChannel* d_channels = nullptr;
+  const DevPackSpot* d_spots = nullptr;
+  if (channels.size() > kPackParamEntries || spots.size() > kPackParamEntries) {
+    d_channels = static_cast<const DevPackChannel*>(upload_temp(channels.data(), channels.size() * sizeof(DevPackChannel)));
+    if (!spots.empty()) d_spots = static_cast<const DevPackSpot*>(upload_temp(spots.data(), spots.size() * sizeof(DevPackSpot)));
+  }
   void* out = dst_on_device ? dst : dmalloc(bytes);
   begin_k("pack");
-  launch_pack(p, d_channels, d_spots, out, S());
+  launch_pack(p, channels.data(), spots.data(), d_channels, d_spots, out, S());
   end_k();
   if (!dst_on_device) CUDA_CHECK(cudaMemcpyAsync(dst, out, bytes, cudaMemcpyDeviceToHost, S()));
   sync();  // a device destination may go to any stream (NCCL's, torch's) afterwards

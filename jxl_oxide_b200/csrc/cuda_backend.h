@@ -138,12 +138,8 @@ class CudaBackend : public Backend, private TableSink {
   // launch accounting for bench.py ("gpu_launches")
   uint64_t launches = 0;
   // per-kernel device timing (CUDA events on the launching stream), for bench.py's roofline
-  // Interleave + convert on the device, then one linear copy to `dst` (host).
-  void pack_to_host(const DevPackParams& p, void* dst, size_t bytes);
-  // Same, straight into the caller's device buffer (no host copy): the packed frame stays in HBM for an NCCL gather.
-  void pack_to_device(const DevPackParams& p, void* d_dst);
-  // Any layout (launch_pack): the tables go up with the launch; `dst` is host memory of `bytes`, or device memory of this
-  // decoder's GPU. Returns after the samples are in `dst`.
+  // Any layout (launch_pack): the tables go with the launch; `dst` is host memory of `bytes`, or device memory of this
+  // decoder's GPU (the packed frame then stays in HBM, e.g. for an NCCL gather). Returns after the samples are in `dst`.
   void pack(const DevPackSpec& p, const std::vector<DevPackChannel>& channels, const std::vector<DevPackSpot>& spots, void* dst,
             size_t bytes, bool dst_on_device);
   bool fuse_filters = true;  // single-kernel Gaborish+EPF+colour (off: stage-by-stage, for stage parity tests)

@@ -185,44 +185,6 @@ __global__ void upsample_kernel(DevView in, DevView out, int k, const float* __r
   static_cast<float*>(out.ptr)[size_t(y) * out.stride + x] = r;
 }
 
-// One thread per output pixel; (x, y) are coordinates in the oriented output image
-// (fb.rs:387-401 to_original_coord, sample rules fb.rs:436-520).
-__global__ void pack_interleaved_kernel(DevPackParams p, void* out) {
-  const uint32_t ow = p.orientation >= 5 ? p.height : p.width, oh = p.orientation >= 5 ? p.width : p.height;
-  const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
-  if (x >= ow || y >= oh) return;
-  uint32_t sx, sy;
-  switch (p.orientation) {
-    case 2: sx = ow - x - 1, sy = y; break;
-    case 3: sx = ow - x - 1, sy = oh - y - 1; break;
-    case 4: sx = x, sy = oh - y - 1; break;
-    case 5: sx = y, sy = x; break;
-    case 6: sx = y, sy = ow - x - 1; break;
-    case 7: sx = oh - y - 1, sy = ow - x - 1; break;
-    case 8: sx = oh - y - 1, sy = x; break;
-    default: sx = x, sy = y; break;
-  }
-  const size_t o = (size_t(y) * ow + x) * p.num_channels;
-  for (uint32_t c = 0; c < p.num_channels; ++c) {
-    float v = p.planes[c][size_t(sy) * p.strides[c] + sx];
-    if (c < 3)
-      for (uint32_t s = 0; s < p.num_spots; ++s) {
-        const float mix = fmul(p.spot_planes[s][size_t(sy) * p.spot_strides[s] + sx], p.spot_solidity[s]);
-        v = fadd(fmul(p.spot_rgb[s][c], mix), fmul(v, fsub(1.0f, mix)));
-      }
-    if (p.sample_type == 2) {
-      static_cast<float*>(out)[o + c] = v;
-    } else {
-      const float hi = p.sample_type == 0 ? 255.0f : 65535.0f;
-      float t = fadd(fmul(v, hi), 0.5f);
-      t = t < 0.0f ? 0.0f : (t > hi ? hi : t);  // f32::clamp; NaN falls through and casts to 0
-      const uint32_t q = (t == t) ? uint32_t(t) : 0u;
-      if (p.sample_type == 0) static_cast<uint8_t*>(out)[o + c] = uint8_t(q);
-      else static_cast<uint16_t*>(out)[o + c] = uint16_t(q);
-    }
-  }
-}
-
 // ---------------------------------------------------------------------------------------------
 // Patches without alpha (blend.rs:550-606). Jobs of one launch may overlap in `dst` only if the bitstream
 // makes patches overlap; they are then applied in job order by launching overlapping batches separately
@@ -455,14 +417,6 @@ void launch_add_noise(const DevView v[3], float* const field[3], uint32_t field_
   dim3 block(32, 8);
   dim3 grid((v[0].w + 31) / 32, (v[0].h + 7) / 8);
   noise_apply_kernel<<<grid, block, 0, stream>>>(v[0], v[1], v[2], field[0], field[1], field[2], int(field_w), int(field_h), p);
-}
-
-void launch_pack_interleaved(DevPackParams p, void* out, cudaStream_t stream) {
-  if (!p.width || !p.height || !p.num_channels) return;
-  const uint32_t ow = p.orientation >= 5 ? p.height : p.width, oh = p.orientation >= 5 ? p.width : p.height;
-  dim3 block(32, 8);
-  dim3 grid((ow + 31) / 32, (oh + 7) / 8);
-  pack_interleaved_kernel<<<grid, block, 0, stream>>>(p, out);
 }
 
 void launch_upsample(DevView in, DevView out, int k, const float* quarter, cudaStream_t stream) {

@@ -237,27 +237,9 @@ void launch_ycbcr_to_rgb(DevView cb, DevView y, DevView cr, DevYcbcrParams p, cu
 void launch_copy_rect(DevView src, DevView dst, cudaStream_t stream);
 // One k-times upsampling pass (k = 2, 4, 8); `quarter`: (k/2)^2 kernels of 25 weights (device).
 void launch_upsample(DevView in, DevView out, int k, const float* quarter, cudaStream_t stream);
-// ImageStream::write_to_buffer (crates/jxl-oxide/src/fb.rs:309-410): interleave up to 8 f32 planes into
-// u8 / u16 / f32 samples (channel fastest), applying the image orientation (1..8).
-struct DevPackParams {
-  const float* planes[8];
-  uint32_t strides[8];
-  uint32_t num_channels;
-  uint32_t width, height;  // of the stored (un-oriented) planes
-  uint32_t orientation;    // 1..8
-  uint32_t sample_type;    // 0: u8, 1: u16, 2: f32
-  // spot colours mixed into channels 0..2 in list order (fb.rs:335-362): v = rgb[c] * mix + v * (1 - mix),
-  // mix = spot sample * solidity
-  uint32_t num_spots;
-  const float* spot_planes[8];
-  uint32_t spot_strides[8];
-  float spot_rgb[8][3];
-  float spot_solidity[8];
-};
-void launch_pack_interleaved(DevPackParams p, void* out, cudaStream_t stream);
 // Every output layout of a frame (pack.cu, per-sample rules in pack.cuh): any number of f32 planes, read through channel
-// and spot tables in device memory, to u8 / u16 / f32 samples interleaved (channel fastest) or planar (channel-major), with
-// the orientation applied.
+// and spot tables, to u8 / u16 / f32 samples interleaved (channel fastest) or planar (channel-major), with the orientation
+// applied.
 struct DevPackChannel {
   const float* plane;
   uint32_t stride;
@@ -275,7 +257,12 @@ struct DevPackSpec {
   uint32_t sample_type;    // 0: u8, 1: u16, 2: f32
   uint32_t planar;         // 0: interleaved, 1: one plane per channel
 };
-void launch_pack(const DevPackSpec& p, const DevPackChannel* channels, const DevPackSpot* spots, void* out, cudaStream_t stream);
+// `channels` and `spots` are host tables of p.num_channels and p.num_spots entries. Up to kPackParamEntries of each go to
+// the kernel by value; when either table is longer, the kernel reads `d_channels` and `d_spots`, their copies in device
+// memory, instead (null otherwise).
+constexpr uint32_t kPackParamEntries = 8;
+void launch_pack(const DevPackSpec& p, const DevPackChannel* channels, const DevPackSpot* spots, const DevPackChannel* d_channels,
+                 const DevPackSpot* d_spots, void* out, cudaStream_t stream);
 // Rectangle blending (jxl-render/src/blend.rs:550-727), one CTA per job; modes 1 Replace, 2 Add, 3 Mul,
 // 4 Blend, 5 MulAdd, 6 MixAlpha.
 struct DevPatchJob {

@@ -1,11 +1,15 @@
 // Frame packer: the stored f32 planes of a decoded frame -> the sample buffers the reference's Render hands out
 // (ImageStream::write_to_buffer, Render::image_all_channels, Render::image_planar; crates/jxl-oxide/src/{lib.rs,fb.rs}).
-// The per-sample rules are in pack.cuh; this file only decides which thread handles which sample.
+// The per-sample rules are in pack.cuh; this file only decides which thread handles which sample and where the channel
+// and spot tables are read from.
 //
 // A CTA of 32 x 8 threads packs a 32 x 32 tile of output samples. For orientations 1..4 an output row is a stored row
 // (possibly mirrored), so a warp reads one stored row segment per channel, and each thread writes all channels of its
 // sample. For 5..8 an output row is a stored column: a warp would read 32 different rows. The tile then goes through
 // shared memory one channel at a time: the warps read stored rows into it and write output rows out of it, both coalesced.
+//
+// Tables of up to kPackParamEntries entries travel in the kernel's parameter block, so that every plane pointer and stride
+// is a constant-bank load; longer tables are read from device memory.
 #include "kernels.h"
 #include "pack.cuh"
 
@@ -15,9 +19,20 @@ namespace {
 
 constexpr uint32_t kTile = 32, kRows = 8;
 
-__global__ void __launch_bounds__(kTile* kRows) pack_kernel(DevPackSpec p, const DevPackChannel* __restrict__ channels,
-                                                           const DevPackSpot* __restrict__ spots, void* out) {
+struct PackParams {
+  DevPackSpec spec;
+  const DevPackChannel* d_channels;  // device tables, read when the tables do not fit below
+  const DevPackSpot* d_spots;
+  DevPackChannel channels[kPackParamEntries];
+  DevPackSpot spots[kPackParamEntries];
+};
+
+template <bool kTablesInParams>
+__global__ void __launch_bounds__(kTile* kRows) pack_kernel(const __grid_constant__ PackParams params, void* out) {
   __shared__ float tile[kTile][kTile + 1];
+  const DevPackSpec& p = params.spec;
+  const DevPackChannel* __restrict__ channels = kTablesInParams ? params.channels : params.d_channels;
+  const DevPackSpot* __restrict__ spots = kTablesInParams ? params.spots : params.d_spots;
   const uint32_t ow = p.orientation >= 5 ? p.height : p.width, oh = p.orientation >= 5 ? p.width : p.height;
   const uint32_t ox0 = blockIdx.x * kTile, oy0 = blockIdx.y * kTile;
   const uint32_t tx = threadIdx.x, ty = threadIdx.y;
@@ -52,11 +67,22 @@ __global__ void __launch_bounds__(kTile* kRows) pack_kernel(DevPackSpec p, const
 
 }  // namespace
 
-void launch_pack(const DevPackSpec& p, const DevPackChannel* channels, const DevPackSpot* spots, void* out, cudaStream_t stream) {
+void launch_pack(const DevPackSpec& p, const DevPackChannel* channels, const DevPackSpot* spots, const DevPackChannel* d_channels,
+                 const DevPackSpot* d_spots, void* out, cudaStream_t stream) {
   if (!p.width || !p.height || !p.num_channels) return;
   const uint32_t ow = p.orientation >= 5 ? p.height : p.width, oh = p.orientation >= 5 ? p.width : p.height;
   const dim3 grid((ow + kTile - 1) / kTile, (oh + kTile - 1) / kTile);
-  pack_kernel<<<grid, dim3(kTile, kRows), 0, stream>>>(p, channels, spots, out);
+  PackParams params = {};
+  params.spec = p;
+  params.d_channels = d_channels;
+  params.d_spots = d_spots;
+  if (p.num_channels <= kPackParamEntries && p.num_spots <= kPackParamEntries) {
+    for (uint32_t c = 0; c < p.num_channels; ++c) params.channels[c] = channels[c];
+    for (uint32_t s = 0; s < p.num_spots; ++s) params.spots[s] = spots[s];
+    pack_kernel<true><<<grid, dim3(kTile, kRows), 0, stream>>>(params, out);
+  } else {
+    pack_kernel<false><<<grid, dim3(kTile, kRows), 0, stream>>>(params, out);
+  }
 }
 
 }  // namespace jxlb

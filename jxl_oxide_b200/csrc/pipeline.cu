@@ -42,14 +42,17 @@ struct KeyframeSubmission {
   FrameIndex index;
 };
 
+// What a job delivers: nothing (out_mode 0), the stored planes as planar f32 (out_mode 1), or a write as `spec` asks
+// (jxlb_pipeline_submit_ex, and out_mode 2..5, which are stream writes).
+enum class Output { kNone, kPlanar, kSpec };
+
 struct Job {
   std::shared_ptr<const KeyframeSubmission> keyframes;  // a segment task of a keyframe submission
   size_t segment = 0;
   const uint8_t* data = nullptr;  // host bytes (caller keeps them alive until the job is reported done) or
   size_t size = 0;
   int32_t slot = -1;              // a preloaded slot
-  int32_t out_mode = 0;
-  bool has_spec = false;  // jxlb_pipeline_submit_ex: `spec` replaces out_mode
+  Output output = Output::kNone;
   jxlb_write_spec spec{};
   bool dst_on_device = false;
   void* dst = nullptr;
@@ -554,31 +557,24 @@ struct jxlb_pipeline {
     cv_done.notify_all();
   }
 
-  // Packs frame 0 of `dec` as the job's spec or, without one, its `out_mode` asks into `dst` (NULL: a buffer of the ring)
-  // and records in `d` where it went.
+  // Writes frame 0 of `dec` as the job asks into `dst` (NULL: a buffer of the ring) and records in `d` where it went.
   int32_t deliver(jxlb_decoder* dec, const Job& job, void* dst, size_t dst_bytes, Done& d) {
-    const jxlb_write_spec* spec = job.has_spec ? &job.spec : nullptr;
-    const int32_t out_mode = job.out_mode;
     int32_t rc = JXLB_OK;
     const bool own = !dst;
-    if (spec ? job.dst_on_device : (out_mode == 4 || out_mode == 5)) {
+    if (job.output == Output::kSpec && job.dst_on_device) {
       // packed straight into the caller's device buffer (input of an NCCL gather): no host link involved
-      rc = spec ? jxlb_frame_write_ex(dec, 0, spec, dst, dst_bytes, 1) : jxlb_frame_write_to_device(dec, 0, out_mode - 4, 0, dst, dst_bytes);
+      rc = jxlb_frame_write_ex(dec, 0, &job.spec, dst, dst_bytes, 1);
       d.out = dst;
       d.out_bytes = dst_bytes;
-    } else if (spec || out_mode != 0) {
+    } else if (job.output != Output::kNone) {
       if (!dst) {  // library-owned pinned staging, sized from the decoded frame
-        jxlb_frame_info fi;
-        jxlb_frame_get_info(dec, 0, &fi);
-        if (spec) {
+        if (job.output == Output::kSpec) {
           uint64_t bytes = 0;
-          rc = jxlb_frame_write_size(dec, 0, spec, nullptr, &bytes);
+          rc = jxlb_frame_write_size(dec, 0, &job.spec, nullptr, &bytes);
           dst_bytes = size_t(bytes);
-        } else if (out_mode == 1) {
+        } else {
           dst_bytes = 0;
           for (const View& v : dec->res.frames[0].channels) dst_bytes += size_t(v.w) * v.h * 4;
-        } else {
-          dst_bytes = size_t(fi.width) * fi.height * size_t(jxlb_frame_stream_channels(dec, 0)) * (out_mode == 2 ? 1 : 2);
         }
         if (rc != JXLB_OK) return rc;
         dst = acquire_host(dst_bytes);
@@ -594,9 +590,8 @@ struct jxlb_pipeline {
         rc = jxlb_sync(dec);
         std::lock_guard<std::mutex> copy_lock(copy_mu);
         if (rc != JXLB_OK) {
-        } else if (spec) rc = jxlb_frame_write_ex(dec, 0, spec, dst, dst_bytes, 0);
-        else if (out_mode == 1) rc = frame_planar_to_host(dec, 0, static_cast<float*>(dst), dst_bytes);
-        else rc = jxlb_frame_write_to_buffer(dec, 0, out_mode - 2, 0, dst, dst_bytes);
+        } else if (job.output == Output::kSpec) rc = jxlb_frame_write_ex(dec, 0, &job.spec, dst, dst_bytes, 0);
+        else rc = frame_planar_to_host(dec, 0, static_cast<float*>(dst), dst_bytes);
         d.out = dst;
         d.out_bytes = dst_bytes;
         if (rc != JXLB_OK && own) {
@@ -725,7 +720,7 @@ int32_t jxlb_pipeline_preload(jxlb_pipeline* p, int32_t slot, const uint8_t* dat
 }  // extern "C"
 
 namespace {
-// Queues one frame; `out` carries the output fields of the Job (out_mode or spec, destination).
+// Queues one frame; `out` carries the output fields of the Job (what to deliver, destination).
 int32_t submit_frame(jxlb_pipeline* p, const uint8_t* data, size_t size, int32_t slot, const Job& out) {
   Job j = out;
   j.data = data;
@@ -782,20 +777,22 @@ int32_t submit_keyframes(jxlb_pipeline* p, const uint8_t* data, size_t size, int
   return JXLB_OK;
 }
 
-Job mode_output(int32_t out_mode, void* dst, size_t dst_bytes, uint64_t tag) {
+Job spec_output(const jxlb_write_spec& spec, void* dst, size_t dst_bytes, int32_t dst_on_device, uint64_t tag) {
   Job j;
-  j.out_mode = out_mode;
+  j.output = Output::kSpec;
+  j.spec = spec;
+  j.dst_on_device = dst_on_device != 0;
   j.dst = dst;
   j.dst_bytes = dst_bytes;
   j.tag = tag;
   return j;
 }
 
-Job spec_output(const jxlb_write_spec& spec, void* dst, size_t dst_bytes, int32_t dst_on_device, uint64_t tag) {
+// out_mode 2 / 3 are ImageStream::write_to_buffer::<u8 / u16> to host memory, 4 / 5 the same to device memory.
+Job mode_output(int32_t out_mode, void* dst, size_t dst_bytes, uint64_t tag) {
+  if (out_mode >= 2) return spec_output(jxlb_write_spec{JXLB_LAYOUT_STREAM, out_mode % 2, 0, 1}, dst, dst_bytes, out_mode >= 4, tag);
   Job j;
-  j.has_spec = true;
-  j.spec = spec;
-  j.dst_on_device = dst_on_device != 0;
+  j.output = out_mode == 1 ? Output::kPlanar : Output::kNone;
   j.dst = dst;
   j.dst_bytes = dst_bytes;
   j.tag = tag;

@@ -1,7 +1,8 @@
 """Times the frame packer (kernels/pack.cu, jxlb_frame_write_ex) on an 8K frame resident in HBM, per layout, sample type
 and orientation, and reports the bytes it moves per second against the H100 SXM's 3.35 TB/s HBM3 (data-sheet figure).
 Kernel times come from CUDA events around each launch (Decoder.set_profile); the destination is a torch tensor in HBM, so
-no host copy is timed. jxlb_frame_write_to_device's interleaving kernel is timed beside it on the same frame.
+no host copy is timed. The stream entry point that predates the write specs (jxlb_frame_write_to_device, through
+Decoder.frame_to_torch) runs the same kernel and is timed beside it on the same frame.
 
     python tools/pack_probe.py [--reps 20] [--json out.json]
 """
@@ -71,19 +72,18 @@ def main():
             ms = kernel_ms(dec, "pack", lambda: dec.frame_write(0, layout, dtype, orientation, out=out), args.reps)
             read_planes = nc + (spots if layout.startswith("stream") else 0)
             moved = W * H * read_planes * 4 + nbytes
-            results.append(dict(kernel="pack", layout=layout, dtype=np.dtype(dtype).name, orientation=orientation, channels=nc,
+            results.append(dict(kernel="pack", entry="frame_write", layout=layout, dtype=np.dtype(dtype).name, orientation=orientation, channels=nc,
                                 ms=round(ms, 4), bytes=moved, gb_s=round(moved / ms / 1e6, 1),
                                 hbm_share=round(moved / (ms / 1e3) / HBM_BYTES_PER_S, 3)))
             print(json.dumps(results[-1]), flush=True)
     for dtype in (np.uint8, np.uint16):
         for orientation in (1, 6):
             out = dec.frame_to_torch(0, dtype=dtype, orientation=orientation)
-            ms = kernel_ms(dec, "pack_interleaved", lambda: dec.frame_to_torch(0, dtype=dtype, orientation=orientation, out=out),
-                           args.reps)
+            ms = kernel_ms(dec, "pack", lambda: dec.frame_to_torch(0, dtype=dtype, orientation=orientation, out=out), args.reps)
             nc = out.shape[2]
             moved = W * H * (nc + spots) * 4 + out.numel() * out.element_size()
-            results.append(dict(kernel="pack_interleaved", layout="stream", dtype=np.dtype(dtype).name, orientation=orientation,
-                                channels=nc, ms=round(ms, 4), bytes=moved, gb_s=round(moved / ms / 1e6, 1),
+            results.append(dict(kernel="pack", entry="frame_to_torch", layout="stream", dtype=np.dtype(dtype).name,
+                                orientation=orientation, channels=nc, ms=round(ms, 4), bytes=moved, gb_s=round(moved / ms / 1e6, 1),
                                 hbm_share=round(moved / (ms / 1e3) / HBM_BYTES_PER_S, 3)))
             print(json.dumps(results[-1]), flush=True)
     report = dict(gpu=gpu_name_and_power_limit(), frame=[W, H], channels=info.num_channels, results=results)
